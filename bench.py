@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native ScaViSLAM BA hot path.
+"""bench.py -- headline benchmark of the H100-native ScaViSLAM BA hot path.
 
 Metric (BASELINE.json): Gauss-Newton/LM iterations per second on the 200-keyframe /
 20k-landmark synthetic double window (config C2), 10 iterations per step.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one svs_ba_optimize(num_iters=10) over the whole window, starting from the same
 initial state (svs_ba_reset_state, device-to-device).  `value` counts iterations with the
@@ -19,6 +19,8 @@ g2o path; the reference itself cannot be built here, see DESIGN.md) on the host 
 from __future__ import annotations
 
 import argparse
+import contextlib
+import ctypes
 import json
 import os
 import sys
@@ -39,12 +41,12 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
     """Samples SM clock / throttle reasons through NVML while the timed regions run.  NVML is initialised in the
-    constructor (round 1 initialised it inside the thread and the 80 ms region was over before the first sample)."""
+    constructor (initialised inside the thread, a short timed region can be over before the first sample)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -185,7 +187,7 @@ def run_ours(args):
     pb = sdist.window_for_rank(rank)
     ba = capi.BundleAdjuster(device=local)
     ba.set_problem(pb)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")   # > 50 MB L2
 
     def barrier():
         torch.cuda.synchronize()
@@ -223,6 +225,8 @@ def run_ours(args):
             agg[k] += st[k]
     barrier()
     wall = time.perf_counter() - wall0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ba, st)
 
     # end to end through the reference-facing call with host buffers
     e2e_iters = 0
@@ -306,25 +310,20 @@ def run_ours(args):
 
     if rank == 0:
         peak, peak_src = load_peaks()
-        traffic = {}
-        tp = os.path.join(ROOT, "profiles", "kernel_traffic.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f)
 
-        def roof(kernel, key, nbytes, ms_kernel, note):
+        def roof(kernel, nbytes, ms_kernel, note):
             k_ms = ms_kernel / max(trials, 1)
             ach = nbytes / (k_ms * 1e-3) / 1e9
             return {"bound": "hbm", "kernel": kernel, "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                    "traffic": traffic.get(key), "peak_source": peak_src, "algorithmic_bytes_per_launch": nbytes,
+                    "traffic": None, "peak_source": peak_src, "algorithmic_bytes_per_launch": nbytes,
                     "avg_launch_ms": k_ms, "share_of_step": ms_kernel / ms, "note": note}
 
         roofs = {
-            "k_solve": roof("k_solve (block-sparse Cholesky + forward/backward solve, 2-CTA cluster)", "k_solve",
+            "k_solve": roof("k_solve (block-sparse Cholesky + forward/backward solve, cluster of two CTAs)",
                             solve_kernel_bytes(st, pb), agg["ms_solve"],
                             "a dependent chain of P/2 + w block pivots per CTA: bounded by instruction latency, neither "
                             "HBM nor tensor throughput applies (DESIGN.md 4)"),
-            "k_build": roof("k_build_wave (fused linearise + J^T W J + Schur elimination)", "k_build_wave",
+            "k_build": roof("k_build_wave (fused linearise + J^T W J + Schur elimination)",
                             schur_kernel_bytes(st, pb), agg["ms_build"],
                             "the kernel north_star names for HBM utilisation; FP64 issue/latency-bound at this window "
                             "size: 25 MB per launch, L2-resident between iterations (DESIGN.md 4)"),
@@ -383,6 +382,30 @@ def run_ours(args):
 
 
 
+def dump_outputs(out_dir, ba, st):
+    """What a caller of the timed path receives after its last step: the optimised poses [P][7] and inverse-depth
+    points psi [L][3] of the window and the per-iteration chi2 of that call, all float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in (("poses", ba.poses()), ("psi", ba.points()), ("chi2_iter", np.asarray(st["chi2_iter"]))):
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, np.float64))
+
+
+@contextlib.contextmanager
+def c_stdout_to_stderr():
+    """Points file descriptor 1 at stderr for the duration, for what native libraries print with printf."""
+    libc = ctypes.CDLL(None)
+    sys.stdout.flush()
+    libc.fflush(None)
+    saved = os.dup(1)
+    os.dup2(2, 1)
+    try:
+        yield
+    finally:
+        libc.fflush(None)
+        os.dup2(saved, 1)
+        os.close(saved)
+
+
 def c5_sharded_block(args, torch, dist, rank, world, local, flush):
     """BASELINE config C5: ONE 1000-keyframe / 100k-landmark window whose landmarks are split over all ranks
     (SURVEY.md 8e), driven inside the library: per Levenberg trial one ncclAllReduce of S|bp|bc, a replicated solve
@@ -392,13 +415,14 @@ def c5_sharded_block(args, torch, dist, rank, world, local, flush):
     try:
         pb5 = synth.make_config("C5")
         ba5 = capi.BundleAdjuster(device=local)
-        if rank == 0:
-            uid = torch.tensor(list(capi.comm_unique_id()), dtype=torch.uint8, device="cuda")
-        else:
-            uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
-        if dist is not None:
-            dist.broadcast(uid, src=0)
-        ba5.comm_init(world, rank, bytes(uid.cpu().numpy().tobytes()))
+        with c_stdout_to_stderr():    # NCCL prints its version banner there; stdout is the one JSON line
+            if rank == 0:
+                uid = torch.tensor(list(capi.comm_unique_id()), dtype=torch.uint8, device="cuda")
+            else:
+                uid = torch.zeros(128, dtype=torch.uint8, device="cuda")
+            if dist is not None:
+                dist.broadcast(uid, src=0)
+            ba5.comm_init(world, rank, bytes(uid.cpu().numpy().tobytes()))
         ba5.set_problem_sharded(pb5)
         steps = max(3, args.steps // 4)
         ms, iters, agg = 0.0, 0, {"ms_build": 0.0, "ms_solve": 0.0, "ms_update": 0.0, "ms_control": 0.0}
@@ -593,7 +617,14 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--frames", type=int, default=200, help="frames of the synthetic C3 sequence (0: skip the front-end part)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="--impl ours only: after the timed steps, write the poses, psi and chi2 trace of the last "
+                         "step as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs applies to the project's own path (--impl ours) only")
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs --steps >= 1: it saves what the last timed step computed")
     if args.impl == "reference":
         run_reference(args)
     else:

@@ -1,5 +1,5 @@
 /*
- * svs_b200.h -- C ABI of libsvsb200.so: B200-native (sm_100a) implementation of
+ * svs_b200.h -- C ABI of libsvsb200.so: H100-native (sm_90a) implementation of
  * ScaViSLAM's double-window bundle-adjustment iteration and dense stereo
  * front-end kernels.  Plain pointers and sizes only; no C++ or torch types.
  *

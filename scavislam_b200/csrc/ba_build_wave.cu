@@ -8,9 +8,8 @@
 //     keeps every lane busy where one-warp-per-landmark leaves 3/4 of them idle;
 //   * the Schur products Y_m B_n^T (and the direct J^T W J terms) are accumulated over all
 //     landmarks of the task in registers -- each lane owns up to 7 (pair, row) units of 6 doubles --
-//     and flushed with ONE set of RED.F64 per task instead of one per landmark
-//     (measured on B200: 450 G coalesced FP64 reductions/s, scripts/ubench/lat.cu -- the
-//     per-landmark scatter alone would cost 39 us on the 200-keyframe window).
+//     and flushed with ONE set of RED.F64 per task instead of one per landmark (the FP64
+//     reduction rate, scripts/ubench/lat.cu, would make a per-landmark scatter a large share of a launch).
 //
 // Reference semantics: G2oEdgeProjectPSI2UVU::linearizeOplus (anchored_points.cpp:168-189), g2o
 // BaseMultiEdge::constructQuadraticForm, BlockSolver<6,3>::buildSystem / solve (Schur part).
@@ -60,9 +59,8 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
     return __shfl_sync(0xffffffffu, t, 0);
   };
   const double lambda = ctl->lambda;
-  // (Drawing the next ticket early was measured, profiles/r02_build_spill_prefetch_ab.txt: when a task starts, the
-  //  atomic's round trip is hidden but a reserved task waits for its owner while other warps run dry at the end of
-  //  the list -- 0.105 instead of 0.082 ms on the 200-keyframe window; before the flush: no difference.)
+  // (Drawing the next ticket early, when a task starts, hides the atomic's round trip, but a reserved task waits for
+  //  its owner while other warps run dry at the end of the list; it was slower and is not done.)
   for (int task = persist ? next_task() : (int)blockIdx.x * kWvWarps + warp; task < d.ntasks;
        task = persist ? next_task() : d.ntasks) {
   double* sm = reinterpret_cast<double*>(smem_raw) + (size_t)warp * kWvDoubles;
@@ -223,8 +221,8 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
       for (int c = 0; c < 3; ++c) Y[c] = b0 * Di[c] + b1 * Di[3 + c] + b2 * Di[6 + c];
     }
     {
-      // (ncu source view, round 2: written as a double loop over (c, sg) with the address formed per element this
-      //  spill was the hottest line of the kernel -- 16 % of the stall samples, 9 % of the instructions.  A wave has at
+      // (written as a double loop over (c, sg) with the address formed per element, this spill was the hottest source
+      //  line of the kernel in a profiler capture.  A wave has at
       //  most 40 slots: two per lane, one pointer bumped by nslots per component, the 18 values of a slot read with
       //  16-byte shared-memory loads)
       const bool v0 = lane < nslots_w, v1 = lane + 32 < nslots_w;
@@ -372,7 +370,7 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
 // The same kernel with a TEAM of two warps per task: the 32 edge lanes of a wave are warp 0's, every later phase is
 // spread over the 64 lanes, and each lane accumulates at most 4 (pair, row) units instead of 7 -- 24 accumulator
 // registers instead of 42, so that the kernel fits 128 registers and sixteen warps per SM are resident instead of
-// eight (round 1's ncu capture: 255 registers, 10 % of the warp slots active, issue slots 24 % busy).
+// eight (the one-warp kernel uses 255 registers).
 constexpr int kWvTeams = 4;                 // teams per CTA, two warps each; a team owns what a warp owned before
 __device__ __forceinline__ void team_sync(int team) { asm volatile("bar.sync %0, 64;" ::"r"(team + 1) : "memory"); }
 
@@ -688,10 +686,9 @@ static int build_wave_resident_ctas() {
 void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st) {
   if (d.ntasks == 0 && d.C == 0) return;
   static const int prof = getenv("SVS_BUILD_TIMING") ? 1 : 0;
-  // A/B switch.  Measured on B200 (C2 / C5, per 10 launches): one warp per task 1.20 / 7.08 ms, a team of two warps
-  // per task 1.66 / 8.98 ms -- the team halves the accumulators (128 registers, sixteen warps per SM instead of
-  // eight) but pays for it with 1.1 KB of spills, five named barriers per wave and an idle second warp while the
-  // 32 edge lanes linearise; the one-warp kernel stays the default
+  // A/B switch: a team of two warps per task halves the accumulators (128 registers, sixteen warps per SM instead of
+  // eight) but pays for it with spills, five named barriers per wave and an idle second warp while the 32 edge lanes
+  // linearise; the one-warp kernel stays the default
   static const int one_warp = getenv("SVS_BUILD_WAVE2") ? 0 : 1;
   // the opt-in above 48 KB of dynamic shared memory is per device: handles may live on several GPUs of one process
   if (one_warp) {

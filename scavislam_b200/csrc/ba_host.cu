@@ -599,7 +599,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
     if (out_of_range.load()) return fail(h, SVS_ERR_INVALID, "observation edge index out of range");
     // prefix over (landmark, thread).  Only the prefix over the L landmark totals is serial; the totals and the
     // per-thread start offsets are computed on the pool over landmark ranges (the flat double loop was nt x L serial
-    // steps and grew with the thread count: measured 0.26 ms of the grouping phase at 8 threads, 0.50 at 24)
+    // steps and grew with the thread count)
     if (nt == 1) {
       int run = 0;
       for (int l = 0; l < L; ++l) { int& c = cnt[l]; const int n = c; eptr[l] = run; c = run; run += n; }
@@ -759,11 +759,11 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   std::vector<int> task_lm, task_cnt, gen_lm, long_lm;   // long_lm: more than kMaxTrack slots (streaming kernel, any length)
   int Kmax_gen = 1;
   {
-    // landmarks per task.  Measured on B200 with the persistent grid (1 184 resident warps), build kernel per trial on
-    // the 200-keyframe window / with 20 % drop-outs: chunk 8: 0.100 / 0.116 ms, 12: 0.095 / 0.113, 16: 0.097 / 0.110,
-    // 20: 0.108 / 0.113, 24: 0.125 / 0.127, 32: 0.156 / 0.159 (fewer flushes against a coarser tail); the
-    // 1 000-keyframe window is flat from 32 up
-    int chunk = L / (148 * 11);
+    // landmarks per task: about eleven tasks per SM, so that the persistent grid's tail stays short while coarser
+    // tasks flush their accumulators less often; clamped to [4, 32]
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    int chunk = L / (std::max(sms, 1) * 11);
     chunk = chunk < 4 ? 4 : (chunk > 32 ? 32 : chunk);
     if (const char* cs = getenv("SVS_BUILD_CHUNK")) chunk = atoi(cs);   // tuning knob
     if (getenv("SVS_BUILD_V1")) chunk = 0;   // A/B switch: everything through the one-warp-per-landmark kernel

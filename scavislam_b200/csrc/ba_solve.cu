@@ -6,8 +6,7 @@
 // The factor is a latency chain of P block columns.  What bounds it is not HBM and not the tensor
 // cores (6x6 blocks, FP64) but the dependent-instruction latency of the pivot chain
 //     chol(D_j) -> L_{j+1,j} = S_{j+1,j} L_jj^-T -> D_{j+1} -= L_{j+1,j} L_{j+1,j}^T -> chol(D_{j+1}) ...
-// (about 850 cycles per block column on B200: 6 x [rsqrt + 2 Newton, multiply, fma] + the cross-block
-// hand-over), so the kernel is organised around keeping that chain free of everything else:
+// (per block column: 6 x [rsqrt + 2 Newton, multiply, fma] + the cross-block hand-over), so the kernel is organised around keeping that chain free of everything else:
 //   * window-shaped pose graphs are factored from both ends at once ("twisted" / two-ended
 //     elimination, ba_host.cu::choose_branches): each end is one CTA of a 2-CTA cluster with its own
 //     SM (schedulers, shared-memory pipe, 227 KB), so the chain is P/2 + w columns long;
@@ -42,15 +41,14 @@ namespace svs {
 
 constexpr int kSolveThreads = 384;               // 12 warps; warp w issues from scheduler w % 4
 // Roles (factor_range).  Eight working warps, two per scheduler (warps 8-11 idle through the factorisation): what bounds
-// the helpers is the number of instructions their schedulers must issue per column (ncu: with sixteen resident warps
-// that all walked the column loop, 3 300 warp-instructions per column on three schedulers) and the FP64 pipe of a
-// scheduler (54 DFMAs of a quarter unit take 2 cycles each: two unit warps on one scheduler doubled the FMA phase).
-// Measured alternatives (C2 / C5 solve time per 10 iterations):
-//   this layout (unit warps 1-4, one per scheduler, warp 4 next to the chain)            1.40 / 6.6 ms
-//   fourth unit warp on warp 11 (scheduler 3, next to a unit warp and the urgent warp)   1.46 / 6.8 ms
-//   round-2 first layout (unit warps 1, 2, 3, 5; row warps 6, 9; chain alone)            1.64 / 7.8 ms
-//   three unit warps, left-over units on the urgent warp                                 1.65 / 7.9 ms
-//   three unit warps, left-over units on the second row warp                             1.93 / 9.2 ms
+// the helpers is the number of instructions their schedulers must issue per column (sixteen resident warps that all
+// walked the column loop spent most of their issue slots on loop skeletons) and the FP64 pipe of a scheduler (two
+// unit warps on one scheduler double the FMA phase).  Alternatives that were tried, fastest first:
+//   this layout (unit warps 1-4, one per scheduler, warp 4 next to the chain)
+//   fourth unit warp on warp 11 (scheduler 3, next to a unit warp and the urgent warp)
+//   an earlier layout (unit warps 1, 2, 3, 5; row warps 6, 9; chain alone)
+//   three unit warps, left-over units on the urgent warp
+//   three unit warps, left-over units on the second row warp
 constexpr int kChainWarp = 0;
 constexpr int kUnitWarps = 4;                    // warps 1-4: quarter-block units of the trailing update
 constexpr int kRowWarps = 2;                     // warps 5, 6: rows of the column, N rows, right-hand side
@@ -265,8 +263,8 @@ __device__ __forceinline__ void ring_refill(const BaDev& d, const Team& T, const
 //                          c+1 it waits for the URGENT updates of column c-1 (kBarUrg, sync);
 //   urgent warp (warp 15)  after "column j published": scales the first two blocks of the column, (j+1, j) and
 //                          (j+2, j) in a window, and applies the two pair updates the chain is going to read next
-//                          -- D_{j+2} and S_{j+2,j+1} -- then signals (kBarUrg, arrive);  ~550 cycles, well inside
-//                          the chain's ~960;
+//                          -- D_{j+2} and S_{j+2,j+1} -- then signals (kBarUrg, arrive); less work than the
+//                          chain's own column;
 //   general helpers        everything else of column j: the other rows (L_ij), the other pair updates, the
 //                          right-hand side, N_ij for the backward pass.  They re-join the chain only through kBarPub, one
 //                          column later; since every helper must arrive there, "column j published" also means

@@ -1,4 +1,4 @@
-// dt.cu -- dense photometric SE3 tracker on sm_100a (ScaViSLAM GPU-path semantics).
+// dt.cu -- dense photometric SE3 tracker on sm_90a (ScaViSLAM GPU-path semantics).
 //   scavislam/gpu/dense_tracking.cu:82-148   pointcloud_kernel / computePointCloud
 //   scavislam/gpu/dense_tracking.cu:172-356  jacobianReduction_kernel + host-side final sum
 //   scavislam/gpu/dense_tracking.cu:376-491  chi2_kernel + host-side final sum

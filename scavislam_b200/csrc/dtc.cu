@@ -1,6 +1,6 @@
 // dtc.cu -- the dense tracker the reference builds WITHOUT SCAVISLAM_CUDA_SUPPORT (SURVEY.md 8 row a18):
 // DenseTracker::denseTrackingCpu / computeDensePointCloudCpu (scavislam/dense_tracking.cpp:222-423),
-// on sm_100a.  Semantics that differ from the CUDA build of the reference (dt.cu follows that one):
+// on sm_90a.  Semantics that differ from the CUDA build of the reference (dt.cu follows that one):
 // every 4th pixel in u and v (EVERY_NTH_PIXEL, dense_tracking.h:82), the previous intensity comes from
 // the uint8 pyramid, residual clamped to +-0.1, exact software bilinear taps (interpolateMat_32f,
 // maths_utils.cpp:46-65), FP64 point transform and Jacobian, border test isInFrame(uv, 2), the

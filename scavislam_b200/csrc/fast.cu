@@ -1,4 +1,4 @@
-// fast.cu -- grid FAST-9/16 detector on sm_100a, bit-exact with cv::FastFeatureDetector(thr, false)
+// fast.cu -- grid FAST-9/16 detector on sm_90a, bit-exact with cv::FastFeatureDetector(thr, false)
 // run per grid cell as ScaViSLAM does (scavislam/fast_grid.cpp:60-83 FastGrid::detect,
 // :86-152 FastGrid::detectAdaptively).
 //

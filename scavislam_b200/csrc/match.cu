@@ -1,4 +1,4 @@
-// match.cu -- guided patch matcher on sm_100a: GuidedMatcher<StereoCamera>::match
+// match.cu -- guided patch matcher on sm_90a: GuidedMatcher<StereoCamera>::match
 // (scavislam/matcher.cpp:312-398) with computePrediction (:98-142), warpAffinve (:403-458),
 // computePatchScores (:77-96), matchCandidates / matchPatchZeroMeanSSD (:42-74, :144-181),
 // returnBestMatch (:183-216) and createObervation (matcher-impl.cpp:32-51).

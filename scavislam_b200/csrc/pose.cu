@@ -1,4 +1,4 @@
-// pose.cu -- motion-only Levenberg-Marquardt on sm_100a (SURVEY.md 8f rank 1, a "next" row):
+// pose.cu -- motion-only Levenberg-Marquardt on sm_90a (SURVEY.md 8f rank 1, a "next" row):
 // PoseOptimizer<SE3,6,IdObs<3>,3>::calcFastMotionOnly (scavislam/pose_optimizer.h:135-298) with
 // SE3XYZ_STEREO (transformations.h:414-460), called after guided matching by
 // StereoFrontend::matchAndTrack (stereo_frontend.cpp:1058) and Backend::globalLoopClosure
@@ -276,8 +276,7 @@ __global__ void __launch_bounds__(kThreads) k_pose_lm(PoseArgs a, PoseCtl* ctl) 
 
 
 // ---------------------------------------------------------------- the same LM loop on a thread-block cluster
-// The sweep is instruction-bound on one SM (ncu: 38 k warp-instructions per pass for 1 800 observations -- five IEEE
-// divisions, two square roots and a 27-term accumulation per observation, kept operation for operation for parity).
+// The sweep is instruction-bound on one SM (five IEEE divisions, two square roots and a 27-term accumulation per observation, kept operation for operation for parity).
 // For more than kClusterMinObs observations the loop therefore runs on a cluster of kCl CTAs, each with its own SM:
 // every CTA sweeps its share and reduces it in shared memory; after a cluster barrier CTA 0 adds the kCl partial
 // results in rank order through distributed shared memory, its thread 0 takes the Levenberg decision (the code of

@@ -1,4 +1,4 @@
-// prep.cu -- per-frame image preprocessing on sm_100a (SURVEY.md 8f rank 2, a "next" row):
+// prep.cu -- per-frame image preprocessing on sm_90a (SURVEY.md 8f rank 2, a "next" row):
 // FrameGrabber::preprocessing (scavislam/frame_grabber.cpp:287-336):
 //   cv::buildPyramid(uint8)                       -> k_pyrdown_u8   (5x5 [1 4 6 4 1]/16, (s + 128) >> 8, reflect-101)
 //   gpu_uint8.convertTo(CV_32F, 1/255)            -> k_u8_to_f32

@@ -1,4 +1,4 @@
-// Named-barrier hand-over latency on sm_100a.  NW producer warps + one consumer warp.  The LAST producer (it spins a
+// Named-barrier hand-over latency on sm_90a.  NW producer warps + one consumer warp.  The LAST producer (it spins a
 // little first) stamps the clock, optionally issues a memory operation, and then arrives (bar.arrive or bar.sync); the
 // consumer bar.syncs and stamps behind a dependent shared-memory read.  Printed: cycles stamp -> stamp.
 #include <cstdio>

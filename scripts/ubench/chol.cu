@@ -1,5 +1,5 @@
 // Latency of the 6x6 pivot-chain variants of k_solve, one warp alone on an SM (cycles per call).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/chol chol.cu && /tmp/chol
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o chol chol.cu && ./chol
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,4 +1,4 @@
-// FP64 tensor-core rate on B200: mma.sync.m8n8k4.f64 with 8 independent accumulator tiles per warp,
+// FP64 tensor-core rate: mma.sync.m8n8k4.f64 with 8 independent accumulator tiles per warp,
 // nw warps on one sub-partition (warps 0,4,8,12) or spread over the four sub-partitions (warps 0..nw-1);
 // compare with the same warps issuing DFMAs (256 FMAs per DMMA = 8 warp-wide DFMAs).
 #include <cstdio>

@@ -1,5 +1,5 @@
-// Micro-benchmarks that size the design: dependent-issue latency of FP64 ops on B200 (sm_100a),
-// FP64 throughput per SM, RED.F64 throughput.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 lat.cu -o lat
+// Micro-benchmarks that size the design: dependent-issue latency of FP64 ops (sm_90a),
+// FP64 throughput per SM, RED.F64 throughput.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 lat.cu -o lat
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -73,18 +73,20 @@ int main() {
          h[0] / 2048.0, h[1] / 2048.0, h[2] / 2048.0, h[3] / 256.0, h[4] / 256.0, h[5] / 512.0);
   cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   const int iters = 4096;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (int warps = 4; warps <= 32; warps *= 2) {
-    k_tput<<<148, warps * 32>>>(out, 1.0000001, 0.9999999, iters);
-    cudaEventRecord(e0); k_tput<<<148, warps * 32>>>(out, 1.0000001, 0.9999999, iters); cudaEventRecord(e1);
+    k_tput<<<sms, warps * 32>>>(out, 1.0000001, 0.9999999, iters);
+    cudaEventRecord(e0); k_tput<<<sms, warps * 32>>>(out, 1.0000001, 0.9999999, iters); cudaEventRecord(e1);
     cudaEventSynchronize(e1); float ms; cudaEventElapsedTime(&ms, e0, e1);
-    printf("FP64 FMA throughput, 148 CTAs x %2d warps, 8 indep chains: %.2f TFLOP/s\n", warps, 2.0 * 8 * iters * 148.0 * warps * 32 / (ms * 1e-3) / 1e12);
+    printf("FP64 FMA throughput, %d CTAs x %2d warps, 8 indep chains: %.2f TFLOP/s\n", sms, warps, 2.0 * 8 * iters * (double)sms * warps * 32 / (ms * 1e-3) / 1e12);
   }
   for (int stride = 1; stride <= 64; stride *= 8) {
     const int n = 1 << 21;
-    k_red<<<148 * 8, 256>>>(out, n, 64, stride);
-    cudaEventRecord(e0); k_red<<<148 * 8, 256>>>(out, n, 64, stride); cudaEventRecord(e1);
+    k_red<<<sms * 8, 256>>>(out, n, 64, stride);
+    cudaEventRecord(e0); k_red<<<sms * 8, 256>>>(out, n, 64, stride); cudaEventRecord(e1);
     cudaEventSynchronize(e1); float ms; cudaEventElapsedTime(&ms, e0, e1);
-    printf("RED.F64 lane stride %2d doubles over 16 MB: %.1f G atomics/s\n", stride, 148.0 * 8 * 256 * 64 / (ms * 1e-3) / 1e9);
+    printf("RED.F64 lane stride %2d doubles over 16 MB: %.1f G atomics/s\n", stride, (double)sms * 8 * 256 * 64 / (ms * 1e-3) / 1e9);
   }
   printf("%s\n", cudaGetErrorString(cudaDeviceSynchronize()));
   return 0;

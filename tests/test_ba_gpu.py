@@ -30,9 +30,9 @@ def ba(svs):
     b.close()
 
 
-def test_device_is_blackwell(svs):
+def test_device_is_hopper(svs):
     info = svs.device_info()
-    assert "sm_100" in info, info
+    assert "sm_90" in info, info
 
 
 def test_chi2_matches_oracle(ba, oracle, c1):

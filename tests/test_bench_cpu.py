@@ -33,6 +33,13 @@ def test_reference_arm_other_ranks_are_silent():
     assert r.returncode == 0 and r.stdout.strip() == ""
 
 
+def test_dump_outputs_is_refused_where_it_cannot_apply(tmp_path):
+    for args in (["--impl", "reference", "--steps", "1"], ["--steps", "0"]):
+        r = _run(args + ["--dump-outputs", str(tmp_path / "d")])
+        assert r.returncode == 2 and "--dump-outputs" in r.stderr, (args, r.stderr)
+        assert not (tmp_path / "d").exists()
+
+
 def test_product_arm_needs_a_gpu():
     import torch
     if torch.cuda.is_available():
