@@ -105,8 +105,8 @@ struct svs_ba {
   int Kmax = 1;
   int Kmax_gen = 1;
   int nnzb_S = 0;
-  int C_edges = 0;
-  int max_col_blocks = 0, max_col_branch = 0, nbranch = 1, nsep_blk = 0, max_row_blocks = 0;
+  int nbranch = 1, nsep_blk = 0;
+  int solve_col_branch = 0, solve_col_sep = 0;   // launch_solve's column widths, resolved by set_problem
   std::vector<int> extra_pairs;   // svs_ba_set_structure: pose pairs added to the block pattern
   bool extra_pairs_from_caller = false;   // set by svs_ba_set_structure (not by the in-library sharded window)
   // one window sharded by landmarks across ranks (SURVEY.md 8e): NCCL communicator of this handle
@@ -123,7 +123,7 @@ struct svs_ba {
   std::vector<unsigned long long> w_key;
   std::vector<double> w_psi;
   std::vector<int> w_edge_src;
-  cudaEvent_t ev[8] = {};
+  cudaEvent_t ev[2] = {};   // start and end of optimize()'s trials (svs_ba_stats::ms_total)
   // structure of the last problem (index arrays as the caller passed them): a call with the same structure --
   // the second optimize() of a back-end tick (backend.cpp:186-197), repeated measurement -- skips the structure
   // analysis and re-sends only the numbers
@@ -137,7 +137,6 @@ struct svs_ba {
   Symbolic k_sy; std::vector<unsigned char> k_adj; int k_adjP = -1, k_nbranch = 1, k_nsep = 0, k_nnzb = 0; bool k_natural = false;
   int symbolic_hits = 0;
   std::vector<cudaEvent_t> tev;   // per-trial timing events
-  // last optimize() settings
 };
 
 namespace {
@@ -193,22 +192,22 @@ int dev_upload(svs_ba* h, const T** p, const T* src, size_t n) {
 template <typename T>
 int dev_upload(svs_ba* h, const T** p, const std::vector<T>& v) { return dev_upload(h, p, v.data(), v.size()); }
 
-int arena_reserve(svs_ba* h, size_t total, size_t upload) {
-  if (total > h->arena_cap) {
-    if (h->arena) cudaFree(h->arena);
-    h->arena = nullptr; h->arena_cap = 0;
-    const size_t want = total + total / 4;
-    CK(cudaMalloc((void**)&h->arena, want));
-    h->arena_cap = want;
-  }
-  if (upload > h->stage_cap) {
-    if (h->stage) cudaFreeHost(h->stage);
-    h->stage = nullptr; h->stage_cap = 0;
-    const size_t want = upload + upload / 4;
-    CK(cudaMallocHost((void**)&h->stage, want));
-    h->stage_cap = want;
-  }
-  return SVS_OK;
+// Grows a device buffer and/or its pinned host twin (either may be null; both share `cap`) to hold at least n
+// elements, with 25 % headroom so that a slowly growing window does not reallocate on every call.  The contents
+// are not kept.  Only the buffers passed in are touched.
+template <typename T>
+cudaError_t grow(size_t n, size_t* cap, T** dev, T** pinned = nullptr) {
+  if (n <= *cap) return cudaSuccess;
+  if (dev && *dev) cudaFree(*dev);
+  if (pinned && *pinned) cudaFreeHost(*pinned);
+  if (dev) *dev = nullptr;
+  if (pinned) *pinned = nullptr;
+  *cap = 0;
+  const size_t want = n + n / 4;
+  cudaError_t e = dev ? cudaMalloc((void**)dev, want * sizeof(T)) : cudaSuccess;
+  if (e == cudaSuccess && pinned) e = cudaMallocHost((void**)pinned, want * sizeof(T));
+  if (e == cudaSuccess) *cap = want;
+  return e;
 }
 
 void free_problem(svs_ba* h) {
@@ -392,6 +391,34 @@ int fail(svs_ba* h, int code, const std::string& msg) {
   return code;
 }
 
+// Entry points that work on the problem on the device: SVS_ERR_INVALID for a null handle, SVS_ERR_STATE before
+// a successful set_problem.
+int need_problem(svs_ba* h) {
+  if (!h) return SVS_ERR_INVALID;
+  return h->has_problem ? SVS_OK : fail(h, SVS_ERR_STATE, "no problem set");
+}
+
+// Reads the device's control block into h->h_ctl (waits for the stream).
+int read_ctl(svs_ba* h) {
+  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return SVS_OK;
+}
+
+void solve(svs_ba* h) { launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream); }
+
+// The fields of svs_ba_stats that the control block and the problem's shape give (not the timings).
+void fill_stats(const svs_ba* h, svs_ba_stats* st) {
+  const LmCtl& c = *h->h_ctl;
+  st->iterations = c.iter; st->trials_total = c.trials_total; st->chi2_init = c.chi_init; st->chi2_final = c.chi_cur;
+  st->lambda_final = c.lambda;
+  for (int i = 0; i < c.iter && i < SVS_BA_MAX_ITERS; ++i) {
+    st->chi2_iter[i] = c.chi_iter[i]; st->lambda_iter[i] = c.lambda_iter[i]; st->trials_iter[i] = c.trials_iter[i];
+  }
+  st->num_frames = h->d.P; st->num_points = h->d.L; st->num_point_edges = h->d.E_user; st->num_frame_edges = h->d.C;
+  st->nnzb_S = h->nnzb_S; st->nnzb_L = h->d.nblk; st->max_track = h->Kmax;
+}
+
 }  // namespace
 
 extern "C" {
@@ -456,6 +483,20 @@ void svs_ba_destroy(svs_ba* h) {
 
 const char* svs_last_error(const svs_ba* h) { return h ? h->err.c_str() : "null handle"; }
 
+// The end of both set_problem paths: upload the staged bytes from `from` on, gather the observations into the
+// internal order, clear the counters (and, on a new structure, the debug block) and the constraint chi2, and reset
+// the state to the initial values.
+static int finish_problem(svs_ba* h, size_t from, const double* d_obs_info, bool clear_dbg) {
+  BaDev& d = h->d;
+  CK(cudaMemcpyAsync(h->arena + from, h->stage + from, h->upload_bytes - from, cudaMemcpyHostToDevice, h->stream));
+  launch_regroup(d, d_obs_info ? d_obs_info : h->d_raw, h->stream);   // [3][E] internal order <- [E][3] user order
+  CK(cudaMemsetAsync(d.ticket, 0, 4 * sizeof(unsigned), h->stream));   // k_update's ticket, k_build_wave's task counter pair
+  if (clear_dbg) CK(cudaMemsetAsync(d.dbg, 0, 160 * sizeof(long long), h->stream));
+  CK(cudaMemsetAsync(d.chi_c, 0, std::max(d.C, 1) * sizeof(double), h->stream));
+  CK(cudaMemsetAsync(d.chi_c_new, 0, std::max(d.C, 1) * sizeof(double), h->stream));
+  return svs_ba_reset_state(h);
+}
+
 // d_obs_info != nullptr: the observations [E][3] followed by the weights [E][3] already lie on this device in
 // the caller's edge order (assembled there, svs_ba_set_problem_from_map) and e_obs / e_info are not read.
 static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi,
@@ -512,20 +553,13 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
         const double* src = psi + 3 * (size_t)h->lm_to_user[li];
         sp[3 * (size_t)li] = src[0]; sp[3 * (size_t)li + 1] = src[1]; sp[3 * (size_t)li + 2] = src[2];
       }
-      CK(cudaMemcpyAsync(h->arena + h->off_num, h->stage + h->off_num, h->upload_bytes - h->off_num, cudaMemcpyHostToDevice,
-                         h->stream));
-      launch_regroup(d, d_obs_info ? d_obs_info : h->d_raw, h->stream);
-      CK(cudaMemsetAsync(d.ticket, 0, 4 * sizeof(unsigned), h->stream));   // k_update's ticket, k_build_wave's task counter pair
-      CK(cudaMemsetAsync(d.chi_c, 0, std::max(C, 1) * sizeof(double), h->stream));
-      CK(cudaMemsetAsync(d.chi_c_new, 0, std::max(C, 1) * sizeof(double), h->stream));
       ++h->reuse_hits;
       if (host_timing) fprintf(stderr, "set_problem: structure reused (%d)\n", h->reuse_hits);
-      return svs_ba_reset_state(h);
+      return finish_problem(h, h->off_num, d_obs_info, false);
     }
   }
   free_problem(h);
   const int nthr = h->host_threads;
-  (void)nthr;
   auto tp0 = std::chrono::steady_clock::now();
   auto lap = [&](const char* what) {
     if (!host_timing) return;
@@ -538,18 +572,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   //      pinned memory and enqueues the DMA (observations, then weights) while this thread analyses the structure; a
   //      gather kernel brings them into the internal order afterwards.  The helper also keeps the copy of the index
   //      arrays that the same-structure test of the next call compares against.
-  if (E > 0 && !d_obs_info) {
-    const size_t need = 6 * (size_t)E;
-    if (need > h->raw_cap) {
-      if (h->d_raw) cudaFree(h->d_raw);
-      if (h->h_raw) cudaFreeHost(h->h_raw);
-      h->d_raw = h->h_raw = nullptr; h->raw_cap = 0;
-      const size_t want = need + need / 4;
-      CK(cudaMalloc((void**)&h->d_raw, want * sizeof(double)));
-      CK(cudaMallocHost((void**)&h->h_raw, want * sizeof(double)));
-      h->raw_cap = want;
-    }
-  }
+  if (E > 0 && !d_obs_info) CK(grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
   struct Side {   // (every return below waits for the helper: it reads the caller's arrays)
     Worker* w;
     cudaError_t err = cudaSuccess;
@@ -949,32 +972,25 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   h->measuring = true;
   lay();
   h->measuring = false;
-  int rc;
-  if ((rc = arena_reserve(h, h->arena_off, upload_bytes))) return rc;
+  CK(grow(h->arena_off, &h->arena_cap, &h->arena));
+  CK(grow<char>(upload_bytes, &h->stage_cap, nullptr, &h->stage));
   lay();
   lap("stage");
   h->worker.wait();   // its DMA is in the stream ahead of everything enqueued below
   if (side.err != cudaSuccess) return fail(h, SVS_ERR_CUDA, cudaGetErrorString(side.err));
   h->d_pose0 = const_cast<double*>(d_pose0c);
   h->d_psi0 = const_cast<double*>(d_psi0c);
-  CK(cudaMemcpyAsync(h->arena, h->stage, upload_bytes, cudaMemcpyHostToDevice, h->stream));
   d.e_obs = d.e_obs_w; d.e_w = d.e_w_w;
-  launch_regroup(d, d_obs_info ? d_obs_info : h->d_raw, h->stream);   // [3][E] internal order <- [E][3] user order
-  CK(cudaMemsetAsync(d.ticket, 0, 4 * sizeof(unsigned), h->stream));   // k_update's ticket, k_build_wave's task counter pair
-  CK(cudaMemsetAsync(d.dbg, 0, 160 * sizeof(long long), h->stream));
-  h->max_col_blocks = sy.max_col_sep; h->max_col_branch = sy.max_col_branch; h->max_row_blocks = sy.max_row;
+  h->solve_col_branch = sy.max_col_branch; h->solve_col_sep = std::max(sy.max_col_sep, sy.max_row - 2);
   d.nbranch = h->nbranch;
-  CK(cudaMemsetAsync(d.chi_c, 0, std::max(C, 1) * sizeof(double), h->stream));
-  CK(cudaMemsetAsync(d.chi_c_new, 0, std::max(C, 1) * sizeof(double), h->stream));
   h->Kmax = Kmax;
   h->Kmax_gen = Kmax_gen;
   d.ntasks = (int)task_lm.size(); d.ngen = (int)gen_lm.size(); d.nlong = (int)long_lm.size();
-  h->C_edges = C;
   h->has_problem = true;
   h->k_P = P; h->k_L = L; h->k_E = E; h->k_C = C; h->k_flags = h->flags; h->k_extra = h->extra_pairs;
   h->k_ci.assign(c_i, c_i + C); h->k_cj.assign(c_j, c_j + C);
   h->k_fixed = fx;
-  return svs_ba_reset_state(h);
+  return finish_problem(h, 0, d_obs_info, true);
 }
 
 int svs_ba_set_problem(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi,
@@ -988,7 +1004,7 @@ int svs_ba_set_problem(svs_ba* h, int P, const double* T_qt, const unsigned char
 }
 
 int svs_ba_reset_state(svs_ba* h) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   BaDev& d = h->d;
   CK(cudaMemcpyAsync(d.pose[0], h->d_pose0, 7 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
@@ -1010,30 +1026,17 @@ static int clear_system(svs_ba* h) {
   return SVS_OK;
 }
 
-int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, double lambda_init, int max_trials,
+// svs_ba_optimize for a handle with a non-empty problem: SVS_OK after the last trial, else an SVS error code.
+static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, double lambda_init, int max_trials,
                     svs_ba_stats* st) {
-  svs::NvtxRange nvtx_("optimize");
-  if (!h) return -100 + SVS_ERR_INVALID;
-  if (!h->has_problem) { h->err = "no problem set"; return -100 + SVS_ERR_STATE; }
-  if (st) memset(st, 0, sizeof *st);
   BaDev& d = h->d;
-  if (d.P == 0) return -1;   // g2o: "0 vertices to optimize"
   cudaSetDevice(h->device);
   int rc;
   int trials_seen = 0;
-#define CKO(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return -100 + SVS_ERR_CUDA;                                       \
-    }                                                                   \
-  } while (0)
   // LM state is not carried across calls (slam_graph.cpp:338-342, SURVEY B3); the accepted
   // state stays where the previous call (or set_problem) left it.
   if (h->cur_known < 0) {   // someone else may have flipped the state buffers: ask the device
-    CKO(cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-    CKO(cudaStreamSynchronize(h->stream));
+    if ((rc = read_ctl(h))) return rc;
     h->cur_known = h->h_ctl->cur;
   }
   {
@@ -1042,22 +1045,22 @@ int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     LmCtl z{};
     z.cur = cur; z.lambda = lambda_init; z.ni = 2; z.max_trials = max_trials; z.max_iters = num_iters;
     *h->h_ctl = z;
-    CKO(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   }
-  if ((rc = clear_system(h))) return -100 + rc;
+  if ((rc = clear_system(h))) return rc;
   float ms[4] = {0, 0, 0, 0};  // build, solve, update(+decision), collectives
   int launches = 0;
-  CKO(cudaEventRecord(h->ev[0], h->stream));
+  CK(cudaEventRecord(h->ev[0], h->stream));
   int it = 0;
   const NcclApi* nc = h->comm ? nccl_api() : nullptr;   // sharded window: sums across ranks on this stream
-  if (h->comm && !nc) { h->err = "NCCL library not loadable"; return -100 + SVS_ERR_STATE; }
+  if (h->comm && !nc) return fail(h, SVS_ERR_STATE, "NCCL library not loadable");
   const int per_trial = 2 + ((d.ntasks > 0 || d.C > 0) ? 1 : 0) + (d.ngen > 0 ? 1 : 0) + (d.nlong > 0 ? 1 : 0) + (nc ? 1 : 0);
 #define CKN(call)                                                       \
   do {                                                                  \
     const int e_ = (call);                                              \
     if (e_ != 0) {                                                      \
       h->err = std::string(#call) + ": " + nc->GetErrorString(e_);      \
-      return -100 + SVS_ERR_CUDA;                                       \
+      return SVS_ERR_CUDA;                                              \
     }                                                                   \
   } while (0)
   constexpr int kEv = 6;   // events per trial: start | built | summed | solved | updated | decided
@@ -1069,30 +1072,30 @@ int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     const int ntr = num_iters - it;
     while ((int)h->tev.size() < kEv * ntr) { cudaEvent_t e; cudaEventCreate(&e); h->tev.push_back(e); }
     for (int k = 0; k < ntr; ++k) {
-      CKO(cudaEventRecord(h->tev[kEv * k + 0], h->stream));
+      CK(cudaEventRecord(h->tev[kEv * k + 0], h->stream));
       launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
-      CKO(cudaEventRecord(h->tev[kEv * k + 1], h->stream));
+      CK(cudaEventRecord(h->tev[kEv * k + 1], h->stream));
       // every rank holds the partial reduced system of its landmarks: ONE all-reduce of S | bp | bc
       if (nc) CKN(nc->AllReduce(d.S, d.S, h->sys_count, kNcclFloat64, kNcclSum, h->comm, h->stream));
-      CKO(cudaEventRecord(h->tev[kEv * k + 2], h->stream));
-      launch_solve(d, h->max_col_branch, std::max(h->max_col_blocks, h->max_row_blocks - 2), h->nsep_blk, h->stream);
-      CKO(cudaEventRecord(h->tev[kEv * k + 3], h->stream));
+      CK(cudaEventRecord(h->tev[kEv * k + 2], h->stream));
+      solve(h);
+      CK(cudaEventRecord(h->tev[kEv * k + 3], h->stream));
       launch_update(d, robust, huber_delta, nc ? 1 : 0, h->stream);
-      CKO(cudaEventRecord(h->tev[kEv * k + 4], h->stream));
+      CK(cudaEventRecord(h->tev[kEv * k + 4], h->stream));
       if (nc) {   // chi2 (accepted, trial) and the gain-ratio denominator of this rank's landmarks -> the same decision everywhere
         CKN(nc->AllReduce(d.totals, d.totals, 3, kNcclFloat64, kNcclSum, h->comm, h->stream));
         launch_decide_deferred(d, h->stream);
       }
-      CKO(cudaEventRecord(h->tev[kEv * k + 5], h->stream));
+      CK(cudaEventRecord(h->tev[kEv * k + 5], h->stream));
     }
-    CKO(cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
     if (h->export_next) {   // one-call API: the accepted state rides back with the control block, in the caller's order
       const size_t n = 7 * (size_t)d.P + 3 * (size_t)d.L;
       launch_export(d, h->d_out, h->stream);
-      CKO(cudaMemcpyAsync(h->h_out, h->d_out, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+      CK(cudaMemcpyAsync(h->h_out, h->d_out, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     }
-    CKO(cudaStreamSynchronize(h->stream));
-    CKO(cudaGetLastError());
+    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaGetLastError());
     const int done_trials = h->h_ctl->trials_total - trials_seen;
     trials_seen = h->h_ctl->trials_total;
     launches += per_trial * done_trials;
@@ -1107,24 +1110,12 @@ int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     it = h->h_ctl->iter;
     if (it >= num_iters || (h->h_ctl->stop && !h->h_ctl->again)) break;
   }
-  CKO(cudaEventRecord(h->ev[6], h->stream));
-  CKO(cudaEventSynchronize(h->ev[6]));
+  CK(cudaEventRecord(h->ev[1], h->stream));
+  CK(cudaEventSynchronize(h->ev[1]));
   h->cur_known = h->h_ctl->cur;   // read back after the last trial of this call
   if (st) {
-    const LmCtl& c = *h->h_ctl;
-    st->iterations = c.iter;
-    st->trials_total = c.trials_total;
-    st->chi2_init = c.chi_init;
-    st->chi2_final = c.chi_cur;
-    st->lambda_final = c.lambda;
-    for (int i = 0; i < c.iter && i < SVS_BA_MAX_ITERS; ++i) {
-      st->chi2_iter[i] = c.chi_iter[i];
-      st->lambda_iter[i] = c.lambda_iter[i];
-      st->trials_iter[i] = c.trials_iter[i];
-    }
-    st->num_frames = d.P; st->num_points = d.L; st->num_point_edges = d.E_user; st->num_frame_edges = d.C;
-    st->nnzb_S = h->nnzb_S; st->nnzb_L = d.nblk; st->max_track = h->Kmax;
-    cudaEventElapsedTime(&st->ms_total, h->ev[0], h->ev[6]);
+    fill_stats(h, st);
+    cudaEventElapsedTime(&st->ms_total, h->ev[0], h->ev[1]);
     st->ms_build = ms[0]; st->ms_solve = ms[1]; st->ms_update = ms[2]; st->ms_control = ms[3];
     st->launches = launches;
   }
@@ -1163,37 +1154,37 @@ int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
               q[0], q[1], q[2], q[3], q[4], q[5], q[6], q[8], q[9], q[10], q[11], q[12], q[13], q[14]);
     }
   }
-  return h->h_ctl->iter;
+  return SVS_OK;
 #undef CKN
-#undef CKO
 }
 
-static int current_buffer(svs_ba* h, int* cur) {
-  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  *cur = h->h_ctl->cur;
-  return SVS_OK;
+int svs_ba_optimize(svs_ba* h, int num_iters, int robust, double huber_delta, double lambda_init, int max_trials,
+                    svs_ba_stats* st) {
+  svs::NvtxRange nvtx_("optimize");
+  if (int rc = need_problem(h)) return -100 + rc;
+  if (st) memset(st, 0, sizeof *st);
+  if (h->d.P == 0) return -1;   // g2o: "0 vertices to optimize"
+  const int rc = optimize(h, num_iters, robust, huber_delta, lambda_init, max_trials, st);
+  return rc ? -100 + rc : h->h_ctl->iter;
 }
 
 int svs_ba_get_poses(svs_ba* h, double* T_qt) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
-  int cur, rc;
-  if ((rc = current_buffer(h, &cur))) return rc;
+  if (int rc = read_ctl(h)) return rc;
   if (h->d.P)
-    CK(cudaMemcpyAsync(T_qt, h->d.pose[cur], 7 * (size_t)h->d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(T_qt, h->d.pose[h->h_ctl->cur], 7 * (size_t)h->d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
 int svs_ba_get_points(svs_ba* h, double* psi) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
-  int cur, rc;
-  if ((rc = current_buffer(h, &cur))) return rc;
+  if (int rc = read_ctl(h)) return rc;
   const int L = h->d.L;
   std::vector<double> tmp(3 * (size_t)L);
-  if (L) CK(cudaMemcpyAsync(tmp.data(), h->d.psi[cur], 3 * (size_t)L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (L) CK(cudaMemcpyAsync(tmp.data(), h->d.psi[h->h_ctl->cur],3 * (size_t)L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   // a sharded window (svs_ba_set_problem_sharded) addresses the caller's full-size array: only this rank's entries are written
   const size_t mul = h->L_full ? (size_t)h->comm_size : 1, add = h->L_full ? (size_t)h->comm_rank : 0;
@@ -1212,15 +1203,8 @@ int svs_optimiseInnerAndOuterWindow(svs_ba* h, int P, double* T_qt, const unsign
   if (rc) return -100 + rc;
   // the optimised state comes back in ONE copy behind the last trial (no separate read-out round trips)
   const size_t n = 7 * (size_t)P + 3 * (size_t)L;
-  if (n > h->out_cap) {
-    if (h->d_out) cudaFree(h->d_out);
-    if (h->h_out) cudaFreeHost(h->h_out);
-    h->d_out = h->h_out = nullptr; h->out_cap = 0;
-    if (cudaMalloc((void**)&h->d_out, (n + n / 4) * sizeof(double)) != cudaSuccess ||
-        cudaMallocHost((void**)&h->h_out, (n + n / 4) * sizeof(double)) != cudaSuccess)
-      return -100 + fail(h, SVS_ERR_CUDA, "out of memory for the read-out buffer");
-    h->out_cap = n + n / 4;
-  }
+  if (grow(n, &h->out_cap, &h->d_out, &h->h_out) != cudaSuccess)
+    return -100 + fail(h, SVS_ERR_CUDA, "out of memory for the read-out buffer");
   h->export_next = n > 0 && h->L_full == 0;
   // lambda0 = 50, 5 trials: slam_graph.cpp:338, :1073
   const int it = svs_ba_optimize(h, num_iters, robust, huber_delta, 50., 5, stats);
@@ -1238,7 +1222,7 @@ int svs_optimiseInnerAndOuterWindow(svs_ba* h, int P, double* T_qt, const unsign
 }
 
 int svs_ba_chi2(svs_ba* h, int robust, double huber_delta, double* chi2) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   BaDev& d = h->d;
   launch_chi2(d, robust, huber_delta, h->stream);
@@ -1255,8 +1239,7 @@ int svs_ba_chi2(svs_ba* h, int robust, double huber_delta, double* chi2) {
 }
 
 static int set_lambda(svs_ba* h, double lambda) {
-  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = read_ctl(h)) return rc;
   h->h_ctl->lambda = lambda;
   h->h_ctl->max_iters = 0;   // inspection hooks run the kernels unconditionally
   CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
@@ -1265,7 +1248,7 @@ static int set_lambda(svs_ba* h, double lambda) {
 
 int svs_ba_reduced_system(svs_ba* h, int robust, double huber_delta, double lambda, double* Sd, double* bs,
                           double* chi2) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   BaDev& d = h->d;
   int rc;
@@ -1313,17 +1296,16 @@ int svs_ba_reduced_system(svs_ba* h, int robust, double huber_delta, double lamb
 }
 
 int svs_ba_solve_reduced(svs_ba* h, int robust, double huber_delta, double lambda, double* x) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   BaDev& d = h->d;
   int rc;
   if ((rc = set_lambda(h, lambda))) return rc;
   if ((rc = clear_system(h))) return rc;
   launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
-  launch_solve(d, h->max_col_branch, std::max(h->max_col_blocks, h->max_row_blocks - 2), h->nsep_blk, h->stream);
+  solve(h);
   if (d.P) CK(cudaMemcpyAsync(x, d.x, 6 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if ((rc = read_ctl(h))) return rc;
   CK(cudaGetLastError());
   const int failed = h->h_ctl->chol_fail;
   if ((rc = clear_system(h))) return rc;
@@ -1432,23 +1414,16 @@ int svs_ba_set_problem_sharded(svs_ba* h, int P, const double* T_qt, const unsig
 // restoreDataFromG2o on every rank: all landmarks of the sharded window (each rank contributes its own,
 // summed over the communicator)
 int svs_ba_get_points_all(svs_ba* h, double* psi) {
-  if (!h || !h->has_problem || !psi) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
+  if (!psi) return fail(h, SVS_ERR_STATE, "no problem set");
   if (!h->L_full) return svs_ba_get_points(h, psi);
   const size_t n = 3 * (size_t)h->L_full;
   std::fill(psi, psi + n, 0.);
-  int rc;
-  if ((rc = svs_ba_get_points(h, psi))) return rc;
+  if (int rc = svs_ba_get_points(h, psi)) return rc;
   if (!h->comm || h->comm_size == 1) return SVS_OK;
   const NcclApi* nc = nccl_api();
   if (!nc) return fail(h, SVS_ERR_STATE, "NCCL library not loadable");
-  if (n > h->psi_all_cap) {
-    if (h->d_psi_all) cudaFree(h->d_psi_all);
-  if (h->d_out) cudaFree(h->d_out);
-  if (h->h_out) cudaFreeHost(h->h_out);
-    h->d_psi_all = nullptr; h->psi_all_cap = 0;
-    CK(cudaMalloc((void**)&h->d_psi_all, n * sizeof(double)));
-    h->psi_all_cap = n;
-  }
+  CK(grow(n, &h->psi_all_cap, &h->d_psi_all));
   CK(cudaMemcpyAsync(h->d_psi_all, psi, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   if (nc->AllReduce(h->d_psi_all, h->d_psi_all, n, kNcclFloat64, kNcclSum, h->comm, h->stream) != 0)
     return fail(h, SVS_ERR_CUDA, "ncclAllReduce failed");
@@ -1471,10 +1446,9 @@ int svs_ba_set_structure(svs_ba* h, int npairs, const int* pose_i, const int* po
 }
 
 int svs_ba_lm_begin(svs_ba* h, double lambda_init, int max_trials) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
-  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = read_ctl(h)) return rc;
   const int cur = h->h_ctl->cur;
   LmCtl z{};
   z.cur = cur; z.lambda = lambda_init; z.ni = 2; z.max_trials = max_trials;
@@ -1484,7 +1458,7 @@ int svs_ba_lm_begin(svs_ba* h, double lambda_init, int max_trials) {
 }
 
 int svs_ba_trial_build(svs_ba* h, int robust, double huber_delta) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   launch_build(h->d, h->Kmax_gen, robust, huber_delta, h->stream);
   CK(cudaGetLastError());
@@ -1494,7 +1468,7 @@ int svs_ba_trial_build(svs_ba* h, int robust, double huber_delta) {
 
 int svs_ba_system_buffers(svs_ba* h, double** S, long long* nS, double** bp, double** bc, long long* nb,
                           double** totals) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   if (S) *S = h->d.S;
   if (nS) *nS = 36ll * h->d.nblk;
   if (bp) *bp = h->d.bp;
@@ -1505,9 +1479,9 @@ int svs_ba_system_buffers(svs_ba* h, double** S, long long* nS, double** bp, dou
 }
 
 int svs_ba_trial_solve(svs_ba* h, int robust, double huber_delta) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
-  launch_solve(h->d, h->max_col_branch, std::max(h->max_col_blocks, h->max_row_blocks - 2), h->nsep_blk, h->stream);
+  solve(h);
   launch_update(h->d, robust, huber_delta, 1, h->stream);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(h->stream));
@@ -1515,11 +1489,10 @@ int svs_ba_trial_solve(svs_ba* h, int robust, double huber_delta) {
 }
 
 int svs_ba_trial_decide(svs_ba* h, int* again, int* stop, int* iter) {
-  if (!h || !h->has_problem) return h ? fail(h, SVS_ERR_STATE, "no problem set") : SVS_ERR_INVALID;
+  if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   launch_decide_deferred(h->d, h->stream);
-  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = read_ctl(h)) return rc;
   h->cur_known = h->h_ctl->cur;
   CK(cudaGetLastError());
   if (again) *again = h->h_ctl->again;
@@ -1531,14 +1504,7 @@ int svs_ba_trial_decide(svs_ba* h, int* again, int* stop, int* iter) {
 int svs_ba_lm_stats(svs_ba* h, svs_ba_stats* st) {
   if (!h || !h->has_problem || !st) return SVS_ERR_INVALID;
   memset(st, 0, sizeof *st);
-  const LmCtl& c = *h->h_ctl;
-  st->iterations = c.iter; st->trials_total = c.trials_total; st->chi2_init = c.chi_init; st->chi2_final = c.chi_cur;
-  st->lambda_final = c.lambda;
-  for (int i = 0; i < c.iter && i < SVS_BA_MAX_ITERS; ++i) {
-    st->chi2_iter[i] = c.chi_iter[i]; st->lambda_iter[i] = c.lambda_iter[i]; st->trials_iter[i] = c.trials_iter[i];
-  }
-  st->num_frames = h->d.P; st->num_points = h->d.L; st->num_point_edges = h->d.E_user; st->num_frame_edges = h->d.C;
-  st->nnzb_S = h->nnzb_S; st->nnzb_L = h->d.nblk; st->max_track = h->Kmax;
+  fill_stats(h, st);
   return SVS_OK;
 }
 
