@@ -186,6 +186,47 @@ int svs_ba_reduced_system(svs_ba *h, int robust, double huber_delta, double lamb
  * (LinearSolverCSparse::solve, slam_graph.cpp:55-60).  Returns 1 if not positive definite. */
 int svs_ba_solve_reduced(svs_ba *h, int robust, double huber_delta, double lambda, double *x);
 
+/* ------------------------------------------------------------------ block Cholesky of a caller's 6x6-block system
+ * g2o::LinearSolver<Matrix6d>::solve(A, x, b) as LinearSolverCSparse implements it (slam_graph.cpp:55-60), for a
+ * caller that keeps g2o and hands its reduced camera system to the device (INTEGRATION.md).  The elimination order,
+ * the two-ended split and the choice between the cluster solver and the global-memory solver are those of the BA
+ * handle above; a handle owns one internal svs_ba for them.
+ *
+ * Input: the upper triangle of a symmetric positive-definite matrix in block CCS, as g2o's
+ * SparseBlockMatrix::fillCCS(..., upperTriangle = true) sees it:
+ *   col_ptr[P + 1]   starts at 0 and never decreases; nnzb = col_ptr[P];
+ *   row_idx[nnzb]    strictly ascending within each column, row <= column; every column has its diagonal block;
+ *   blocks[nnzb][36] each block column-major (Eigen's Matrix6d::data()).
+ * Only the upper triangle of a diagonal block is read (its lower triangle may hold anything), as CSparse reads an
+ * upper-triangular input.  b and x hold 6P entries in the caller's block order.  The damping is already on the
+ * diagonal (g2o's Levenberg adds lambda before it calls the linear solver): nothing is added or fixed here.
+ * on_device != 0: blocks, b and x are device pointers on the handle's device (e.g. torch CUDA tensors), ready when
+ * the call is made; the pattern arrays are always host arrays (the symbolic analysis runs on the host).
+ * The call returns after x has been written.
+ *
+ * Returns 0 solved; 1 not positive definite (g2o's solve returns false and the trial is rejected), x is zeroed;
+ * SVS_ERR_INVALID for a malformed pattern or a null pointer, checked before anything is enqueued (the handle stays
+ * usable); SVS_ERR_CUDA for a device error.  svs_chol6_create returns SVS_ERR_NOGPU without a device: there is no CPU
+ * fallback.  One handle per thread; each handle has its own stream.
+ *
+ * The symbolic analysis is cached: a call whose pattern equals the previous call's (a cheap host comparison of
+ * col_ptr and row_idx) reuses it, as do the trials of one g2o optimize().  svs_chol6_init is LinearSolver::init():
+ * it forgets the cached analysis. */
+typedef struct svs_chol6 svs_chol6;
+typedef struct {
+  int P, nnzb_A, nnzb_L;   /* block columns, upper blocks given, blocks of the factor */
+  int nbranch;             /* 2 = two-ended elimination, 1 = one chain */
+  int general;             /* 1 = k_solve_general ran */
+  int symbolic_reused;     /* 1 = the cached analysis of the same pattern was used */
+  float ms;                /* device time of scatter + factor + solve */
+} svs_chol6_stats;
+int svs_chol6_create(int device, svs_chol6 **out);   /* device < 0: the current device */
+void svs_chol6_destroy(svs_chol6 *h);
+const char *svs_chol6_last_error(const svs_chol6 *h);
+int svs_chol6_init(svs_chol6 *h);
+int svs_chol6_solve(svs_chol6 *h, int P, const int *col_ptr, const int *row_idx, const double *blocks,
+                    const double *b, double *x, int on_device, svs_chol6_stats *stats);
+
 /* ------------------------------------------------------------------ FAST grid detector */
 
 typedef struct svs_fast svs_fast;

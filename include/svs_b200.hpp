@@ -10,6 +10,7 @@
 //   svs::FastGrid                      <->  ScaViSLAM::FastGrid (fast_grid.h:30-64)
 //   svs::DenseTracker                  <->  ScaViSLAM::DenseTracker / GpuTracker (dense_tracking.h:40-96)
 //   svs::GuidedMatcher                 <->  ScaViSLAM::GuidedMatcher<StereoCamera> (matcher.hpp:62-186)
+//   svs::LinearSolverBlock6            <->  g2o::LinearSolverCSparse<Matrix6d> (slam_graph.cpp:55-60)
 //
 // "We do not use C++ exceptions" (reference README:295): errors come back as bool / int; the
 // text is available from last_error().  There is no CPU fallback anywhere in this layer.
@@ -137,6 +138,36 @@ class StereoGraph {
   std::vector<double> T_, psi_, obs_, info_, cT_, cL_;
   std::vector<unsigned char> fixed_;
   svs_ba_stats last_{};
+};
+
+// g2o::LinearSolver<Matrix6d>::init / solve on the device (svs_chol6_*): the body of a g2o linear solver that
+// keeps the rest of g2o (INTEGRATION.md shows the adapter).  solve() takes the upper triangle of A in block CCS
+// (fillCCS(..., upperTriangle = true)): col_ptr[P + 1], row_idx[nnzb], blocks[nnzb * 36] column-major; x and b
+// hold 6P entries.  Returns false when A is not positive definite (x is zeroed), like g2o; throws
+// std::runtime_error for a malformed input or a device error, and from the constructor without a device.
+class LinearSolverBlock6 {
+ public:
+  explicit LinearSolverBlock6(int device = -1) {
+    if (svs_chol6_create(device, &h_) != SVS_OK) throw std::runtime_error("svs_chol6_create failed (no CUDA device)");
+  }
+  ~LinearSolverBlock6() { if (h_) svs_chol6_destroy(h_); }
+  LinearSolverBlock6(const LinearSolverBlock6&) = delete;
+  LinearSolverBlock6& operator=(const LinearSolverBlock6&) = delete;
+  svs_chol6* handle() { return h_; }
+  // LinearSolver::init(): forget the cached symbolic analysis
+  void init() { check(svs_chol6_init(h_)); }
+  bool solve(int P, const int* col_ptr, const int* row_idx, const double* blocks, double* x, const double* b) {
+    return check(svs_chol6_solve(h_, P, col_ptr, row_idx, blocks, b, x, 0, &last_)) == 0;
+  }
+  const svs_chol6_stats& last_stats() const { return last_; }
+
+ private:
+  int check(int rc) {
+    if (rc < 0) throw std::runtime_error(svs_chol6_last_error(h_));
+    return rc;
+  }
+  svs_chol6* h_ = nullptr;
+  svs_chol6_stats last_{};
 };
 
 // ScaViSLAM::FastGrid (fast_grid.h:30-64).  Keypoints come back as flat (x, y) pairs grouped by

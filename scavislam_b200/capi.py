@@ -53,6 +53,14 @@ class SvsBaStats(C.Structure):
         return d
 
 
+class SvsChol6Stats(C.Structure):
+    _fields_ = [("P", C.c_int), ("nnzb_A", C.c_int), ("nnzb_L", C.c_int), ("nbranch", C.c_int), ("general", C.c_int),
+                ("symbolic_reused", C.c_int), ("ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SvsFastCell(C.Structure):
     _fields_ = [("u0", C.c_int), ("u1", C.c_int), ("v0", C.c_int), ("v1", C.c_int), ("thr", C.c_int)]
 
@@ -130,6 +138,7 @@ EXPORTS = [
     "svs_map_update_points", "svs_map_get", "svs_map_absorb", "svs_map_set_graph", "svs_map_select_window",
     "svs_map_add_keyframe",
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
+    "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
 ]
 
 
@@ -181,6 +190,14 @@ def lib():
     L.svs_ba_comm_init.argtypes = [vp, C.c_int, C.c_int, C.c_char_p]
     L.svs_ba_set_problem_sharded.argtypes = [vp] + prob
     L.svs_ba_get_points_all.argtypes = [vp, c_dp]
+    L.svs_chol6_create.argtypes = [C.c_int, C.POINTER(vp)]
+    L.svs_chol6_destroy.argtypes = [vp]
+    L.svs_chol6_destroy.restype = None
+    L.svs_chol6_last_error.argtypes = [vp]
+    L.svs_chol6_last_error.restype = C.c_char_p
+    L.svs_chol6_init.argtypes = [vp]
+    L.svs_chol6_solve.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                  C.POINTER(SvsChol6Stats)]
     L.svs_fast_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.svs_fast_destroy.argtypes = [vp]
     L.svs_fast_destroy.restype = None
@@ -460,6 +477,64 @@ class BundleAdjuster:
             raise SvsError(it + 100, lib().svs_last_error(self._h).decode())
         self.P, self.L = pb.P, pb.L
         return it, k["pose_qt"], k["psi"], st.as_dict()
+
+
+class BlockCholesky6:
+    """g2o's LinearSolver<Matrix6d>::solve(A, x, b) on the device (svs_chol6_*): A is the upper triangle of a
+    symmetric positive-definite matrix in block CCS -- col_ptr [P+1], row_idx [nnzb] (ascending, row <= column,
+    every column ends in its diagonal block), blocks [nnzb][36] with each block column-major (Eigen's
+    Matrix6d::data(); from numpy, B.ravel(order="F")) -- and b has 6P entries.  No damping is added."""
+
+    def __init__(self, device: int = -1):
+        self._h = C.c_void_p()
+        rc = lib().svs_chol6_create(int(device), C.byref(self._h))
+        if rc != 0:
+            raise SvsError(rc, "svs_chol6_create failed (no CUDA device? there is no CPU fallback)")
+
+    def close(self):
+        if self._h:
+            lib().svs_chol6_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def init(self):
+        """LinearSolver::init(): forget the cached symbolic analysis."""
+        rc = lib().svs_chol6_init(self._h)
+        if rc != 0:
+            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+
+    def solve(self, col_ptr, row_idx, blocks, b):
+        """Returns (x, status, stats): status 0 = solved, 1 = not positive definite (x is zero).  blocks and b are
+        numpy arrays (x comes back as numpy) or CUDA float64 torch tensors on the handle's device (x comes back as a
+        tensor there); col_ptr and row_idx are host integer arrays.  Raises SvsError for a malformed input."""
+        col_ptr = np.ascontiguousarray(col_ptr, np.int32)
+        row_idx = np.ascontiguousarray(row_idx, np.int32)
+        P = len(col_ptr) - 1
+        st = SvsChol6Stats()
+        if isinstance(blocks, np.ndarray) or isinstance(b, np.ndarray):
+            blocks = np.ascontiguousarray(blocks, np.float64)
+            b = np.ascontiguousarray(b, np.float64)
+            x = np.zeros(max(6 * P, 0))
+            args = (blocks.ctypes.data, b.ctypes.data, x.ctypes.data, 0)
+        else:
+            import torch
+            for name, t in (("blocks", blocks), ("b", b)):
+                if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64):
+                    raise TypeError(f"{name}: a numpy array or a CUDA float64 tensor")
+            blocks, b = blocks.contiguous(), b.contiguous()
+            x = torch.zeros(max(6 * P, 0), dtype=torch.float64, device=b.device)
+            torch.cuda.current_stream(b.device).synchronize()   # the handle works on its own stream
+            args = (blocks.data_ptr(), b.data_ptr(), x.data_ptr(), 1)
+        rc = lib().svs_chol6_solve(self._h, P, _ip(col_ptr), _ip(row_idx), C.c_void_p(args[0]), C.c_void_p(args[1]),
+                                   C.c_void_p(args[2]), args[3], C.byref(st))
+        if rc < 0:
+            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+        return x, rc, st.as_dict()
 
 
 class FastGrid:

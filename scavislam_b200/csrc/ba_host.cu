@@ -23,6 +23,7 @@
 
 #include "../../include/svs_b200.h"
 #include "ba_kernels.cuh"
+#include "grow.cuh"
 #include "nccl_dyn.cuh"
 #include "host_pool.hpp"
 #include "svs_nvtx.hpp"
@@ -191,24 +192,6 @@ int dev_upload(svs_ba* h, const T** p, const T* src, size_t n) {
 }
 template <typename T>
 int dev_upload(svs_ba* h, const T** p, const std::vector<T>& v) { return dev_upload(h, p, v.data(), v.size()); }
-
-// Grows a device buffer and/or its pinned host twin (either may be null; both share `cap`) to hold at least n
-// elements, with 25 % headroom so that a slowly growing window does not reallocate on every call.  The contents
-// are not kept.  Only the buffers passed in are touched.
-template <typename T>
-cudaError_t grow(size_t n, size_t* cap, T** dev, T** pinned = nullptr) {
-  if (n <= *cap) return cudaSuccess;
-  if (dev && *dev) cudaFree(*dev);
-  if (pinned && *pinned) cudaFreeHost(*pinned);
-  if (dev) *dev = nullptr;
-  if (pinned) *pinned = nullptr;
-  *cap = 0;
-  const size_t want = n + n / 4;
-  cudaError_t e = dev ? cudaMalloc((void**)dev, want * sizeof(T)) : cudaSuccess;
-  if (e == cudaSuccess && pinned) e = cudaMallocHost((void**)pinned, want * sizeof(T));
-  if (e == cudaSuccess) *cap = want;
-  return e;
-}
 
 void free_problem(svs_ba* h) {
   h->has_problem = false;
@@ -405,7 +388,8 @@ int read_ctl(svs_ba* h) {
   return SVS_OK;
 }
 
-void solve(svs_ba* h) { launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream); }
+// Returns true when the global-memory solver was launched.
+bool solve(svs_ba* h) { return launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream); }
 
 // The fields of svs_ba_stats that the control block and the problem's shape give (not the timings).
 void fill_stats(const svs_ba* h, svs_ba_stats* st) {
@@ -1521,6 +1505,30 @@ int ba_set_problem_device_obs(svs_ba* h, int P, const double* T_qt, const unsign
   return rc;
 }
 int ba_device(const svs_ba* h) { return h->device; }
+int ba_system_on_device(svs_ba* h, const BaDev** d, cudaStream_t* stream, int* symbolic_hits) {
+  if (!h || !h->has_problem) return SVS_ERR_STATE;
+  *d = &h->d; *stream = h->stream; *symbolic_hits = h->symbolic_hits;
+  return SVS_OK;
+}
+int ba_solve_system(svs_ba* h, int* general) {
+  if (int rc = need_problem(h)) return rc;
+  cudaSetDevice(h->device);
+  if (h->cur_known < 0) {
+    if (int rc = read_ctl(h)) return rc;
+    h->cur_known = h->h_ctl->cur;
+  }
+  LmCtl z{};   // lambda = 0, max_iters = 0: the solve runs unconditionally and adds nothing to the diagonal
+  z.cur = h->cur_known;
+  *h->h_ctl = z;
+  CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  *general = solve(h) ? 1 : 0;
+  CK(cudaGetLastError());
+  return SVS_OK;
+}
+void ba_forget_symbolic(svs_ba* h) {
+  h->k_P = -1;      // no same-structure shortcut in the next set_problem
+  h->k_adjP = -1;   // and no reuse of the symbolic analysis
+}
 int ba_state_on_device(svs_ba* h, const double* const** pose, const double* const** psi, const int** lm_user, const int** cur,
                        cudaStream_t* stream, int* P, int* L) {
   if (!h || !h->has_problem) return SVS_ERR_STATE;

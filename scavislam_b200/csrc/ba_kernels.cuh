@@ -10,7 +10,7 @@ size_t build_smem_bytes(int warps, int Kmax);
 void launch_prep(const BaDev& d, int buf, cudaStream_t st);
 void launch_regroup(const BaDev& d, const double* raw, cudaStream_t st);
 void launch_build(const BaDev& d, int Kmax, int robust, double delta, cudaStream_t st);
-void launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st);
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st);   // true: k_solve_general
 int solve_ring_capacity(int P, int nblk, int nsep);
 void launch_solve_general(const BaDev& d, cudaStream_t st);
 int update_grid_blocks(int L, int C);

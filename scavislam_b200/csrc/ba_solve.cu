@@ -918,14 +918,14 @@ int solve_ring_capacity(int P, int nblk, int nsep) {
 }
 
 // Launches the chain/helper kernel when a CTA's ring holds 4 of its widest columns (it keeps two columns
-// live and never checks residency on them); otherwise the global-memory kernel.
-void launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st) {
+// live and never checks residency on them); otherwise the global-memory kernel (returns true).
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st) {
   const int G = d.nbranch;
   int cap = d.P > 0 ? solve_ring_capacity(d.P, d.nblk, G > 1 ? nsep : 0) : 0;
   const int widest = G > 1 ? max_col_branch : max_col_sep;
   if (cap == 0 || cap < 4 * (widest + 1) || cap / 2 < max_col_sep + 2 || G > 2) {
     launch_solve_general(d, st);
-    return;
+    return true;
   }
   while (G == 1 && cap / 2 >= d.nblk && cap / 2 >= 4 * (widest + 1)) cap /= 2;   // small problems: small ring
   int period = cap / (widest + 1) - 3;
@@ -943,6 +943,7 @@ void launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep,
   cfg.numAttrs = 1;
   static const int prof = getenv("SVS_SOLVE_TIMING") ? std::max(1, atoi(getenv("SVS_SOLVE_TIMING"))) : 0;   // 1: phase boundaries, 2: + per-role counters
   cudaLaunchKernelEx(&cfg, k_solve, d, cap, G > 1 ? nsep : 0, period, prof);
+  return false;
 }
 
 }  // namespace svs

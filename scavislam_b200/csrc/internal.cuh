@@ -13,6 +13,16 @@ __attribute__((visibility("hidden"))) int ba_set_problem_device_obs(
     const int* e_pose, const int* e_anchor, const double* d_obs_info, int C, const int* c_i, const int* c_j, const double* c_T,
     const double* c_Lambda, const svs_cam* cam);
 __attribute__((visibility("hidden"))) int ba_device(const svs_ba* h);
+// the block solve of svs_chol6 (chol6.cu) on its internal BA handle: the device image of the problem (S, bp, bc, x,
+// tbl, ctl), the handle's stream and how often the cached symbolic analysis has been reused so far
+struct BaDev;
+__attribute__((visibility("hidden"))) int ba_system_on_device(svs_ba* h, const BaDev** d, cudaStream_t* stream,
+                                                              int* symbolic_hits);
+// sets lambda = 0 and max_iters = 0 in the control block and enqueues the reduced-system solve on the handle's stream
+// (no wait); *general = 1 when the global-memory solver was launched
+__attribute__((visibility("hidden"))) int ba_solve_system(svs_ba* h, int* general);
+// forgets the cached structure and symbolic analysis: the next set_problem analyses the pattern afresh
+__attribute__((visibility("hidden"))) void ba_forget_symbolic(svs_ba* h);
 // the accepted state where it lies on the BA handle's device: pose[2][P][7], psi[2][L][3] (internal landmark order),
 // lm_user[L] (internal -> caller's landmark), *cur = index of the accepted buffers, the handle's stream
 __attribute__((visibility("hidden"))) int ba_state_on_device(svs_ba* h, const double* const** pose, const double* const** psi,
