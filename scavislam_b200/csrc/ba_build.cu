@@ -191,7 +191,6 @@ k_build(BaDev d, const int* __restrict__ lm_list, int n_list, int Kmax, int robu
   }
 }
 
-void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st);
 void launch_build_long(const BaDev& d, int robust, double delta, cudaStream_t st);
 
 // Dispatch: landmark groups with <= 8 frames go to k_build_wave (ba_build_wave.cu); the rest (long

@@ -31,13 +31,36 @@ constexpr int kWvInts = 8 + 40;   // slot poses, pair table (36) padded
 
 size_t build_wave_smem_bytes() { return (size_t)kWvWarps * (kWvDoubles * 8 + kWvInts * 4); }
 
+// kTimeline: the overlap timeline's instance (SVS_SOLVE_TIMING=3, `timeline` = d.dbg + 160); the other one is the plain
+// kernel, whose code the instrumentation must not touch
+template <bool kTimeline>
 __global__ void __launch_bounds__(kWvWarps * 32)
-k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int persist) {
+k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int persist, long long* timeline) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
+  if (!kTimeline) timeline = nullptr;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  pdl_wait();
+  pdl_launch_dependents();
   const LmCtl* __restrict__ ctl = d.ctl;
   if (ctl->max_iters > 0 && (ctl->stop || ctl->iter >= ctl->max_iters)) return;   // speculatively enqueued trial: nothing left to do
   const int cur = ctl->cur;
+  if (threadIdx.x == 0) atomicCAS(&d.ctl->t_build_start, 0ull, global_ns());
+  // overlap timeline (SVS_SOLVE_TIMING=3): every finished task and constraint counts towards the readiness of its poses'
+  // block columns (col_done); timeline[j] gets the moment column j became complete, timeline[2P] the first CTA's entry
+  if (kTimeline && threadIdx.x == 0) atomicCAS(&d.ctl->t_build0, 0ull, global_ns());
+  unsigned* const tctr = d.ticket + 1;
+  // the last warp to leave resets the counter pair for the next launch (on the timeline runs every warp counts, and the
+  // last one files the entry stamp)
+  auto warp_exit = [&]() {
+    if (!(persist || kTimeline)) return;
+    if (kTimeline) __syncwarp();
+    if (lane != 0) return;
+    const unsigned nwarps_total = (unsigned)(kTimeline ? (int)gridDim.x : n_task_blocks) * kWvWarps;
+    if (atomicAdd(tctr + 1, 1u) == nwarps_total - 1) {   // every other warp has drawn its last ticket
+      tctr[0] = 0u; tctr[1] = 0u;
+      if (kTimeline) timeline[2 * d.P] = (long long)atomicExch(&d.ctl->t_build0, 0ull);
+    }
+  };
   // pose-pose constraints (G2oEdgeSE3), one thread each, riding on CTAs of this launch so that their long
   // serial 6x6 arithmetic overlaps the landmark work instead of following it: the trailing CTAs of a
   // one-task-per-warp grid, the LEADING ones of a persistent grid (its task CTAs stay until the list is empty)
@@ -46,13 +69,20 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
     const int cb = persist ? (int)blockIdx.x : (int)blockIdx.x - n_task_blocks;
     if (cb >= 0 && cb < c_blocks) {
       const int c = cb * (kWvWarps * 32) + (int)threadIdx.x;
-      if (c < d.C) constraint_build(d, d.pose[cur], c);
+      if (c < d.C) {
+        constraint_build(d, d.pose[cur], c);
+        if (kTimeline) {
+          __threadfence();
+          signal_column(d, d.pos[d.c_i[c]], timeline);
+          signal_column(d, d.pos[d.c_j[c]], timeline);
+        }
+      }
+      if (kTimeline) warp_exit();
       return;
     }
   }
   // persistent grid: the warps draw tasks from one counter (longest tasks first, set_problem sorts them), so a
   // warp slot is never idle while tasks remain; the last warp to leave resets the counter pair for the next launch
-  unsigned* const tctr = d.ticket + 1;
   auto next_task = [&]() {
     int t = 0;
     if (lane == 0) t = (int)atomicAdd(tctr, 1u);
@@ -355,16 +385,18 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
       atomicAdd(d.bc + 6 * p + r, accc[q]);
     }
   }
+  if (kTimeline) {   // the task's blocks and right-hand sides are complete: count it for each of its slot poses' columns
+    __threadfence();
+    __syncwarp();
+    if (lane < K) signal_column(d, d.pos[sPose[lane]], timeline);
+  }
   PBW(6);
   if (prof && lane == 0)
     for (int i = 0; i < 7; ++i) atomicAdd(reinterpret_cast<unsigned long long*>(d.dbg) + 48 + i, (unsigned long long)pacc[i]);
 #undef PBW
     __syncwarp();   // the next task reuses this warp's shared-memory tables
   }
-  if (persist && lane == 0) {
-    const unsigned nwarps_total = (unsigned)n_task_blocks * kWvWarps;
-    if (atomicAdd(tctr + 1, 1u) == nwarps_total - 1) { tctr[0] = 0u; tctr[1] = 0u; }   // every other warp has drawn its last ticket
-  }
+  warp_exit();
 }
 
 // resident CTAs of k_build_wave on the current device (occupancy x SM count), cached per device
@@ -375,19 +407,21 @@ static int build_wave_resident_ctas() {
   if (dev < 0 || dev >= 64) return 1 << 30;
   if (cache[dev] == 0) {
     int per_sm = 0, sms = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_build_wave, kWvWarps * 32, build_wave_smem_bytes());
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_build_wave<false>, kWvWarps * 32, build_wave_smem_bytes());
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cache[dev] = per_sm > 0 && sms > 0 ? per_sm * sms : 1 << 30;
   }
   return cache[dev];
 }
 
-void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st) {
+void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st, int pdl) {
   if (d.ntasks == 0 && d.C == 0) return;
   static const int prof = getenv("SVS_BUILD_TIMING") ? 1 : 0;
   // the opt-in above 48 KB of dynamic shared memory is per device: handles may live on several GPUs of one process
-  if (device_needs_smem_optin(0, build_wave_smem_bytes()))
-    cudaFuncSetAttribute(k_build_wave, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)build_wave_smem_bytes());
+  if (device_needs_smem_optin(0, build_wave_smem_bytes())) {
+    cudaFuncSetAttribute(k_build_wave<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)build_wave_smem_bytes());
+    cudaFuncSetAttribute(k_build_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)build_wave_smem_bytes());
+  }
   int task_blocks = (d.ntasks + kWvWarps - 1) / kWvWarps;
   const int c_blocks = (d.C + kWvWarps * 32 - 1) / (kWvWarps * 32);
   // persistent grid when the tasks outnumber the warp slots: as many task CTAs as are resident at once (255 registers
@@ -395,7 +429,20 @@ void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st
   const int resident = build_wave_resident_ctas();
   const int persist = task_blocks > resident ? 1 : 0;
   if (persist) task_blocks = resident;
-  k_build_wave<<<task_blocks + c_blocks, kWvWarps * 32, build_wave_smem_bytes(), st>>>(d, robust, delta, task_blocks, prof, persist);
+  static const int timing = getenv("SVS_SOLVE_TIMING") ? atoi(getenv("SVS_SOLVE_TIMING")) : 0;
+  long long* timeline = timing >= 3 ? d.dbg + 160 : nullptr;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(task_blocks + c_blocks, 1, 1);
+  cfg.blockDim = dim3(kWvWarps * 32, 1, 1);
+  cfg.dynamicSmemBytes = build_wave_smem_bytes();
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl ? 1 : 0;
+  if (timeline) cudaLaunchKernelEx(&cfg, k_build_wave<true>, d, robust, delta, task_blocks, prof, persist, timeline);
+  else cudaLaunchKernelEx(&cfg, k_build_wave<false>, d, robust, delta, task_blocks, prof, persist, (long long*)nullptr);
 }
 
 }  // namespace svs

@@ -89,6 +89,26 @@ __device__ __forceinline__ double warp_sum(double v) {
   return v;
 }
 
+// ---- overlap timeline (SVS_SOLVE_TIMING=3, scripts/probes/overlap_timeline.py): when each block column of S is complete
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+// ---- programmatic dependent launch (svs_ba_optimize's trials, DESIGN.md 5).  Every kernel of a trial waits for the
+// whole previous kernel of the stream (completed, its memory visible) before it reads anything that kernel may write,
+// and then lets the next kernel's CTAs be scheduled, so that they are resident and waiting when this one ends instead
+// of being launched after it.  Both are no-ops for a kernel that was launched without the attribute.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// One work item that writes into block column `col` (and its right-hand side) is complete (the caller fences its writes
+// first); the moment the column's last item lands is stamped.
+__device__ __forceinline__ void signal_column(const BaDev& d, int col, long long* ready_ns) {
+  const int was = atomicAdd(d.col_done + col, 1);
+  if (ready_ns && was + 1 == __ldg(d.col_need + col)) ready_ns[col] = (long long)global_ns();
+}
+
 // ------------------------------------------------------------------ pose-pose constraint (one thread)
 
 __device__ inline void third(const double A[7], const double dd[6], double out[36]) {

@@ -907,6 +907,17 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   if (sy.nblk >= (1 << 20)) return fail(h, SVS_ERR_UNSUPPORTED, "reduced system factor has more than 2^20 blocks");
 
   lap("analyse");
+  // ---- column readiness (overlap timeline, SVS_SOLVE_TIMING=3): col_need[j] = the tasks whose slot list holds the pose
+  // of column j, plus the pose-pose constraints on it; k_build_wave counts them in col_done as they finish (bp and bc of a
+  // pose are written by the same items, so a complete column also has a complete right-hand side)
+  std::vector<int> col_need(P, 0);
+  {
+    for (int li : task_lm) {
+      col_need[sy.pos[lm_anchor[li]]]++;
+      for (int x = lm_eptr[li] + lm_self[li]; x < lm_eptr[li + 1]; ++x) col_need[sy.pos[ie_pose[x]]]++;   // the slot poses after the anchor
+    }
+    for (int c = 0; c < C; ++c) { col_need[sy.pos[c_i[c]]]++; col_need[sy.pos[c_j[c]]]++; }
+  }
   // ---- device image: constant arrays (uploaded in one copy) followed by work buffers
   BaDev& d = h->d;
   d.P = P; d.L = L; d.E = ne; d.E_user = E; d.C = C; d.nslots = ns; d.nblk = sy.nblk; d.flags = h->flags;
@@ -924,7 +935,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
     UP(task_lm, task_lm); UP(task_cnt, task_cnt); UP(gen_lm, gen_lm); UP(long_lm, long_lm);
     UP(tbl, sy.tbl); UP(perm, sy.perm); UP(pos, sy.pos); UP(col_ptr, sy.col_ptr); UP(row_idx, sy.row_idx);
     UP(upd_ptr, sy.upd_ptr); UP(upd_dst, sy.upd_dst); UP(upd_ab, sy.upd_ab); UP(urg_dst, sy.urg_dst);
-    UP(branch_ptr, sy.branch_ptr); UP(rptr, sy.rptr); UP(rowpos, sy.rowpos); UP(rcol, sy.rcol);
+    UP(branch_ptr, sy.branch_ptr); UP(rptr, sy.rptr); UP(rowpos, sy.rowpos); UP(rcol, sy.rcol); UP(col_need, col_need);
     dev_upload(h, &d.c_i, c_i, (size_t)C); dev_upload(h, &d.c_j, c_j, (size_t)C);
     h->off_num = h->off_cT = h->arena_off;   // the numbers (everything a same-structure call re-sends) lie last
     dev_upload(h, &d.c_T, c_T, 7 * (size_t)C);
@@ -950,7 +961,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
     AL(x, 6 * (size_t)P); AL(Nrow, 36 * (size_t)std::max(sy.nblk - P, 1));
     AL(chi_c, C); AL(chi_c_new, C); AL(Linv, 36 * (size_t)P); AL(ywork, 6 * (size_t)P);
     AL(ctl, 1);
-    AL(part, 3 * (size_t)update_grid_blocks(L, C)); AL(ticket, 4); AL(dbg, 160);
+    AL(part, 3 * (size_t)update_grid_blocks(L, C)); AL(ticket, 4); AL(dbg, 160 + 2 * (size_t)P + 2); AL(col_done, P);
 #undef AL
   };
   h->measuring = true;
@@ -1007,6 +1018,7 @@ static int clear_system(svs_ba* h) {
   CK(cudaMemsetAsync(d.S, 0, 36 * (size_t)d.nblk * sizeof(double), h->stream));
   CK(cudaMemsetAsync(d.bp, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
   CK(cudaMemsetAsync(d.bc, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
+  CK(cudaMemsetAsync(d.col_done, 0, std::max(d.P, 1) * sizeof(int), h->stream));
   return SVS_OK;
 }
 
@@ -1039,6 +1051,12 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
   const NcclApi* nc = h->comm ? nccl_api() : nullptr;   // sharded window: sums across ranks on this stream
   if (h->comm && !nc) return fail(h, SVS_ERR_STATE, "NCCL library not loadable");
   const int per_trial = 2 + ((d.ntasks > 0 || d.C > 0) ? 1 : 0) + (d.ngen > 0 ? 1 : 0) + (d.nlong > 0 ? 1 : 0) + (nc ? 1 : 0);
+  // A trial that is exactly k_build_wave -> k_solve -> k_update (no all-reduce, no generic or long tracks, the chain
+  // solver) runs as one chain of programmatic dependent launches: each kernel's CTAs are scheduled while the previous
+  // kernel still runs and wait for it on the device (griddepcontrol.wait before they read anything), which removes the
+  // launch gap at every kernel boundary.  No event may stand between the launches, so the kernels time themselves.
+  const bool chained = !nc && d.ngen == 0 && d.nlong == 0 && (d.ntasks > 0 || d.C > 0) &&
+                       solve_uses_chain_kernel(d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk);
 #define CKN(call)                                                       \
   do {                                                                  \
     const int e_ = (call);                                              \
@@ -1055,7 +1073,12 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     // Terminate) return at once (LmCtl::max_iters).  Only rejected steps cost another round trip.
     const int ntr = num_iters - it;
     while ((int)h->tev.size() < kEv * ntr) { cudaEvent_t e; cudaEventCreate(&e); h->tev.push_back(e); }
-    for (int k = 0; k < ntr; ++k) {
+    for (int k = 0; k < ntr && chained; ++k) {
+      launch_build_wave(d, robust, huber_delta, h->stream, 1);
+      launch_solve(d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream, 1);
+      launch_update(d, robust, huber_delta, 0, h->stream, 1);
+    }
+    for (int k = 0; k < ntr && !chained; ++k) {
       CK(cudaEventRecord(h->tev[kEv * k + 0], h->stream));
       launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
       CK(cudaEventRecord(h->tev[kEv * k + 1], h->stream));
@@ -1083,7 +1106,7 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     const int done_trials = h->h_ctl->trials_total - trials_seen;
     trials_seen = h->h_ctl->trials_total;
     launches += per_trial * done_trials;
-    for (int k = 0; k < done_trials && k < ntr; ++k) {
+    for (int k = 0; k < done_trials && k < ntr && !chained; ++k) {
       static const int slot[kEv - 1] = {0, 3, 1, 2, 3};   // build | collective | solve | update | collective + decision
       for (int q = 0; q < kEv - 1; ++q) {
         float t = 0;
@@ -1100,6 +1123,10 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
   if (st) {
     fill_stats(h, st);
     cudaEventElapsedTime(&st->ms_total, h->ev[0], h->ev[1]);
+    if (chained) {   // the kernels' own stamps (LmCtl), summed over the call's trials on the device
+      const LmCtl& c = *h->h_ctl;
+      ms[0] = 1e-6f * (float)c.ns_build; ms[1] = 1e-6f * (float)c.ns_solve; ms[2] = 1e-6f * (float)c.ns_update;
+    }
     st->ms_build = ms[0]; st->ms_solve = ms[1]; st->ms_update = ms[2]; st->ms_control = ms[3];
     st->launches = launches;
   }
@@ -1110,8 +1137,26 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
             "schur+direct %lld gradients %lld flush %lld\n", dbg[48], dbg[49], dbg[50], dbg[51], dbg[52], dbg[53], dbg[54]);
     cudaMemset(d.dbg + 48, 0, 8 * sizeof(long long));
   }
+  if (getenv("SVS_SOLVE_TIMING") && atoi(getenv("SVS_SOLVE_TIMING")) >= 3) {
+    // the last trial's overlap timeline (scripts/probes/overlap_timeline.py): per column in elimination order the moment
+    // it became ready (the build's last work item on it) and the moment the chain published it, in microseconds since
+    // the first k_build_wave CTA entered
+    std::vector<long long> tl(2 * (size_t)d.P + 2);
+    std::vector<int> bptr(d.nbranch + 1);
+    cudaMemcpy(tl.data(), d.dbg + 160, tl.size() * sizeof(long long), cudaMemcpyDeviceToHost);
+    cudaMemcpy(bptr.data(), d.branch_ptr, bptr.size() * sizeof(int), cudaMemcpyDeviceToHost);
+    const long long t0 = tl[2 * d.P];
+    fprintf(stderr, "overlap timeline: branches %d solve_entry_us %.3f\n", d.nbranch,
+            1e-3 * (double)(tl[2 * d.P + 1] - t0));
+    for (int j = 0; j < d.P; ++j) {
+      int g = 0;
+      while (g < d.nbranch && j >= bptr[g + 1]) ++g;   // g == nbranch: separator
+      fprintf(stderr, "  col %d group %d pos %d ready_us %.3f chain_us %.3f\n", j, g, j - bptr[g],
+              1e-3 * (double)(tl[j] - t0), 1e-3 * (double)(tl[d.P + j] - t0));
+    }
+  }
   if (getenv("SVS_SOLVE_TIMING")) {
-    const bool roles = atoi(getenv("SVS_SOLVE_TIMING")) > 1;
+    const bool roles = atoi(getenv("SVS_SOLVE_TIMING")) == 2;
     if (roles) {
       long long tr[160];
       cudaMemcpy(tr, d.dbg, sizeof tr, cudaMemcpyDeviceToHost);

@@ -10,11 +10,16 @@ size_t build_smem_bytes(int warps, int Kmax);
 void launch_prep(const BaDev& d, int buf, cudaStream_t st);
 void launch_regroup(const BaDev& d, const double* raw, cudaStream_t st);
 void launch_build(const BaDev& d, int Kmax, int robust, double delta, cudaStream_t st);
-bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st);   // true: k_solve_general
+// pdl = 1 (launch_build_wave, launch_solve, launch_update): launched with programmatic stream serialisation, so the
+// kernel's CTAs are scheduled while the previous kernel of the stream still runs and wait for it on the device
+// (svs_ba_optimize's trials, DESIGN.md 5)
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl = 0);   // true: k_solve_general
+bool solve_uses_chain_kernel(const BaDev& d, int max_col_branch, int max_col_sep, int nsep);
+void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st, int pdl = 0);
 int solve_ring_capacity(int P, int nblk, int nsep);
 void launch_solve_general(const BaDev& d, cudaStream_t st);
 int update_grid_blocks(int L, int C);
-void launch_update(const BaDev& d, int robust, double delta, int defer_decision, cudaStream_t st);
+void launch_update(const BaDev& d, int robust, double delta, int defer_decision, cudaStream_t st, int pdl = 0);
 void launch_decide_deferred(const BaDev& d, cudaStream_t st);
 void launch_chi2(const BaDev& d, int robust, double delta, cudaStream_t st);
 void launch_export(const BaDev& d, double* out, cudaStream_t st);

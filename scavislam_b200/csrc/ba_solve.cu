@@ -152,7 +152,8 @@ struct Team {
   int area_off;               // separator accumulation area of this CTA: block b at area + (b - sep_blk0) * 36
   int slot;                   // index of the team's fail flags / diagonal-factor buffers
   int refill_period;
-  long long* prof;            // nullptr or 16 cycle counters (developer knob SVS_SOLVE_TIMING)
+  long long* prof;            // nullptr or 16 cycle counters (developer knob SVS_SOLVE_TIMING=2)
+  long long* timeline;        // nullptr or [P] %globaltimer when the chain publishes each column (SVS_SOLVE_TIMING=3)
 };
 
 #define TRACE(k, j) do { if (T.prof && T.slot == 0 && (j) - T.j0 >= 10 && (j) - T.j0 < 26 && (threadIdx.x & 31) == 0) T.prof[52 + (k) * 16 + ((j) - T.j0 - 10)] = clock64(); } while (0)
@@ -269,6 +270,7 @@ __device__ __forceinline__ void ring_refill(const BaDev& d, const Team& T, const
 //                          right-hand side, N_ij for the backward pass.  They re-join the chain only through kBarPub, one
 //                          column later; since every helper must arrive there, "column j published" also means
 //                          "all of column j-1 applied".
+template <bool kTimeline>
 __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S, double lambda) {
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int* col_ptr = S.col_ptr; const int* upd_ptr = S.upd_ptr; const int* row_idx = S.row_idx;
@@ -356,6 +358,7 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
       }
       bar_arrive(kBarPub, kPubAll);
       TRACE(0, j);
+      if (kTimeline && T.timeline && lane == 0) T.timeline[d.P + j] = (long long)global_ns();
       PCH(3);
       if (!ok) { produced = j - T.j0; break; }
       linked = nlinked;
@@ -708,6 +711,8 @@ __device__ void load_row_index(const BaDev& d, const SolveShared& S) {
 // smem layout: [ring: cap*36 doubles][area: nsep*36 doubles][y: 6P doubles][meta ints: col_ptr (P+1),
 //               upd_ptr (P+1), row_idx (nblk)][fixed-by-position bytes (P)]
 // cap is a power of two >= 4 * (widest column of a branch + 1).
+// kTimeline: the overlap timeline's instance (SVS_SOLVE_TIMING=3): the chain stamps each column it publishes
+template <bool kTimeline>
 __global__ void __launch_bounds__(kSolveThreads)
 k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   __shared__ int sFail[2][2];
@@ -716,14 +721,23 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   __shared__ __align__(16) double sCdiag[22];
   __shared__ int sXfail;   // written by the other CTA of the cluster
   __shared__ int sChunk[kMaxChunks + 2];
+  pdl_wait();
+  pdl_launch_dependents();
   LmCtl* ctl = d.ctl;
   if (ctl->max_iters > 0 && (ctl->stop || ctl->iter >= ctl->max_iters)) return;   // speculatively enqueued trial: nothing left to do
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   const int t = threadIdx.x, nt = kSolveThreads, lane = t & 31, warp = t >> 5;
+  const unsigned long long t_start = global_ns();
+  if (rank == 0 && t == 0 && ctl->t_build_start) {   // the build before this launch has completed
+    ctl->ns_build += (long long)(t_start - ctl->t_build_start);
+    ctl->t_build_start = 0;
+  }
   const int P = d.P, nblk = d.nblk;
   const double lambda = ctl->lambda;
   const int cur = ctl->cur;
+  long long* const timeline = (kTimeline && d.dbg) ? d.dbg + 160 : nullptr;
+  if (timeline && rank == 0 && t == 0) timeline[2 * d.P + 1] = (long long)global_ns();
   const int G = d.nbranch;                 // 1: a single chain, 2: two ends + separator (cluster of 2 CTAs)
   const int sep0 = d.branch_ptr[G];        // first separator column (= P when G == 1)
   SolveShared S;
@@ -760,8 +774,9 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   Team br;
   br.ring_off = ring_off; br.org = 0; br.mask = (unsigned)cap - 1u; br.cap = cap; br.prefilled = 0;
   br.j0 = my0; br.j1 = my1; br.sep_blk0 = sep_blk0; br.area_off = area_off; br.slot = 0; br.refill_period = refill_branch;
-  br.prof = (prof > 1 && d.dbg) ? d.dbg + 12 + 16 * rank : nullptr;   // [.. + 32 + 3): unit phases of helper 0 (rank 0: dbg 44..46, rank 1: 56..58)
-  factor_range(d, br, S, lambda);
+  br.prof = (prof == 2 && d.dbg) ? d.dbg + 12 + 16 * rank : nullptr;   // [.. + 32 + 3): unit phases of helper 0 (rank 0: dbg 44..46, rank 1: 56..58)
+  br.timeline = timeline;
+  factor_range<kTimeline>(d, br, S, lambda);
   tk[1] = clock64();
   int failed = sFail[0][0] | sFail[0][1];
   if (G > 1) {
@@ -785,7 +800,8 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
         Team sp;
         sp.ring_off = area_off; sp.org = sep_blk0; sp.mask = 0xffffffffu; sp.cap = nsep; sp.prefilled = 1;
         sp.j0 = sep0; sp.j1 = P; sp.sep_blk0 = nblk; sp.area_off = area_off; sp.slot = 1; sp.refill_period = 1 << 30; sp.prof = nullptr;
-        factor_range(d, sp, S, lambda);
+        sp.timeline = timeline;
+        factor_range<kTimeline>(d, sp, S, lambda);
         failed = sFail[1][0] | sFail[1][1];
       }
       tk[3] = clock64();
@@ -814,6 +830,7 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
       for (int i = t; i < 7 * P; i += nt) d.pose[1 - cur][i] = d.pose[cur][i];
       for (int i = t; i < 12 * P; i += nt) d.Rt[1 - cur][i] = d.Rt[cur][i];
       for (int i = t; i < 6 * P; i += nt) d.x[i] = 0;
+      if (t == 0) ctl->ns_solve += (long long)(global_ns() - t_start);
     }
     if (G > 1) cluster.sync();   // keeps the barrier count of the two CTAs equal (#3)
     return;
@@ -867,6 +884,7 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   if (rank == 0 && t == 0) {
     ctl->scale_pose = mine + sRed[kSolveThreads / 32];
     ctl->chol_fail = 0;
+    ctl->ns_solve += (long long)(global_ns() - t_start);
   }
   tk[6] = clock64();
   if (d.dbg && t == 0)   // phase boundaries in cycles since the setup
@@ -890,7 +908,8 @@ int solve_smem_optin() {
   SolveDev& s = g_dev[dev];
   if (!s.done) {
     cudaDeviceGetAttribute(&s.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    cudaFuncSetAttribute(k_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
+    cudaFuncSetAttribute(k_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
+    cudaFuncSetAttribute(k_solve<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
     s.done = true;
   }
   return s.smem_optin;
@@ -917,16 +936,24 @@ int solve_ring_capacity(int P, int nblk, int nsep) {
   return cap <= avail ? cap : 0;
 }
 
-// Launches the chain/helper kernel when a CTA's ring holds 4 of its widest columns (it keeps two columns
-// live and never checks residency on them); otherwise the global-memory kernel (returns true).
-bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st) {
+// The chain/helper kernel runs when a CTA's ring holds 4 of its widest columns (it keeps two columns live and never
+// checks residency on them); otherwise the global-memory kernel.
+bool solve_uses_chain_kernel(const BaDev& d, int max_col_branch, int max_col_sep, int nsep) {
   const int G = d.nbranch;
-  int cap = d.P > 0 ? solve_ring_capacity(d.P, d.nblk, G > 1 ? nsep : 0) : 0;
+  const int cap = d.P > 0 ? solve_ring_capacity(d.P, d.nblk, G > 1 ? nsep : 0) : 0;
   const int widest = G > 1 ? max_col_branch : max_col_sep;
-  if (cap == 0 || cap < 4 * (widest + 1) || cap / 2 < max_col_sep + 2 || G > 2) {
+  return !(cap == 0 || cap < 4 * (widest + 1) || cap / 2 < max_col_sep + 2 || G > 2);
+}
+
+// Launches k_solve, or the global-memory kernel (returns true).
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl) {
+  const int G = d.nbranch;
+  if (!solve_uses_chain_kernel(d, max_col_branch, max_col_sep, nsep)) {
     launch_solve_general(d, st);
     return true;
   }
+  int cap = solve_ring_capacity(d.P, d.nblk, G > 1 ? nsep : 0);
+  const int widest = G > 1 ? max_col_branch : max_col_sep;
   while (G == 1 && cap / 2 >= d.nblk && cap / 2 >= 4 * (widest + 1)) cap /= 2;   // small problems: small ring
   int period = cap / (widest + 1) - 3;
   period = period < 1 ? 1 : (period > 64 ? 64 : period);
@@ -936,13 +963,18 @@ bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep,
   cfg.blockDim = dim3(kSolveThreads, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = G; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  static const int prof = getenv("SVS_SOLVE_TIMING") ? std::max(1, atoi(getenv("SVS_SOLVE_TIMING"))) : 0;   // 1: phase boundaries, 2: + per-role counters
-  cudaLaunchKernelEx(&cfg, k_solve, d, cap, G > 1 ? nsep : 0, period, prof);
+  cfg.numAttrs = pdl ? 2 : 1;
+  // 1: phase boundaries, 2: + per-role counters, 3: phase boundaries + the overlap timeline (when the chain publishes each
+  // column; k_build_wave stamps when each column became complete)
+  static const int prof = getenv("SVS_SOLVE_TIMING") ? std::max(1, atoi(getenv("SVS_SOLVE_TIMING"))) : 0;
+  if (prof >= 3) cudaLaunchKernelEx(&cfg, k_solve<true>, d, cap, G > 1 ? nsep : 0, period, prof);
+  else cudaLaunchKernelEx(&cfg, k_solve<false>, d, cap, G > 1 ? nsep : 0, period, prof);
   return false;
 }
 

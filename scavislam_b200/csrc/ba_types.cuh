@@ -24,6 +24,13 @@ struct LmCtl {
   int trials_total;
   int max_trials;
   int max_iters;   // > 0: kernels of trials enqueued past the end (or after Terminate) return at once
+  // device durations of the trials of svs_ba_optimize's chained launch, where no stream event may sit between two kernels
+  // (%globaltimer, ns): the first k_build_wave CTA past its wait -> k_solve past its wait; k_solve's CTA 0; the first
+  // k_update CTA past its wait -> the end of its last CTA
+  unsigned long long t_build_start, t_update_start;
+  long long ns_build, ns_solve, ns_update;
+  unsigned long long t_build0;   // overlap timeline (SVS_SOLVE_TIMING=3): %globaltimer at the entry of the first
+                                 // k_build_wave CTA of the trial (0: none yet)
   double chi_init;
   double chi_iter[kMaxIters];
   double lambda_iter[kMaxIters];
@@ -92,7 +99,11 @@ struct BaDev {
   double* part;        // [update grid][3] per-CTA partial sums (chi2 accepted, chi2 trial, scale)
   unsigned* ticket;    // [4] last-CTA-done counter of k_update; [1], [2]: task counter / warps-done counter of a persistent k_build_wave
   double* totals;      // [3] chi2 accepted / chi2 trial / scale of this rank's landmarks (sharded window)
-  long long* dbg;      // [24] per-phase cycle counters of k_solve (thread 0, thread 64)
+  long long* dbg;      // [160 + 2P + 2] per-phase cycle counters of k_solve and k_build_wave; from 160 on the
+                       // overlap timeline (SVS_SOLVE_TIMING=3): column ready, chain at column, build / solve entry
+  // readiness of the block columns of S (elimination order), counted by k_build_wave on the overlap timeline runs
+  const int* col_need;  // [P] work items that write column j or its right-hand side (build tasks + constraints)
+  int* col_done;        // [P] of them finished in this trial (cleared by k_update)
   LmCtl* ctl;
 };
 

@@ -78,8 +78,11 @@ __global__ void __launch_bounds__(WARPS * 32)
 k_update(BaDev d, int robust, double delta, int n_lm_blocks, int defer_decision) {
   __shared__ double sPart[WARPS][3];
   __shared__ int sLast;
+  pdl_wait();
+  pdl_launch_dependents();
   LmCtl* ctl = d.ctl;
   if (ctl->max_iters > 0 && (ctl->stop || ctl->iter >= ctl->max_iters)) return;   // speculatively enqueued trial: nothing left to do
+  if (threadIdx.x == 0) atomicCAS(&ctl->t_update_start, 0ull, global_ns());
   const int cur = ctl->cur, trial = 1 - cur;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // every CTA helps clearing the reduced system for the next build
@@ -87,6 +90,7 @@ k_update(BaDev d, int robust, double delta, int n_lm_blocks, int defer_decision)
     const size_t gid = (size_t)blockIdx.x * blockDim.x + threadIdx.x, gn = (size_t)gridDim.x * blockDim.x;
     for (size_t i = gid; i < (size_t)d.nblk * 36; i += gn) d.S[i] = 0.;
     for (size_t i = gid; i < (size_t)6 * d.P; i += gn) { d.bp[i] = 0.; d.bc[i] = 0.; }
+    for (size_t i = gid; i < (size_t)d.P; i += gn) d.col_done[i] = 0;   // (counted on the overlap timeline runs)
   }
   double part_cur = 0, part_new = 0, part_scale = 0;   // this warp's share (valid on lane 0)
   if ((int)blockIdx.x >= n_lm_blocks) {
@@ -202,6 +206,8 @@ k_update(BaDev d, int robust, double delta, int n_lm_blocks, int defer_decision)
   }
   if (threadIdx.x == 0) {
     *d.ticket = 0;
+    ctl->ns_update += (long long)(global_ns() - ctl->t_update_start);
+    ctl->t_update_start = 0;
     if (defer_decision) {   // sharded window: the totals are summed over ranks before the decision
       d.totals[0] = sFin[0][0]; d.totals[1] = sFin[0][1]; d.totals[2] = sFin[0][2];
     } else {
@@ -215,14 +221,23 @@ __global__ void k_decide_deferred(BaDev d) {
 }
 void launch_decide_deferred(const BaDev& d, cudaStream_t st) { k_decide_deferred<<<1, 32, 0, st>>>(d); }
 
-void launch_update(const BaDev& d, int robust, double delta, int defer_decision, cudaStream_t st) {
+void launch_update(const BaDev& d, int robust, double delta, int defer_decision, cudaStream_t st, int pdl) {
   constexpr int WARPS = 8;
   constexpr int kPerBlock = WARPS * (32 / kLmLanes);
   const int n_lm_blocks = (d.L + kPerBlock - 1) / kPerBlock;
   const int n_c_blocks = (d.C + WARPS * 32 - 1) / (WARPS * 32);
   int nb = n_lm_blocks + n_c_blocks;
   if (nb == 0) nb = 1;   // still clears the reduced system and takes the LM decision
-  k_update<WARPS><<<nb, WARPS * 32, 0, st>>>(d, robust, delta, n_lm_blocks, defer_decision);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(nb, 1, 1);
+  cfg.blockDim = dim3(WARPS * 32, 1, 1);
+  cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = pdl ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, k_update<WARPS>, d, robust, delta, n_lm_blocks, defer_decision);
 }
 int update_grid_blocks(int L, int C) {
   constexpr int WARPS = 8;
