@@ -227,6 +227,28 @@ int svs_chol6_init(svs_chol6 *h);
 int svs_chol6_solve(svs_chol6 *h, int P, const int *col_ptr, const int *row_idx, const double *blocks,
                     const double *b, double *x, int on_device, svs_chol6_stats *stats);
 
+/* Marginals: blocks of A^-1 from the same factor, as LinearSolverCSparse's solveBlocks / solvePattern compute them
+ * for SparseOptimizer::computeMarginals.  The pattern, blocks, on_device, the return codes, the validation and the
+ * analysis cache are those of svs_chol6_solve (a solve and an inversion on one pattern share one analysis).  Every
+ * block the factor stores (the pattern of A plus fill-in) comes from one selected inversion over the factor; a
+ * requested block outside it from a solve of its block column (stats->n_cols_solved).  Each output block is
+ * column-major (Eigen's data()); block (r, c) with r > c is the transpose of (c, r), so any order is valid.
+ * Returns 1 with all outputs zeroed when A is not positive definite.  req_r / req_c are always host arrays; a request
+ * outside [0, P), n < 0 or a null request array with n > 0 is SVS_ERR_INVALID, before anything is enqueued. */
+typedef struct {
+  int P, nnzb_A, nnzb_L, nbranch, general, symbolic_reused;   /* as in svs_chol6_stats */
+  int n_in_pattern;        /* requests served from the selected inversion */
+  int n_cols_solved;       /* block columns solved for requests outside the factor's pattern */
+  float ms;                /* device time of scatter + factor + inversion */
+} svs_chol6_inv_stats;
+/* LinearSolver::solveBlocks(blocks, A): the P diagonal blocks of A^-1, inv_diag [P][36] column-major */
+int svs_chol6_solve_blocks(svs_chol6 *h, int P, const int *col_ptr, const int *row_idx, const double *blocks,
+                           double *inv_diag, int on_device, svs_chol6_inv_stats *stats);
+/* LinearSolver::solvePattern(spinv, blockIndices, A): blocks (req_r[k], req_c[k]) of A^-1, out [n][36] column-major */
+int svs_chol6_solve_pattern(svs_chol6 *h, int P, const int *col_ptr, const int *row_idx, const double *blocks,
+                            int n, const int *req_r, const int *req_c, double *out, int on_device,
+                            svs_chol6_inv_stats *stats);
+
 /* ------------------------------------------------------------------ FAST grid detector */
 
 typedef struct svs_fast svs_fast;

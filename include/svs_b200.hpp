@@ -159,7 +159,17 @@ class LinearSolverBlock6 {
   bool solve(int P, const int* col_ptr, const int* row_idx, const double* blocks, double* x, const double* b) {
     return check(svs_chol6_solve(h_, P, col_ptr, row_idx, blocks, b, x, 0, &last_)) == 0;
   }
+  // LinearSolver::solveBlocks: the P diagonal blocks of A^-1 into inv_diag [P][36] (column-major)
+  bool solveBlocks(int P, const int* col_ptr, const int* row_idx, const double* blocks, double* inv_diag) {
+    return check(svs_chol6_solve_blocks(h_, P, col_ptr, row_idx, blocks, inv_diag, 0, &last_inv_)) == 0;
+  }
+  // LinearSolver::solvePattern: blocks (r[k], c[k]) of A^-1 into out [n][36] (column-major)
+  bool solvePattern(int P, const int* col_ptr, const int* row_idx, const double* blocks, int n, const int* r,
+                    const int* c, double* out) {
+    return check(svs_chol6_solve_pattern(h_, P, col_ptr, row_idx, blocks, n, r, c, out, 0, &last_inv_)) == 0;
+  }
   const svs_chol6_stats& last_stats() const { return last_; }
+  const svs_chol6_inv_stats& last_inv_stats() const { return last_inv_; }
 
  private:
   int check(int rc) {
@@ -168,6 +178,7 @@ class LinearSolverBlock6 {
   }
   svs_chol6* h_ = nullptr;
   svs_chol6_stats last_{};
+  svs_chol6_inv_stats last_inv_{};
 };
 
 // ScaViSLAM::FastGrid (fast_grid.h:30-64).  Keypoints come back as flat (x, y) pairs grouped by

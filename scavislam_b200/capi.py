@@ -61,6 +61,14 @@ class SvsChol6Stats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class SvsChol6InvStats(C.Structure):
+    _fields_ = [("P", C.c_int), ("nnzb_A", C.c_int), ("nnzb_L", C.c_int), ("nbranch", C.c_int), ("general", C.c_int),
+                ("symbolic_reused", C.c_int), ("n_in_pattern", C.c_int), ("n_cols_solved", C.c_int), ("ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SvsFastCell(C.Structure):
     _fields_ = [("u0", C.c_int), ("u1", C.c_int), ("v0", C.c_int), ("v1", C.c_int), ("thr", C.c_int)]
 
@@ -139,6 +147,7 @@ EXPORTS = [
     "svs_map_add_keyframe",
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
+    "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
 ]
 
 
@@ -198,6 +207,10 @@ def lib():
     L.svs_chol6_init.argtypes = [vp]
     L.svs_chol6_solve.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                   C.POINTER(SvsChol6Stats)]
+    L.svs_chol6_solve_blocks.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.POINTER(SvsChol6InvStats)]
+    L.svs_chol6_solve_pattern.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_int, c_ip, c_ip, C.c_void_p, C.c_int,
+                                          C.POINTER(SvsChol6InvStats)]
     L.svs_fast_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.svs_fast_destroy.argtypes = [vp]
     L.svs_fast_destroy.restype = None
@@ -535,6 +548,48 @@ class BlockCholesky6:
         if rc < 0:
             raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
         return x, rc, st.as_dict()
+
+    def _inverse(self, col_ptr, row_idx, blocks, n, call):
+        """Shared by solve_blocks / solve_pattern: n output blocks, host or device like `blocks`; call(P, cp, ri,
+        blocks_ptr, out_ptr, on_device, stats) runs the C entry point."""
+        col_ptr = np.ascontiguousarray(col_ptr, np.int32)
+        row_idx = np.ascontiguousarray(row_idx, np.int32)
+        P = len(col_ptr) - 1
+        st = SvsChol6InvStats()
+        if isinstance(blocks, np.ndarray):
+            blocks = np.ascontiguousarray(blocks, np.float64)
+            out = np.zeros((n, 36))
+            args = (blocks.ctypes.data, out.ctypes.data, 0)
+        else:
+            import torch
+            if not (isinstance(blocks, torch.Tensor) and blocks.is_cuda and blocks.dtype == torch.float64):
+                raise TypeError("blocks: a numpy array or a CUDA float64 tensor")
+            blocks = blocks.contiguous()
+            out = torch.zeros((n, 36), dtype=torch.float64, device=blocks.device)
+            torch.cuda.current_stream(blocks.device).synchronize()   # the handle works on its own stream
+            args = (blocks.data_ptr(), out.data_ptr(), 1)
+        rc = call(P, _ip(col_ptr), _ip(row_idx), C.c_void_p(args[0]), C.c_void_p(args[1]), args[2], C.byref(st))
+        if rc < 0:
+            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+        # column-major blocks -> ordinary 6x6 matrices
+        return out.reshape(n, 6, 6).swapaxes(1, 2), rc, st.as_dict()
+
+    def solve_blocks(self, col_ptr, row_idx, blocks):
+        """LinearSolver::solveBlocks: returns (inv_diag [P, 6, 6], status, stats), the diagonal blocks of A^-1;
+        status 1 = not positive definite (all zero).  Inputs as for solve()."""
+        P = max(len(col_ptr) - 1, 0)
+        return self._inverse(col_ptr, row_idx, blocks, P, lambda *a: lib().svs_chol6_solve_blocks(self._h, *a))
+
+    def solve_pattern(self, col_ptr, row_idx, blocks, pairs):
+        """LinearSolver::solvePattern: returns (out [n, 6, 6], status, stats) with out[k] = block (r, c) of A^-1 for
+        pairs[k] = (r, c), in any order; status 1 = not positive definite (all zero).  Inputs as for solve()."""
+        pairs = np.asarray(pairs, np.int64).reshape(-1, 2)
+        r = np.ascontiguousarray(pairs[:, 0], np.int32)
+        c = np.ascontiguousarray(pairs[:, 1], np.int32)
+        n = len(pairs)
+        return self._inverse(col_ptr, row_idx, blocks, n,
+                             lambda P, cp, ri, bl, out, dev, st: lib().svs_chol6_solve_pattern(
+                                 self._h, P, cp, ri, bl, n, _ip(r), _ip(c), out, dev, st))
 
 
 class FastGrid:

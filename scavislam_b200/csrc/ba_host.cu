@@ -1555,7 +1555,7 @@ int ba_system_on_device(svs_ba* h, const BaDev** d, cudaStream_t* stream, int* s
   *d = &h->d; *stream = h->stream; *symbolic_hits = h->symbolic_hits;
   return SVS_OK;
 }
-int ba_solve_system(svs_ba* h, int* general) {
+int ba_solve_system(svs_ba* h, int* general, int keep_diag) {
   if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   if (h->cur_known < 0) {
@@ -1566,7 +1566,7 @@ int ba_solve_system(svs_ba* h, int* general) {
   z.cur = h->cur_known;
   *h->h_ctl = z;
   CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
-  *general = solve(h) ? 1 : 0;
+  *general = launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream, 0, keep_diag) ? 1 : 0;
   CK(cudaGetLastError());
   return SVS_OK;
 }

@@ -13,7 +13,9 @@ void launch_build(const BaDev& d, int Kmax, int robust, double delta, cudaStream
 // pdl = 1 (launch_build_wave, launch_solve, launch_update): launched with programmatic stream serialisation, so the
 // kernel's CTAs are scheduled while the previous kernel of the stream still runs and wait for it on the device
 // (svs_ba_optimize's trials, DESIGN.md 5)
-bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl = 0);   // true: k_solve_general
+// keep_diag = 1: k_solve also stores L_jj^-1 of every column into d.Linv (k_solve_general always does)
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl = 0,
+                  int keep_diag = 0);   // true: k_solve_general
 bool solve_uses_chain_kernel(const BaDev& d, int max_col_branch, int max_col_sep, int nsep);
 void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st, int pdl = 0);
 int solve_ring_capacity(int P, int nblk, int nsep);

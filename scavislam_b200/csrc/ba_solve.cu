@@ -270,7 +270,9 @@ __device__ __forceinline__ void ring_refill(const BaDev& d, const Team& T, const
 //                          right-hand side, N_ij for the backward pass.  They re-join the chain only through kBarPub, one
 //                          column later; since every helper must arrive there, "column j published" also means
 //                          "all of column j-1 applied".
-template <bool kTimeline>
+// kDiag: the chain warp also stores L_jj^-1 of every column it factors into d.Linv (row-major, zero above the
+// diagonal: k_solve_general's layout), for the selected inversion of svs_chol6 (chol6_inv.cu)
+template <bool kTimeline, bool kDiag>
 __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S, double lambda) {
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int* col_ptr = S.col_ptr; const int* upd_ptr = S.upd_ptr; const int* row_idx = S.row_idx;
@@ -359,6 +361,20 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
       bar_arrive(kBarPub, kPubAll);
       TRACE(0, j);
       if (kTimeline && T.timeline && lane == 0) T.timeline[d.P + j] = (long long)global_ns();
+      if (kDiag) {   // behind the publish: lane c < 6 forms column c of L_jj^-1 from l and rinv
+        const int cc = lane < 6 ? lane : 0;
+        double ai[6];
+#pragma unroll
+        for (int r2 = 0; r2 < 6; ++r2) {
+          double v = r2 == cc ? 1. : 0.;
+#pragma unroll
+          for (int q = 0; q < r2; ++q) v = fma(-l[r2 * (r2 + 1) / 2 + q], ai[q], v);   // ai[q] = 0 above the diagonal
+          ai[r2] = r2 < cc ? 0. : v * rinv[r2];
+        }
+        if (lane < 6)
+#pragma unroll
+          for (int r2 = 0; r2 < 6; ++r2) d.Linv[36 * (size_t)j + 6 * r2 + cc] = ai[r2];
+      }
       PCH(3);
       if (!ok) { produced = j - T.j0; break; }
       linked = nlinked;
@@ -712,7 +728,8 @@ __device__ void load_row_index(const BaDev& d, const SolveShared& S) {
 //               upd_ptr (P+1), row_idx (nblk)][fixed-by-position bytes (P)]
 // cap is a power of two >= 4 * (widest column of a branch + 1).
 // kTimeline: the overlap timeline's instance (SVS_SOLVE_TIMING=3): the chain stamps each column it publishes
-template <bool kTimeline>
+// kDiag: svs_chol6's marginals instance: the diagonal factor blocks are kept (factor_range)
+template <bool kTimeline, bool kDiag>
 __global__ void __launch_bounds__(kSolveThreads)
 k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   __shared__ int sFail[2][2];
@@ -776,7 +793,7 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   br.j0 = my0; br.j1 = my1; br.sep_blk0 = sep_blk0; br.area_off = area_off; br.slot = 0; br.refill_period = refill_branch;
   br.prof = (prof == 2 && d.dbg) ? d.dbg + 12 + 16 * rank : nullptr;   // [.. + 32 + 3): unit phases of helper 0 (rank 0: dbg 44..46, rank 1: 56..58)
   br.timeline = timeline;
-  factor_range<kTimeline>(d, br, S, lambda);
+  factor_range<kTimeline, kDiag>(d, br, S, lambda);
   tk[1] = clock64();
   int failed = sFail[0][0] | sFail[0][1];
   if (G > 1) {
@@ -801,7 +818,7 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
         sp.ring_off = area_off; sp.org = sep_blk0; sp.mask = 0xffffffffu; sp.cap = nsep; sp.prefilled = 1;
         sp.j0 = sep0; sp.j1 = P; sp.sep_blk0 = nblk; sp.area_off = area_off; sp.slot = 1; sp.refill_period = 1 << 30; sp.prof = nullptr;
         sp.timeline = timeline;
-        factor_range<kTimeline>(d, sp, S, lambda);
+        factor_range<kTimeline, kDiag>(d, sp, S, lambda);
         failed = sFail[1][0] | sFail[1][1];
       }
       tk[3] = clock64();
@@ -908,8 +925,9 @@ int solve_smem_optin() {
   SolveDev& s = g_dev[dev];
   if (!s.done) {
     cudaDeviceGetAttribute(&s.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    cudaFuncSetAttribute(k_solve<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
-    cudaFuncSetAttribute(k_solve<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
+    cudaFuncSetAttribute(k_solve<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
+    cudaFuncSetAttribute(k_solve<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
+    cudaFuncSetAttribute(k_solve<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, s.smem_optin - kStaticSmem);
     s.done = true;
   }
   return s.smem_optin;
@@ -946,7 +964,7 @@ bool solve_uses_chain_kernel(const BaDev& d, int max_col_branch, int max_col_sep
 }
 
 // Launches k_solve, or the global-memory kernel (returns true).
-bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl) {
+bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep, cudaStream_t st, int pdl, int keep_diag) {
   const int G = d.nbranch;
   if (!solve_uses_chain_kernel(d, max_col_branch, max_col_sep, nsep)) {
     launch_solve_general(d, st);
@@ -973,8 +991,9 @@ bool launch_solve(const BaDev& d, int max_col_branch, int max_col_sep, int nsep,
   // 1: phase boundaries, 2: + per-role counters, 3: phase boundaries + the overlap timeline (when the chain publishes each
   // column; k_build_wave stamps when each column became complete)
   static const int prof = getenv("SVS_SOLVE_TIMING") ? std::max(1, atoi(getenv("SVS_SOLVE_TIMING"))) : 0;
-  if (prof >= 3) cudaLaunchKernelEx(&cfg, k_solve<true>, d, cap, G > 1 ? nsep : 0, period, prof);
-  else cudaLaunchKernelEx(&cfg, k_solve<false>, d, cap, G > 1 ? nsep : 0, period, prof);
+  if (keep_diag) cudaLaunchKernelEx(&cfg, k_solve<false, true>, d, cap, G > 1 ? nsep : 0, period, prof);
+  else if (prof >= 3) cudaLaunchKernelEx(&cfg, k_solve<true, false>, d, cap, G > 1 ? nsep : 0, period, prof);
+  else cudaLaunchKernelEx(&cfg, k_solve<false, false>, d, cap, G > 1 ? nsep : 0, period, prof);
   return false;
 }
 

@@ -19,8 +19,9 @@ struct BaDev;
 __attribute__((visibility("hidden"))) int ba_system_on_device(svs_ba* h, const BaDev** d, cudaStream_t* stream,
                                                               int* symbolic_hits);
 // sets lambda = 0 and max_iters = 0 in the control block and enqueues the reduced-system solve on the handle's stream
-// (no wait); *general = 1 when the global-memory solver was launched
-__attribute__((visibility("hidden"))) int ba_solve_system(svs_ba* h, int* general);
+// (no wait); *general = 1 when the global-memory solver was launched.  keep_diag = 1: the chain solver also leaves
+// L_jj^-1 in BaDev::Linv, as the general one always does
+__attribute__((visibility("hidden"))) int ba_solve_system(svs_ba* h, int* general, int keep_diag = 0);
 // forgets the cached structure and symbolic analysis: the next set_problem analyses the pattern afresh
 __attribute__((visibility("hidden"))) void ba_forget_symbolic(svs_ba* h);
 // the accepted state where it lies on the BA handle's device: pose[2][P][7], psi[2][L][3] (internal landmark order),
