@@ -186,6 +186,38 @@ int svs_ba_reduced_system(svs_ba *h, int robust, double huber_delta, double lamb
  * (LinearSolverCSparse::solve, slam_graph.cpp:55-60).  Returns 1 if not positive definite. */
 int svs_ba_solve_reduced(svs_ba *h, int robust, double huber_delta, double lambda, double *x);
 
+/* Marginal covariances of the window (g2o SparseOptimizer::computeMarginals for the caller who replaced all of
+ * SlamGraph::optimize): blocks of (H + lambda I)^-1 over the free variables.
+ *   State: the handle's accepted state -- the initial one after set_problem / set_problem_from_map, or the result of
+ *     the last optimize.  H is the Gauss-Newton matrix the build kernels form there, with the robust weights of
+ *     `robust` / `huber_delta` as in svs_ba_reduced_system; lambda (finite, >= 0) is added to every pose and landmark
+ *     diagonal, as a Levenberg trial adds it.  The rows and columns of fixed poses are dropped (they are not
+ *     variables): every block that involves a fixed pose is returned as zero.
+ *   Outputs (each may be NULL; blocks row-major):
+ *     pose_cov [P][36]       diagonal pose blocks in the caller's pose order, tangent order (upsilon, omega);
+ *     pair_cov [npairs][36]  Cov(x_i, x_j) for i = pair_i[k], j = pair_j[k] (poses, any order; (j, i) is the transpose);
+ *     point_cov [L][9]       landmark blocks in psi = (x/z, y/z, 1/z), the variable the optimiser estimates, in the
+ *                            caller's landmark order; exactly symmetric; zero for a landmark without edges.  For
+ *                            xyz_anchor = invert_depth(psi), apply the Jacobian J of invert_depth: J Sigma J^T.
+ *   Method: one factor of the reduced system at lambda, one selected inversion on the factor's pattern (every pose
+ *   pair a landmark couples lies in it), a solve of the block column of each requested pair outside the pattern, and
+ *   Sigma_ll = D + sum_ab Y_a^T Z_ab Y_b per landmark (D = (Hll + lambda I)^-1, Y_a = Hpl_a D, Z = S^-1).
+ *   Returns 0; 1 when the reduced system is not positive definite (all outputs zeroed); SVS_ERR_STATE before a problem
+ *   is set; SVS_ERR_INVALID for lambda < 0 or not finite, npairs < 0, npairs > 0 with a null pair_i, pair_j or
+ *   pair_cov, a pair index outside [0, P), and for lambda = 0 with no fixed pose (H is then exactly singular: every
+ *   edge is invariant under one global SE3, SURVEY.md B2) -- all checked before anything is enqueued;
+ *   SVS_ERR_UNSUPPORTED when the handle has a communicator (sharded windows).  The Levenberg state is left as it was
+ *   found: a later svs_ba_optimize gives the same bits whether or not this call ran in between. */
+typedef struct {
+  int P, L, nnzb_L, nbranch, general;   /* as in svs_chol6_stats, for the handle's own factor */
+  int n_pairs_in_pattern;               /* pairs served from the selected inversion */
+  int n_cols_solved;                    /* block columns solved for pairs outside the factor's pattern */
+  float ms;                             /* device time: build + factor + inversion + landmark kernel */
+} svs_ba_cov_stats;
+int svs_ba_covariance(svs_ba *h, int robust, double huber_delta, double lambda, double *pose_cov, int npairs,
+                      const int *pair_i, const int *pair_j, double *pair_cov, double *point_cov,
+                      svs_ba_cov_stats *stats);
+
 /* ------------------------------------------------------------------ block Cholesky of a caller's 6x6-block system
  * g2o::LinearSolver<Matrix6d>::solve(A, x, b) as LinearSolverCSparse implements it (slam_graph.cpp:55-60), for a
  * caller that keeps g2o and hands its reduced camera system to the device (INTEGRATION.md).  The elimination order,

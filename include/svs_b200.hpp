@@ -7,6 +7,7 @@
 //                                           SlamGraph::Statistics (slam_graph.hpp:366-386)
 //   svs::StereoGraph::optimize         <->  SlamGraph<SE3,StereoCamera,SE3XYZ_STEREO,3>::optimize
 //                                           (slam_graph.cpp:319-355) = copyDataToG2o + g2o + restore
+//   svs::StereoGraph::computeMarginals <->  g2o::SparseOptimizer::computeMarginals on that window
 //   svs::FastGrid                      <->  ScaViSLAM::FastGrid (fast_grid.h:30-64)
 //   svs::DenseTracker                  <->  ScaViSLAM::DenseTracker / GpuTracker (dense_tracking.h:40-96)
 //   svs::GuidedMatcher                 <->  ScaViSLAM::GuidedMatcher<StereoCamera> (matcher.hpp:62-186)
@@ -93,10 +94,13 @@ class StereoGraph {
         !remap(ci_, pose_id_, ci) || !remap(cj_, pose_id_, cj))
       return -100 + SVS_ERR_INVALID;
     svs_ba_stats st{};
+    robust_ = p.use_robust_kernel ? 1 : 0;
+    delta_ = apply_huber_width ? p.huber_kernel_width : 1.0;
+    opt_P_ = pose_id_.size(); opt_L_ = point_id_.size();
     const int it = svs_optimiseInnerAndOuterWindow(
         h_, (int)pose_id_.size(), T_.data(), fixed_.data(), (int)point_id_.size(), psi_.data(), (int)ep.size(), ep.data(),
         ef.data(), ea.data(), obs_.data(), info_.data(), (int)ci.size(), ci.data(), cj.data(), cT_.data(), cL_.data(), &cam_,
-        p.num_iters, p.use_robust_kernel ? 1 : 0, apply_huber_width ? p.huber_kernel_width : 1.0, &st);
+        p.num_iters, robust_, delta_, &st);
     if (stats && it > -100) {
       stats->num_frames = st.num_frames; stats->num_points = st.num_points;
       stats->num_point_edges = st.num_point_edges; stats->num_frame_edges = st.num_frame_edges;
@@ -113,6 +117,27 @@ class StereoGraph {
   size_t num_poses() const { return pose_id_.size(); }
   size_t num_points() const { return point_id_.size(); }
   const svs_ba_stats& last_stats() const { return last_; }
+
+  // SparseOptimizer::computeMarginals for the window the last optimize() ran on (svs_ba_covariance): blocks of
+  // (H + lambda I)^-1 at the optimised state, with the robust kernel of that call; row-major, zero for fixed poses.
+  //   pose_cov  [P][36]  in addPose order;   point_cov [L][9] in psi = (x/z, y/z, 1/z), in addPoint order;
+  //   pair_cov  [n][36]  Cov(x_i, x_j) for the frame ids (i, j) of pose_pairs[k].
+  // Any output may be null (pair_cov only when pose_pairs is empty).  Returns false when the factor fails (the outputs
+  // are zero), and when there is nothing to take them from: no optimize() on the current poses and points, an unknown
+  // frame id, or an error of the C ABI (last_error(); lambda = 0 needs a fixed pose).
+  bool computeMarginals(double lambda, std::vector<double>* pose_cov, std::vector<double>* point_cov,
+                        const std::vector<std::pair<int, int>>& pose_pairs = {}, std::vector<double>* pair_cov = nullptr) {
+    if (!ok_ || opt_P_ != pose_id_.size() || opt_L_ != point_id_.size()) return false;
+    const size_t n = pose_pairs.size();
+    std::vector<int> fi(n), fj(n), pi(n), pj(n);
+    for (size_t k = 0; k < n; ++k) { fi[k] = pose_pairs[k].first; fj[k] = pose_pairs[k].second; }
+    if (n && (!pair_cov || !remap(fi, pose_id_, pi) || !remap(fj, pose_id_, pj))) return false;
+    if (pose_cov) pose_cov->assign(36 * pose_id_.size(), 0.);
+    if (point_cov) point_cov->assign(9 * point_id_.size(), 0.);
+    if (pair_cov) pair_cov->assign(36 * n, 0.);
+    return svs_ba_covariance(h_, robust_, delta_, lambda, pose_cov ? pose_cov->data() : nullptr, (int)n, pi.data(), pj.data(),
+                             n ? pair_cov->data() : nullptr, point_cov ? point_cov->data() : nullptr, nullptr) == 0;
+  }
 
  private:
   static void push7(std::vector<double>& v, const SE3d& T) { v.insert(v.end(), T.q, T.q + 4); v.insert(v.end(), T.t, T.t + 3); }
@@ -138,6 +163,9 @@ class StereoGraph {
   std::vector<double> T_, psi_, obs_, info_, cT_, cL_;
   std::vector<unsigned char> fixed_;
   svs_ba_stats last_{};
+  int robust_ = 0;
+  double delta_ = 1.0;
+  size_t opt_P_ = (size_t)-1, opt_L_ = (size_t)-1;   // window of the last optimize()
 };
 
 // g2o::LinearSolver<Matrix6d>::init / solve on the device (svs_chol6_*): the body of a g2o linear solver that

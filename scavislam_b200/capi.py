@@ -69,6 +69,14 @@ class SvsChol6InvStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class SvsBaCovStats(C.Structure):
+    _fields_ = [("P", C.c_int), ("L", C.c_int), ("nnzb_L", C.c_int), ("nbranch", C.c_int), ("general", C.c_int),
+                ("n_pairs_in_pattern", C.c_int), ("n_cols_solved", C.c_int), ("ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SvsFastCell(C.Structure):
     _fields_ = [("u0", C.c_int), ("u1", C.c_int), ("v0", C.c_int), ("v1", C.c_int), ("thr", C.c_int)]
 
@@ -148,6 +156,7 @@ EXPORTS = [
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
+    "svs_ba_covariance",
 ]
 
 
@@ -185,6 +194,8 @@ def lib():
     L.svs_ba_chi2.argtypes = [vp, C.c_int, C.c_double, c_dp]
     L.svs_ba_reduced_system.argtypes = [vp, C.c_int, C.c_double, C.c_double, c_dp, c_dp, c_dp]
     L.svs_ba_solve_reduced.argtypes = [vp, C.c_int, C.c_double, C.c_double, c_dp]
+    L.svs_ba_covariance.argtypes = [vp, C.c_int, C.c_double, C.c_double, c_dp, C.c_int, c_ip, c_ip, c_dp, c_dp,
+                                    C.POINTER(SvsBaCovStats)]
     L.svs_device_info.argtypes = [C.c_char_p, C.c_int]
     L.svs_ba_set_structure.argtypes = [vp, C.c_int, c_ip, c_ip]
     L.svs_ba_lm_begin.argtypes = [vp, C.c_double, C.c_int]
@@ -426,6 +437,23 @@ class BundleAdjuster:
         if rc < 0:
             self._check(rc)
         return x, rc
+
+    def covariance(self, robust=True, huber_delta=1.0, lam=0.0, pairs=()):
+        """Marginal covariances at the accepted state (svs_ba_covariance): blocks of (H + lam I)^-1 over the free
+        variables, zero for fixed poses.  Returns (pose_cov [P,6,6], pair_cov [n,6,6] with pair_cov[k] =
+        Cov(x_i, x_j) for pairs[k] = (i, j), point_cov [L,3,3] in psi, rc, stats); rc = 1: not positive definite
+        (outputs zeroed)."""
+        pr = np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+        pi, pj = np.ascontiguousarray(pr[:, 0]), np.ascontiguousarray(pr[:, 1])
+        n = len(pr)
+        pose, pair, point = np.zeros((self.P, 6, 6)), np.zeros((n, 6, 6)), np.zeros((self.L, 3, 3))
+        st = SvsBaCovStats()
+        rc = lib().svs_ba_covariance(self._h, int(robust), float(huber_delta), float(lam), _dp(pose), n,
+                                     _ip(pi) if n else None, _ip(pj) if n else None, _dp(pair) if n else None,
+                                     _dp(point), C.byref(st))
+        if rc < 0:
+            self._check(rc)
+        return pose, pair, point, rc, st.as_dict()
 
     # ---- stepwise trial API (window split by landmarks across ranks, SURVEY.md 8e)
     def set_structure(self, pairs):

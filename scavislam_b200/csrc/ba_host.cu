@@ -7,6 +7,7 @@
 // when the device path is unavailable.
 #include <algorithm>
 #include <atomic>
+#include <cmath>
 #include <cstdio>
 #include <chrono>
 #include <cstdlib>
@@ -26,6 +27,7 @@
 #include "grow.cuh"
 #include "nccl_dyn.cuh"
 #include "host_pool.hpp"
+#include "marginals.cuh"
 #include "svs_nvtx.hpp"
 
 using namespace svs;
@@ -138,6 +140,12 @@ struct svs_ba {
   Symbolic k_sy; std::vector<unsigned char> k_adj; int k_adjP = -1, k_nbranch = 1, k_nsep = 0, k_nnzb = 0; bool k_natural = false;
   int symbolic_hits = 0;
   std::vector<cudaEvent_t> tev;   // per-trial timing events
+  // svs_ba_covariance: host copies of the analysis' table and positions (fetched once per structure), the selected
+  // inversion's scratch, the requested blocks | landmark blocks
+  std::vector<int> cov_tbl, cov_pos;
+  bool cov_tables = false;
+  InvScratch inv;
+  double* d_cov = nullptr; double* h_cov = nullptr; size_t cov_cap = 0;
 };
 
 namespace {
@@ -195,6 +203,7 @@ int dev_upload(svs_ba* h, const T** p, const std::vector<T>& v) { return dev_upl
 
 void free_problem(svs_ba* h) {
   h->has_problem = false;
+  h->cov_tables = false;
   h->d = BaDev{};
 }
 
@@ -388,8 +397,11 @@ int read_ctl(svs_ba* h) {
   return SVS_OK;
 }
 
-// Returns true when the global-memory solver was launched.
-bool solve(svs_ba* h) { return launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream); }
+// Returns true when the global-memory solver was launched.  keep_diag = 1: L_jj^-1 is kept in BaDev::Linv (the
+// selected inversion of marginals.cu reads it), with the same solver choice as the trials.
+bool solve(svs_ba* h, int keep_diag = 0) {
+  return launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream, 0, keep_diag);
+}
 
 // The fields of svs_ba_stats that the control block and the problem's shape give (not the timings).
 void fill_stats(const svs_ba* h, svs_ba_stats* st) {
@@ -458,6 +470,9 @@ void svs_ba_destroy(svs_ba* h) {
   if (h->d_psi_all) cudaFree(h->d_psi_all);
   if (h->d_out) cudaFree(h->d_out);
   if (h->h_out) cudaFreeHost(h->h_out);
+  h->inv.release();
+  if (h->d_cov) cudaFree(h->d_cov);
+  if (h->h_cov) cudaFreeHost(h->h_cov);
   for (auto& e : h->ev) cudaEventDestroy(e);
   for (auto& e : h->tev) cudaEventDestroy(e);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
@@ -1341,6 +1356,89 @@ int svs_ba_solve_reduced(svs_ba* h, int robust, double huber_delta, double lambd
   return failed ? 1 : 0;
 }
 
+int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, double* pose_cov, int npairs,
+                      const int* pair_i, const int* pair_j, double* pair_cov, double* point_cov, svs_ba_cov_stats* stats) {
+  svs::NvtxRange nvtx_("computeMarginals");
+  if (int rc = need_problem(h)) return rc;
+  if (stats) memset(stats, 0, sizeof *stats);
+  const std::string fn = "svs_ba_covariance: ";
+  BaDev& d = h->d;
+  const int P = d.P, L = d.L;
+  if (h->comm) return fail(h, SVS_ERR_UNSUPPORTED, fn + "the handle has a communicator (sharded windows are not supported)");
+  if (!std::isfinite(lambda) || lambda < 0.) return fail(h, SVS_ERR_INVALID, fn + "lambda must be finite and >= 0");
+  if (npairs < 0) return fail(h, SVS_ERR_INVALID, fn + "npairs < 0");
+  if (npairs > 0 && (!pair_i || !pair_j || !pair_cov)) return fail(h, SVS_ERR_INVALID, fn + "null pair_i, pair_j or pair_cov");
+  for (int k = 0; k < npairs; ++k)
+    if (pair_i[k] < 0 || pair_i[k] >= P || pair_j[k] < 0 || pair_j[k] >= P)
+      return fail(h, SVS_ERR_INVALID, fn + "pair " + std::to_string(k) + " (" + std::to_string(pair_i[k]) + ", " +
+                                          std::to_string(pair_j[k]) + ") is outside [0, P)");
+  if (P == 0) {   // no poses, hence no edges: every landmark block is zero
+    if (point_cov) std::fill(point_cov, point_cov + 9 * (size_t)L, 0.);
+    return 0;
+  }
+  const unsigned char* fx = h->k_fixed.data();
+  if (lambda == 0. && std::none_of(fx, fx + P, [](unsigned char f) { return f != 0; }))
+    return fail(h, SVS_ERR_INVALID, fn + "H is singular with no fixed pose and lambda = 0 (every edge is invariant under one "
+                                         "global SE3): fix a pose or pass lambda > 0");
+  cudaSetDevice(h->device);
+  int rc;
+  if (!h->cov_tables) {
+    h->cov_tbl.resize((size_t)P * P);
+    h->cov_pos.resize(P);
+    CK(cudaMemcpyAsync(h->cov_tbl.data(), d.tbl, h->cov_tbl.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(h->cov_pos.data(), d.pos, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    h->cov_tables = true;
+  }
+  // the kernels run unconditionally at this lambda; the control block is put back as it was found at the end
+  if ((rc = read_ctl(h))) return rc;
+  const LmCtl saved = *h->h_ctl;
+  h->h_ctl->lambda = lambda;
+  h->h_ctl->max_iters = 0;
+  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  if ((rc = clear_system(h))) return rc;
+  CK(cudaEventRecord(h->ev[0], h->stream));
+  launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
+  const int general = solve(h, 1) ? 1 : 0;
+  // requests: the diagonal blocks, then (j, i) for pair k -- its column-major gather is Cov(x_i, x_j) row-major
+  const int ndiag = pose_cov ? P : 0, n = ndiag + npairs;
+  std::vector<int> rq_r(n), rq_c(n);
+  for (int p = 0; p < ndiag; ++p) rq_r[p] = rq_c[p] = p;
+  for (int k = 0; k < npairs; ++k) { rq_r[ndiag + k] = pair_j[k]; rq_c[ndiag + k] = pair_i[k]; }
+  int in_pattern = 0, ncols = 0;
+  CK(invert(d, general, h->cov_tbl.data(), h->cov_pos.data(), n, rq_r.data(), rq_c.data(), &h->inv, h->stream, &in_pattern,
+            &ncols));
+  const size_t nb = 36 * (size_t)n, npt = point_cov ? 9 * (size_t)L : 0;
+  CK(grow(nb + npt, &h->cov_cap, &h->d_cov, &h->h_cov));
+  if (npt) launch_point_cov(d, h->inv.zx, lambda, h->d_cov + nb, h->stream);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(h->ev[1], h->stream));
+  CK(gather(d, h->inv, h->d_cov, h->stream));
+  if (nb + npt) CK(cudaMemcpyAsync(h->h_cov, h->d_cov, (nb + npt) * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if ((rc = read_ctl(h))) return rc;
+  const int failed = h->h_ctl->chol_fail;
+  if ((rc = clear_system(h))) return rc;
+  *h->h_ctl = saved;
+  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  // fixed poses are not variables: every block that involves one is zero
+  const double* hc = h->h_cov;
+  auto put = [&](double* dst, const double* src, bool zero) {
+    if (zero) std::fill(dst, dst + 36, 0.);
+    else memcpy(dst, src, 36 * sizeof(double));
+  };
+  for (int p = 0; p < ndiag; ++p) put(pose_cov + 36 * (size_t)p, hc + 36 * (size_t)p, fx[p] != 0);
+  for (int k = 0; k < npairs; ++k)
+    put(pair_cov + 36 * (size_t)k, hc + 36 * (size_t)(ndiag + k), fx[pair_i[k]] || fx[pair_j[k]]);
+  if (npt) memcpy(point_cov, hc + nb, npt * sizeof(double));
+  if (stats) {
+    stats->P = P; stats->L = L; stats->nnzb_L = d.nblk; stats->nbranch = d.nbranch; stats->general = general;
+    stats->n_pairs_in_pattern = in_pattern - ndiag; stats->n_cols_solved = ncols;
+    cudaEventElapsedTime(&stats->ms, h->ev[0], h->ev[1]);
+  }
+  return failed ? 1 : 0;
+}
+
 // ---- one window sharded by landmarks across GPUs, driven inside the library (SURVEY.md 8e, BASELINE config C5)
 
 int svs_comm_unique_id(char id[128]) {
@@ -1566,7 +1664,7 @@ int ba_solve_system(svs_ba* h, int* general, int keep_diag) {
   z.cur = h->cur_known;
   *h->h_ctl = z;
   CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
-  *general = launch_solve(h->d, h->solve_col_branch, h->solve_col_sep, h->nsep_blk, h->stream, 0, keep_diag) ? 1 : 0;
+  *general = solve(h, keep_diag) ? 1 : 0;
   CK(cudaGetLastError());
   return SVS_OK;
 }

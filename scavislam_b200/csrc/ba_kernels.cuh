@@ -25,4 +25,7 @@ void launch_update(const BaDev& d, int robust, double delta, int defer_decision,
 void launch_decide_deferred(const BaDev& d, cudaStream_t st);
 void launch_chi2(const BaDev& d, int robust, double delta, cudaStream_t st);
 void launch_export(const BaDev& d, double* out, cudaStream_t st);
+// landmark blocks of (H + lambda I)^-1 into out [L][9] (caller's landmark order) from Z = S^-1 on the factor's pattern
+// and the build's W / Dbl at the same lambda (ba_cov.cu)
+void launch_point_cov(const BaDev& d, const double* Z, double lambda, double* out, cudaStream_t st);
 }  // namespace svs
