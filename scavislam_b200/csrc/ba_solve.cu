@@ -40,7 +40,7 @@ namespace cg = cooperative_groups;
 namespace svs {
 
 constexpr int kSolveThreads = 384;               // 12 warps; warp w issues from scheduler w % 4
-// Roles (factor_range).  Eight working warps, two per scheduler (warps 8-11 idle through the factorisation): what bounds
+// Roles (factor_range).  Ten working warps (warps 8 and 11 idle through the factorisation): what bounds
 // the helpers is the number of instructions their schedulers must issue per column (sixteen resident warps that all
 // walked the column loop spent most of their issue slots on loop skeletons) and the FP64 pipe of a scheduler (two
 // unit warps on one scheduler double the FMA phase).  Alternatives that were tried, fastest first:
@@ -51,19 +51,22 @@ constexpr int kSolveThreads = 384;               // 12 warps; warp w issues from
 //   three unit warps, left-over units on the second row warp
 constexpr int kChainWarp = 0;
 constexpr int kUnitWarps = 4;                    // warps 1-4: quarter-block units of the trailing update
-constexpr int kRowWarps = 2;                     // warps 5, 6: rows of the column, N rows, right-hand side
+constexpr int kRowWarps = 2;                     // warps 5, 6: rows of the column, right-hand side
 constexpr int kUrgentWarp = 7;                   // the two pair updates the chain reads next
+constexpr int kNWarps = 2;                       // warps 9, 10: N rows for the backward pass (same schedulers as the row
+                                                 // warps, so the instructions per scheduler hardly change)
 __device__ __forceinline__ int unit_warp_index(int w) { return (w >= 1 && w <= 4) ? w - 1 : -1; }
 __device__ __forceinline__ int row_warp_index(int w) { return w == 5 ? 0 : (w == 6 ? 1 : -1); }
-constexpr int kUnitThreads = kUnitWarps * 32, kRowThreads = kRowWarps * 32;
-constexpr int kPubAll = 32 * (1 + kUnitWarps + kRowWarps + 1);   // chain + unit + row + urgent warps
-constexpr int kRowsAll = 32 * (kUnitWarps + kRowWarps + 1);      // unit warps wait, row warps produce and wait, urgent produces
-constexpr int kRefillAll = 32 * (kUnitWarps + kRowWarps);       // the urgent warp only touches the next two columns: resident
+__device__ __forceinline__ int n_warp_index(int w) { return w == 9 ? 0 : (w == 10 ? 1 : -1); }
+constexpr int kUnitThreads = kUnitWarps * 32, kRowThreads = kRowWarps * 32, kNThreads = kNWarps * 32;
+constexpr int kPubAll = 32 * (1 + kUnitWarps + kRowWarps + 1 + kNWarps);   // chain + unit + row + urgent + N warps
+constexpr int kRowsAll = 32 * (kUnitWarps + kRowWarps + 1 + kNWarps);      // unit, row and N warps wait, row warps and urgent produce
+constexpr int kRefillAll = 32 * (kUnitWarps + kRowWarps + kNWarps);       // the urgent warp only touches the next two columns: resident
 constexpr int kUnitStride = kUnitThreads;
 constexpr int kBarPub = 1;    // chain arrives, helpers + urgent warp sync: column j's diagonal factor is published
 constexpr int kBarUrg = 2;    // urgent warp arrives, chain syncs: the chain's next inputs are up to date
 constexpr int kBarH = 3;      // all rows of the column are scaled (row + urgent warps produce, unit + row warps wait)
-constexpr int kBarH2 = 5;     // unit + row warps (ring refill)
+constexpr int kBarH2 = 5;     // unit + row + N warps (ring refill)
 constexpr int kBarBack = 4;   // backward pass, all threads of the CTA
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
@@ -266,8 +269,8 @@ __device__ __forceinline__ void ring_refill(const BaDev& d, const Team& T, const
 //                          (j+2, j) in a window, and applies the two pair updates the chain is going to read next
 //                          -- D_{j+2} and S_{j+2,j+1} -- then signals (kBarUrg, arrive); less work than the
 //                          chain's own column;
-//   general helpers        everything else of column j: the other rows (L_ij), the other pair updates, the
-//                          right-hand side, N_ij for the backward pass.  They re-join the chain only through kBarPub, one
+//   general helpers        everything else of column j: the other rows (L_ij) and the right-hand side (row warps), the
+//                          other pair updates (unit warps), N_ij for the backward pass (N warps).  They re-join the chain only through kBarPub, one
 //                          column later; since every helper must arrive there, "column j published" also means
 //                          "all of column j-1 applied".
 // kDiag: the chain warp also stores L_jj^-1 of every column it factors into d.Linv (row-major, zero above the
@@ -523,7 +526,7 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
       for (int i = 0; i < 4; ++i) T.prof[4 + i] = ph[i];
 #undef PHL
   } else if (row_warp_index(warp) >= 0) {
-    // ------------------------------------------------------------------ row warps: L rows, N rows, right-hand side
+    // ------------------------------------------------------------------ row warps: L rows, right-hand side
     const int rt = row_warp_index(warp) * 32 + lane;
     int until_refill = T.refill_period;
     long long ph[5] = {0, 0, 0, 0, 0}, pt = T.prof ? clock64() : 0;
@@ -559,28 +562,6 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
       PHL(1);
       bar_sync(kBarH, kRowsAll);
       if (T.prof && *reinterpret_cast<volatile int*>(&S.fail[T.slot][j & 1]) >= 0) PHL(2);
-      // ---- N_ij = L_ij L_jj^-1 (and z_j = y_j L_jj^-1) for the backward pass, stored transposed in row-major order;
-      //      nothing in the forward pass waits for it
-      for (int row = rt; row < nrows; row += kRowThreads) {
-        const double* src;
-        double* gdst;
-        int gstride;
-        if (row < nb * 6) {
-          const int a = row / 6, rr = row - a * 6;
-          src = sm_solve + ring_idx(T, base + 1 + a) + rr * 6;
-          gdst = d.Nrow + (size_t)__ldg(d.rowpos + base + 1 + a) * 36 + rr;   // transposed inside the block
-          gstride = 6;
-        } else {
-          src = sm_solve + S.yv_off + 6 * j;
-          gdst = d.ywork + 6 * (size_t)j;
-          gstride = 1;
-        }
-        double o[6], n[6];
-        load_row6(src, o);
-        row_bwd(o, L_, L_ + 21, n);
-#pragma unroll
-        for (int q = 0; q < 6; ++q) gdst[q * gstride] = n[q];
-      }
       // ---- b_a -= L_aj y_j
       for (int w = rt; w < nb * 6; w += kRowThreads) {
         const int a = w / 6, rr = w - a * 6;
@@ -596,6 +577,53 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
     if (T.prof && rt == 0)
       for (int i = 0; i < 4; ++i) T.prof[8 + i] = ph[i];
 #undef PHL
+  } else if (n_warp_index(warp) >= 0) {
+    // ------------------------------------------------------------------ N warps: the folded factor for the backward pass
+    // N_ij = L_ij L_jj^-1 (and z_j = y_j L_jj^-1), stored transposed in row-major order.  Nothing in the forward pass
+    // waits for it, but every helper must be through a column before kBarPub opens for the next one: on warps of their
+    // own these rows run beside the row warps' right-hand side instead of in front of it.
+    const int nt = n_warp_index(warp) * 32 + lane;
+    int until_refill = T.refill_period;
+    for (int j = T.j0; j < T.j1; ++j) {
+      const int base = col_ptr[j], nb = col_ptr[j + 1] - base - 1;
+      const int nrows = nb * 6 + 1;
+      const double* sl = S.sL[T.slot][j & 1];
+      const int* pfail = &S.fail[T.slot][j & 1];
+      bar_sync(kBarPub, kPubAll);
+      // row-major position of the block of this thread's first row: a global load (an L2 round trip), in flight while
+      // the rows are scaled.  Not issued before the barrier: its release would wait for it
+      const int rpos0 = nt < nb * 6 ? __ldg(d.rowpos + base + 1 + nt / 6) : 0;
+      if (*pfail) break;
+      double L_[28];
+      {
+        const double2* l2 = reinterpret_cast<const double2*>(sl);
+#pragma unroll
+        for (int q = 0; q < 14; ++q) { const double2 t2 = l2[q]; L_[2 * q] = t2.x; L_[2 * q + 1] = t2.y; }
+      }
+      bar_sync(kBarH, kRowsAll);   // the column's rows are scaled
+      for (int row = nt; row < nrows; row += kNThreads) {
+        const double* src;
+        double* gdst;
+        int gstride;
+        if (row < nb * 6) {
+          const int a = row / 6, rr = row - a * 6;
+          src = sm_solve + ring_idx(T, base + 1 + a) + rr * 6;
+          const int rp = row == nt ? rpos0 : __ldg(d.rowpos + base + 1 + a);
+          gdst = d.Nrow + (size_t)rp * 36 + rr;   // transposed inside the block
+          gstride = 6;
+        } else {
+          src = sm_solve + S.yv_off + 6 * j;
+          gdst = d.ywork + 6 * (size_t)j;
+          gstride = 1;
+        }
+        double o[6], n[6];
+        load_row6(src, o);
+        row_bwd(o, L_, L_ + 21, n);
+#pragma unroll
+        for (int q = 0; q < 6; ++q) gdst[q * gstride] = n[q];
+      }
+      ring_refill(d, T, col_ptr, blk_end, j, kUnitThreads + kRowThreads + nt, until_refill, hi);
+    }
   }
   __threadfence();   // N blocks and z (global) before the backward pass streams them back
   __syncthreads();
