@@ -102,6 +102,25 @@ int svs_ba_set_problem(svs_ba *h, int P, const double *T_qt, const unsigned char
                        int C, const int *c_i, const int *c_j, const double *c_T_ji,
                        const double *c_Lambda, const svs_cam *cam);
 
+/* svs_ba_set_problem for a window that already lies in GPU memory (assembled by CUDA code or held in
+ * PyTorch tensors): the same arguments, but every array is a device pointer on the handle's device
+ * (fixed may be NULL).  The structure analysis -- validation, grouping per landmark, the internal
+ * landmark order, track padding, the build work lists and the co-visibility pattern -- runs on the
+ * device; only a few counts and the P x P pattern (P*P/8 bytes) come back for the symbolic
+ * factorisation.  Same return codes and svs_last_error texts as svs_ba_set_problem.
+ *   A host pointer or memory of another device gives SVS_ERR_INVALID before anything is enqueued.
+ *   The arrays are read on the handle's stream, which does not wait for other streams: the caller
+ *   must have finished producing them (e.g. synchronised its own stream) before the call.  They may
+ *   be reused or freed once the call returns.
+ *   Calling it again with index arrays equal to the last device problem's re-sends only the numbers,
+ *   device to device. */
+int svs_ba_set_problem_device(svs_ba *h, int P, const double *T_qt, const unsigned char *fixed,
+                              int L, const double *psi,
+                              int E, const int *e_point, const int *e_pose, const int *e_anchor,
+                              const double *e_obs, const double *e_info_diag,
+                              int C, const int *c_i, const int *c_j, const double *c_T_ji,
+                              const double *c_Lambda, const svs_cam *cam);
+
 /* Replaces optimizer.initializeOptimization(); lm->setUserLambdaInit(lambda);
  * optimizer.optimize(num_iters) (slam_graph.cpp:336-346) with RobustKernelHuber(delta) on the
  * observation edges when `robust` (slam_graph-impl.cpp:86-90; the reference leaves delta = 1).

@@ -156,7 +156,7 @@ EXPORTS = [
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
-    "svs_ba_covariance",
+    "svs_ba_covariance", "svs_ba_set_problem_device",
 ]
 
 
@@ -186,6 +186,8 @@ def lib():
     prob = [C.c_int, c_dp, c_up, C.c_int, c_dp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp,
             C.c_int, c_ip, c_ip, c_dp, c_dp, C.POINTER(SvsCam)]
     L.svs_ba_set_problem.argtypes = [vp] + prob
+    L.svs_ba_set_problem_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp,
+                                            C.c_int, vp, vp, vp, vp, C.POINTER(SvsCam)]
     L.svs_ba_optimize.argtypes = [vp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_int, C.POINTER(SvsBaStats)]
     L.svs_ba_get_poses.argtypes = [vp, c_dp]
     L.svs_ba_get_points.argtypes = [vp, c_dp]
@@ -340,6 +342,11 @@ def _ip(a):
     return a.ctypes.data_as(c_ip)
 
 
+def _is_torch_tensor(a):
+    t = type(a)
+    return t.__module__.startswith("torch") and t.__name__ == "Tensor"
+
+
 class SvsError(RuntimeError):
     def __init__(self, rc, msg):
         super().__init__(f"svs error {rc}: {msg}")
@@ -391,11 +398,45 @@ class BundleAdjuster:
                 pb.E, _ip(k["e_point"]), _ip(k["e_pose"]), _ip(k["e_anchor"]), _dp(k["e_obs"]), _dp(k["e_info"]),
                 pb.C, _ip(k["c_i"]), _ip(k["c_j"]), _dp(k["c_T"]), _dp(k["c_Lambda"]), C.byref(cam)], cam
 
+    _DEVICE_ARRAYS = (("pose_qt", "float64"), ("fixed", "uint8"), ("psi", "float64"), ("e_point", "int32"),
+                      ("e_pose", "int32"), ("e_anchor", "int32"), ("e_obs", "float64"), ("e_info", "float64"),
+                      ("c_i", "int32"), ("c_j", "int32"), ("c_T", "float64"), ("c_Lambda", "float64"))
+
     def set_problem(self, pb):
-        k = self._arrays(pb)
-        args, cam = self._prob_args(pb, k)
-        self._check(lib().svs_ba_set_problem(self._h, *args))
+        """Load a window.  Its arrays are numpy arrays, or CUDA torch tensors on the handle's device (int32 indices,
+        uint8 fixed flags or None, float64 numbers): then the window never passes through the host and its structure
+        is analysed on the device (svs_ba_set_problem_device).  The current torch stream is synchronised first."""
+        if any(_is_torch_tensor(getattr(pb, name)) for name, _ in self._DEVICE_ARRAYS):
+            self._set_problem_device(pb)
+        else:
+            k = self._arrays(pb)
+            args, cam = self._prob_args(pb, k)
+            self._check(lib().svs_ba_set_problem(self._h, *args))
         self.P, self.L = pb.P, pb.L
+
+    def _set_problem_device(self, pb):
+        import torch
+        ptr, keep, dev = {}, [], None
+        for name, dtype in self._DEVICE_ARRAYS:
+            t = getattr(pb, name)
+            if name == "fixed" and t is None:
+                ptr[name] = None
+                continue
+            if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == getattr(torch, dtype)):
+                raise TypeError(f"{name}: a CUDA {dtype} tensor (all arrays of a device problem are)")
+            if dev is not None and t.device != dev:
+                raise ValueError(f"{name}: on {t.device}, the other arrays on {dev}")
+            dev = t.device
+            t = t.contiguous()
+            keep.append(t)
+            ptr[name] = t.data_ptr() if t.numel() else None
+        cam = SvsCam(float(pb.cam[0]), float(pb.cam[1]), float(pb.cam[2]), float(pb.cam[3]))
+        torch.cuda.current_stream(dev).synchronize()   # the handle reads the arrays on its own stream
+        p = ptr
+        self._check(lib().svs_ba_set_problem_device(
+            self._h, int(pb.P), p["pose_qt"], p["fixed"], int(pb.L), p["psi"], int(pb.E), p["e_point"], p["e_pose"],
+            p["e_anchor"], p["e_obs"], p["e_info"], int(pb.C), p["c_i"], p["c_j"], p["c_T"], p["c_Lambda"],
+            C.byref(cam)))
 
     def optimize(self, num_iters, robust=True, huber_delta=1.0, lambda_init=50.0, max_trials=5):
         st = SvsBaStats()

@@ -24,6 +24,8 @@
 
 #include "../../include/svs_b200.h"
 #include "ba_kernels.cuh"
+#include "ba_rules.cuh"
+#include "ba_structure.cuh"
 #include "grow.cuh"
 #include "nccl_dyn.cuh"
 #include "host_pool.hpp"
@@ -133,7 +135,15 @@ struct svs_ba {
   std::vector<int> k_epoint, k_epose, k_eanchor, k_ci, k_cj, k_extra;
   std::vector<unsigned char> k_fixed;
   int k_P = -1, k_L = -1, k_E = -1, k_C = -1, k_flags = 0;
+  bool k_on_device = false;   // the last structure came as device arrays: its index arrays are kept in d_keep
   size_t off_num = 0, off_cT = 0, off_cLam = 0, off_pose0 = 0, off_psi0 = 0, upload_bytes = 0;
+  size_t off_sym = 0, off_sym_end = 0;   // the symbolic arrays in the arena: all a device set-up uploads
+  // device set-up (svs_ba_set_problem_device, svs_ba_set_problem_from_map): the analysis' scratch, its readback
+  // (pinned), the last structure's index arrays e_point | e_pose | e_anchor | c_i | c_j | fixed
+  char* d_scr = nullptr; size_t scr_cap = 0;
+  char* h_rb = nullptr; size_t rb_cap = 0;
+  char* d_keep = nullptr; size_t keep_cap = 0;
+  bool lm_user_stale = false;   // lm_to_user is only on the device (d.lm_user) after a device set-up
   int reuse_hits = 0;
   // symbolic factorisation of the last pose graph: reused while the co-visibility pattern (P x P) stays the same,
   // which it does from tick to tick unless a keyframe enters or leaves the double window
@@ -213,6 +223,10 @@ void free_arena(svs_ba* h) {
   if (h->d_raw) cudaFree(h->d_raw);
   if (h->h_raw) cudaFreeHost(h->h_raw);
   h->d_raw = h->h_raw = nullptr; h->raw_cap = 0;
+  if (h->d_scr) cudaFree(h->d_scr);
+  if (h->h_rb) cudaFreeHost(h->h_rb);
+  if (h->d_keep) cudaFree(h->d_keep);
+  h->d_scr = h->h_rb = h->d_keep = nullptr; h->scr_cap = h->rb_cap = h->keep_cap = 0;
   h->arena = nullptr; h->stage = nullptr; h->arena_cap = h->stage_cap = 0;
 }
 
@@ -367,17 +381,6 @@ int choose_branches(int P, const std::vector<std::vector<int>>& adj, std::vector
   return 2;
 }
 
-// Track padding rule (set_problem_impl, 'Track padding'): a track of m >= 2 non-anchor observers lo..hi is completed
-// with zero-weight edges to the np frames of lo..hi it skips (the anchor frame is never one of them) when the completed
-// track has at most 8 slots and np <= max(1, m / 2).  Returns np (0: leave the track as it is).  The sharded window
-// uses the same rule for the block pattern every rank must agree on.
-inline int track_padding(int m, int lo, int hi, int anchor) {
-  if (m < 2) return 0;
-  const int span = hi - lo + 1 - ((anchor > lo && anchor < hi) ? 1 : 0);   // frames lo..hi without the anchor
-  const int np = span - m;
-  return (np > 0 && 1 + span <= 8 && np <= std::max(1, m / 2)) ? np : 0;
-}
-
 int fail(svs_ba* h, int code, const std::string& msg) {
   h->err = msg;
   return code;
@@ -496,6 +499,146 @@ static int finish_problem(svs_ba* h, size_t from, const double* d_obs_info, bool
   return svs_ba_reset_state(h);
 }
 
+// The pose graph of the reduced system from its P x P byte pattern h->w_adj (co-visibility, constraints, prescribed
+// pairs) and its symbolic analysis, reused while the pattern stays the same.  Sets h->nnzb_S, nbranch and nsep_blk.
+static int analyse_pattern(svs_ba* h, int P, Symbolic& sy) {
+  std::vector<std::vector<int>> adj(P);
+  int nnz = 0;
+  for (int i = 0; i < P; ++i) {
+    const unsigned char* row = h->w_adj.data() + (size_t)i * P;
+    for (int j = 0; j < P; ++j)
+      if (row[j] && j != i) adj[i].push_back(j);
+    nnz += (int)adj[i].size();
+  }
+  h->nnzb_S = nnz / 2 + P;
+  const bool natural_order = (h->flags & SVS_BA_NATURAL_ORDER) != 0;
+  const bool chain_only = getenv("SVS_SOLVE_CHAIN") != nullptr;
+  if (h->k_adjP == P && h->k_natural == natural_order && !chain_only &&
+      h->k_adj.size() == h->w_adj.size() && memcmp(h->k_adj.data(), h->w_adj.data(), h->w_adj.size()) == 0) {
+    sy = h->k_sy;
+    h->nbranch = h->k_nbranch; h->nsep_blk = h->k_nsep;
+    ++h->symbolic_hits;
+  } else {
+    // two concurrent branches when the window is banded and each team's share of k_solve's
+    // shared-memory ring holds its widest columns, else a single chain (minimum degree order)
+    const bool natural = natural_order;
+    int G = (natural || chain_only) ? 1 : 2;
+    for (;;) {
+      std::vector<int> order, bptr;
+      G = G > 1 ? choose_branches(P, adj, order, bptr) : 1;
+      analyse(P, adj, natural, order, sy);
+      if (G == 1) { sy.branch_ptr = {0, P}; h->nsep_blk = 0; }
+      else sy.branch_ptr = bptr;
+      const int sep0 = sy.branch_ptr[G];
+      sy.max_col_branch = sy.max_col_sep = 0;
+      for (int j = 0; j < P; ++j) {
+        const int nb = sy.col_ptr[j + 1] - sy.col_ptr[j] - 1;
+        if (G > 1 && j < sep0) sy.max_col_branch = std::max(sy.max_col_branch, nb);
+        else sy.max_col_sep = std::max(sy.max_col_sep, nb);
+      }
+      if (G == 1) break;
+      // each end of the window is factored by its own CTA: its ring must hold four of the widest columns
+      const int nsep = sy.nblk - sy.col_ptr[sep0];
+      const int cap = solve_ring_capacity(P, sy.nblk, nsep);
+      if (cap >= 4 * (sy.max_col_branch + 1) && cap / 2 >= sy.max_col_sep + 2) { h->nsep_blk = nsep; break; }
+      G /= 2;
+    }
+    h->nbranch = (int)sy.branch_ptr.size() - 1;
+    if (!chain_only) { h->k_sy = sy; h->k_adj = h->w_adj; h->k_adjP = P; h->k_natural = natural_order; h->k_nbranch = h->nbranch; h->k_nsep = h->nsep_blk; }
+  }
+  if (sy.nblk >= (1 << 20)) return fail(h, SVS_ERR_UNSUPPORTED, "reduced system factor has more than 2^20 blocks");
+  return SVS_OK;
+}
+
+// Host sources of the constant arrays of the device image.  nullptr: the array is produced on the device (a device
+// set-up) and only its place in the arena is reserved.
+struct LaySrc {
+  const unsigned char* fixed = nullptr;
+  const int* lm_eptr = nullptr; const int* lm_sptr = nullptr; const int* lm_anchor = nullptr;
+  const unsigned char* lm_self = nullptr; const int* lm_user = nullptr;
+  const int* e_pose = nullptr; const int* edge_src = nullptr;
+  const int* task_lm = nullptr; const int* task_cnt = nullptr; const int* gen_lm = nullptr; const int* long_lm = nullptr;
+  const int* col_need = nullptr; const int* c_i = nullptr; const int* c_j = nullptr;
+  const double* c_T = nullptr; const double* c_Lam = nullptr; const double* pose0 = nullptr; const double* psi0 = nullptr;
+};
+
+// Device image of the problem in h->d (sizes set by the caller): the constant arrays (the uploaded ones mirrored in the
+// staging buffer) followed by the work buffers.  With h->measuring only h->arena_off advances.
+static void lay(svs_ba* h, const Symbolic& sy, const LaySrc& s, const double** d_pose0, const double** d_psi0) {
+  BaDev& d = h->d;
+  const int P = d.P, L = d.L, C = d.C, ne = d.E, ns = d.nslots;
+  h->arena_off = 0;
+  auto put = [&](auto& field, auto src, size_t n) {
+    if (src) dev_upload(h, &field, src, n);
+    else dev_alloc(h, &field, n);
+  };
+  put(d.fixed, s.fixed, P); put(d.lm_eptr, s.lm_eptr, (size_t)L + 1); put(d.lm_sptr, s.lm_sptr, (size_t)L + 1);
+  put(d.lm_anchor, s.lm_anchor, L); put(d.lm_self, s.lm_self, L); put(d.lm_user, s.lm_user, L);
+  put(d.e_pose, s.e_pose, ne); put(d.edge_src, s.edge_src, ne);
+  put(d.task_lm, s.task_lm, d.ntasks); put(d.task_cnt, s.task_cnt, d.ntasks); put(d.gen_lm, s.gen_lm, d.ngen);
+  put(d.long_lm, s.long_lm, d.nlong);
+  h->off_sym = h->arena_off;
+#define UP(field, vec) dev_upload(h, &d.field, vec)
+  UP(tbl, sy.tbl); UP(perm, sy.perm); UP(pos, sy.pos); UP(col_ptr, sy.col_ptr); UP(row_idx, sy.row_idx);
+  UP(upd_ptr, sy.upd_ptr); UP(upd_dst, sy.upd_dst); UP(upd_ab, sy.upd_ab); UP(urg_dst, sy.urg_dst);
+  UP(branch_ptr, sy.branch_ptr); UP(rptr, sy.rptr); UP(rowpos, sy.rowpos); UP(rcol, sy.rcol);
+#undef UP
+  h->off_sym_end = h->arena_off;
+  put(d.col_need, s.col_need, P);
+  put(d.c_i, s.c_i, C); put(d.c_j, s.c_j, C);
+  h->off_num = h->off_cT = h->arena_off;   // the numbers (everything a same-structure call re-sends) lie last
+  put(d.c_T, s.c_T, 7 * (size_t)C);
+  h->off_cLam = h->arena_off;
+  put(d.c_Lam, s.c_Lam, 36 * (size_t)C);
+  h->off_pose0 = h->arena_off;
+  put(*d_pose0, s.pose0, 7 * (size_t)P);
+  h->off_psi0 = h->arena_off;
+  put(*d_psi0, s.psi0, 3 * (size_t)L);
+  h->upload_bytes = h->arena_off;
+#define AL(field, n) dev_alloc(h, &d.field, (size_t)(n))
+  for (int b = 0; b < 2; ++b) { AL(pose[b], 7 * (size_t)P); AL(Rt[b], 12 * (size_t)P); AL(psi[b], 3 * (size_t)L); }
+  AL(e_obs_w, 3 * (size_t)ne); AL(e_w_w, 3 * (size_t)ne);
+  AL(W, 18 * (size_t)ns); AL(Dbl, 12 * (size_t)L); AL(chi_l, L); AL(chi_new_l, L); AL(scale_l, L);
+  {   // reduced system S | bp | bc | totals in ONE buffer: a sharded window sums it with a single all-reduce
+    double* sys = nullptr;
+    dev_alloc(h, &sys, 36 * (size_t)sy.nblk + 12 * (size_t)P + 4);
+    if (!h->measuring) { d.S = sys; d.bp = sys + 36 * (size_t)sy.nblk; d.bc = d.bp + 6 * (size_t)P; d.totals = d.bc + 6 * (size_t)P; }
+    h->sys_count = 36 * (size_t)sy.nblk + 12 * (size_t)P;
+  }
+  AL(x, 6 * (size_t)P); AL(Nrow, 36 * (size_t)std::max(sy.nblk - P, 1));
+  AL(chi_c, C); AL(chi_c_new, C); AL(Linv, 36 * (size_t)P); AL(ywork, 6 * (size_t)P);
+  AL(ctl, 1);
+  AL(part, 3 * (size_t)update_grid_blocks(L, C)); AL(ticket, 4); AL(dbg, 160 + 2 * (size_t)P + 2); AL(col_done, P);
+#undef AL
+}
+
+// lay() twice: sizes, then the arena and the staging buffer grown to them, then the pointers (and staged uploads)
+static int lay_arena(svs_ba* h, const Symbolic& sy, const LaySrc& s) {
+  const double* d_pose0c = nullptr;
+  const double* d_psi0c = nullptr;
+  h->measuring = true;
+  lay(h, sy, s, &d_pose0c, &d_psi0c);
+  h->measuring = false;
+  CK(grow(h->arena_off, &h->arena_cap, &h->arena));
+  CK(grow<char>(h->upload_bytes, &h->stage_cap, nullptr, &h->stage));
+  lay(h, sy, s, &d_pose0c, &d_psi0c);
+  h->d_pose0 = const_cast<double*>(d_pose0c);
+  h->d_psi0 = const_cast<double*>(d_psi0c);
+  return SVS_OK;
+}
+
+// The rest of a new structure, shared by both set-ups: state pointers, solver widths, counts and the structure key.
+static void adopt_structure(svs_ba* h, const Symbolic& sy, int Kmax, int Kmax_gen, int P, int L, int E, int C) {
+  BaDev& d = h->d;
+  d.e_obs = d.e_obs_w; d.e_w = d.e_w_w;
+  h->solve_col_branch = sy.max_col_branch; h->solve_col_sep = std::max(sy.max_col_sep, sy.max_row - 2);
+  d.nbranch = h->nbranch;
+  h->Kmax = Kmax;
+  h->Kmax_gen = Kmax_gen;
+  h->has_problem = true;
+  h->k_P = P; h->k_L = L; h->k_E = E; h->k_C = C; h->k_flags = h->flags; h->k_extra = h->extra_pairs;
+}
+
 // d_obs_info != nullptr: the observations [E][3] followed by the weights [E][3] already lie on this device in
 // the caller's edge order (assembled there, svs_ba_set_problem_from_map) and e_obs / e_info are not read.
 static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi,
@@ -518,7 +661,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   CK(cudaStreamSynchronize(h->stream));   // the arena and the staging buffer are about to be reused
   const bool host_timing = getenv("SVS_HOST_TIMING") != nullptr;
   // ---- same structure as the problem on the device: only the numbers travel
-  if (h->has_problem && P == h->k_P && L == h->k_L && E == h->k_E && C == h->k_C &&
+  if (h->has_problem && !h->k_on_device && P == h->k_P && L == h->k_L && E == h->k_E && C == h->k_C &&
       h->flags == h->k_flags && h->extra_pairs == h->k_extra &&
       (E == 0 || (memcmp(e_point, h->k_epoint.data(), sizeof(int) * E) == 0 && memcmp(e_pose, h->k_epose.data(), sizeof(int) * E) == 0 &&
                   memcmp(e_anchor, h->k_eanchor.data(), sizeof(int) * E) == 0)) &&
@@ -704,11 +847,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
       }
       l_anchor[l] = anchor; l_self[l] = (unsigned char)nself; l_K[l] = K;
       Kmax = std::max(Kmax, K);
-      // locality key: track shape (self flag, length, first and last observer) inside an anchor, so that
-      // neighbouring warps of the fused kernel scatter into the same blocks of the reduced system
-      const unsigned long long first = (unsigned long long)(e_pose[eord[b + (nself ? 1 : 0) < en ? b + (nself ? 1 : 0) : b]] & 0xfffff);
-      const unsigned long long last = (unsigned long long)(e_pose[eord[en - 1]] & 0xfffff);
-      key[l] = ((unsigned long long)(nself ? 0 : 1) << 61) | ((unsigned long long)(K & 0xfffff) << 40) | (first << 20) | last;
+      key[l] = locality_key(nself, K, e_pose[eord[b + (nself ? 1 : 0) < en ? b + (nself ? 1 : 0) : b]], e_pose[eord[en - 1]]);
     }
     c_kmax[ck] = Kmax; c_bad[ck] = bad;
   });
@@ -781,13 +920,9 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   std::vector<int> task_lm, task_cnt, gen_lm, long_lm;   // long_lm: more than kMaxTrack slots (streaming kernel, any length)
   int Kmax_gen = 1;
   {
-    // landmarks per task: about eleven tasks per SM, so that the persistent grid's tail stays short while coarser
-    // tasks flush their accumulators less often; clamped to [4, 32]
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
-    int chunk = L / (std::max(sms, 1) * 11);
-    chunk = chunk < 4 ? 4 : (chunk > 32 ? 32 : chunk);
-    if (const char* cs = getenv("SVS_BUILD_CHUNK")) chunk = std::max(1, atoi(cs));   // tuning knob, at least one landmark per task
+    const int chunk = build_chunk(L, sms);
     auto same_slots = [&](int la, int lb) {   // internal indices
       const int ka = lm_eptr[la + 1] - lm_eptr[la], kb = lm_eptr[lb + 1] - lm_eptr[lb];
       if (ka != kb || lm_anchor[la] != lm_anchor[lb] || lm_self[la] != lm_self[lb]) return false;
@@ -828,14 +963,11 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
     // sort by waves, descending (landmark order inside a class is kept for the locality of the scatter)
     if (task_lm.size() > 1) {
       const size_t nt_all = task_lm.size();
-      constexpr int kMaxWaves = 64;
       std::vector<unsigned char> wv(nt_all);
       int hist[kMaxWaves + 1] = {};
       for (size_t t = 0; t < nt_all; ++t) {
-        const int li = task_lm[t], cnt = task_cnt[t];
-        const int kk = lm_eptr[li + 1] - lm_eptr[li], KK = lm_sptr[li + 1] - lm_sptr[li];
-        const int nw_max = std::max(1, std::min(std::min(32 / std::max(kk, 1), 40 / std::max(KK, 1)), 8));
-        const int waves = std::min((cnt + nw_max - 1) / nw_max, kMaxWaves);
+        const int li = task_lm[t];
+        const int waves = task_waves(lm_eptr[li + 1] - lm_eptr[li], lm_sptr[li + 1] - lm_sptr[li], task_cnt[t]);
         wv[t] = (unsigned char)waves;
         hist[waves]++;
       }
@@ -849,7 +981,6 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
 
   lap("tasks");
   // ---- pose graph of the reduced system: co-visibility (all pairs inside a track) + constraints
-  std::vector<std::vector<int>> adj(P);
   {
     auto& A = h->w_adj;
     A.assign((size_t)P * P, 0);
@@ -873,53 +1004,10 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
       if (a < 0 || b < 0 || a >= P || b >= P) return fail(h, SVS_ERR_INVALID, "structure pair out of range");
       if (a != b) { A[(size_t)a * P + b] = 1; A[(size_t)b * P + a] = 1; }
     }
-    int nnz = 0;
-    for (int i = 0; i < P; ++i) {
-      const unsigned char* row = A.data() + (size_t)i * P;
-      for (int j = 0; j < P; ++j)
-        if (row[j] && j != i) adj[i].push_back(j);
-      nnz += (int)adj[i].size();
-    }
-    h->nnzb_S = nnz / 2 + P;
   }
   lap("adjacency");
   Symbolic sy;
-  const bool natural_order = (h->flags & SVS_BA_NATURAL_ORDER) != 0;
-  const bool chain_only = getenv("SVS_SOLVE_CHAIN") != nullptr;
-  if (h->k_adjP == P && h->k_natural == natural_order && !chain_only &&
-      h->k_adj.size() == h->w_adj.size() && memcmp(h->k_adj.data(), h->w_adj.data(), h->w_adj.size()) == 0) {
-    sy = h->k_sy;
-    h->nbranch = h->k_nbranch; h->nsep_blk = h->k_nsep;
-    ++h->symbolic_hits;
-  } else {
-    // two concurrent branches when the window is banded and each team's share of k_solve's
-    // shared-memory ring holds its widest columns, else a single chain (minimum degree order)
-    const bool natural = natural_order;
-    int G = (natural || getenv("SVS_SOLVE_CHAIN")) ? 1 : 2;
-    for (;;) {
-      std::vector<int> order, bptr;
-      G = G > 1 ? choose_branches(P, adj, order, bptr) : 1;
-      analyse(P, adj, natural, order, sy);
-      if (G == 1) { sy.branch_ptr = {0, P}; h->nsep_blk = 0; }
-      else sy.branch_ptr = bptr;
-      const int sep0 = sy.branch_ptr[G];
-      sy.max_col_branch = sy.max_col_sep = 0;
-      for (int j = 0; j < P; ++j) {
-        const int nb = sy.col_ptr[j + 1] - sy.col_ptr[j] - 1;
-        if (G > 1 && j < sep0) sy.max_col_branch = std::max(sy.max_col_branch, nb);
-        else sy.max_col_sep = std::max(sy.max_col_sep, nb);
-      }
-      if (G == 1) break;
-      // each end of the window is factored by its own CTA: its ring must hold four of the widest columns
-      const int nsep = sy.nblk - sy.col_ptr[sep0];
-      const int cap = solve_ring_capacity(P, sy.nblk, nsep);
-      if (cap >= 4 * (sy.max_col_branch + 1) && cap / 2 >= sy.max_col_sep + 2) { h->nsep_blk = nsep; break; }
-      G /= 2;
-    }
-    h->nbranch = (int)sy.branch_ptr.size() - 1;
-    if (!chain_only) { h->k_sy = sy; h->k_adj = h->w_adj; h->k_adjP = P; h->k_natural = natural_order; h->k_nbranch = h->nbranch; h->k_nsep = h->nsep_blk; }
-  }
-  if (sy.nblk >= (1 << 20)) return fail(h, SVS_ERR_UNSUPPORTED, "reduced system factor has more than 2^20 blocks");
+  if (int rc = analyse_pattern(h, P, sy)) return rc;
 
   lap("analyse");
   // ---- column readiness (overlap timeline, SVS_SOLVE_TIMING=3): col_need[j] = the tasks whose slot list holds the pose
@@ -937,67 +1025,21 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   BaDev& d = h->d;
   d.P = P; d.L = L; d.E = ne; d.E_user = E; d.C = C; d.nslots = ns; d.nblk = sy.nblk; d.flags = h->flags;
   d.f = cam->f; d.px = cam->px; d.py = cam->py; d.b = cam->b;
+  d.ntasks = (int)task_lm.size(); d.ngen = (int)gen_lm.size(); d.nlong = (int)long_lm.size();
   std::vector<unsigned char> fx(P, 0);
   if (fixed) fx.assign(fixed, fixed + P);
-  const double* d_pose0c = nullptr;
-  const double* d_psi0c = nullptr;
-  size_t upload_bytes = 0;
-  auto lay = [&]() {
-    h->arena_off = 0;
-#define UP(field, vec) dev_upload(h, &d.field, vec)
-    UP(fixed, fx); UP(lm_eptr, lm_eptr); UP(lm_sptr, lm_sptr); UP(lm_anchor, lm_anchor); UP(lm_self, lm_self); UP(lm_user, h->lm_to_user);
-    UP(e_pose, ie_pose); UP(edge_src, edge_src);
-    UP(task_lm, task_lm); UP(task_cnt, task_cnt); UP(gen_lm, gen_lm); UP(long_lm, long_lm);
-    UP(tbl, sy.tbl); UP(perm, sy.perm); UP(pos, sy.pos); UP(col_ptr, sy.col_ptr); UP(row_idx, sy.row_idx);
-    UP(upd_ptr, sy.upd_ptr); UP(upd_dst, sy.upd_dst); UP(upd_ab, sy.upd_ab); UP(urg_dst, sy.urg_dst);
-    UP(branch_ptr, sy.branch_ptr); UP(rptr, sy.rptr); UP(rowpos, sy.rowpos); UP(rcol, sy.rcol); UP(col_need, col_need);
-    dev_upload(h, &d.c_i, c_i, (size_t)C); dev_upload(h, &d.c_j, c_j, (size_t)C);
-    h->off_num = h->off_cT = h->arena_off;   // the numbers (everything a same-structure call re-sends) lie last
-    dev_upload(h, &d.c_T, c_T, 7 * (size_t)C);
-    h->off_cLam = h->arena_off;
-    dev_upload(h, &d.c_Lam, c_Lambda, 36 * (size_t)C);
-    h->off_pose0 = h->arena_off;
-    dev_upload(h, &d_pose0c, T_qt, 7 * (size_t)P);
-    h->off_psi0 = h->arena_off;
-    dev_upload(h, &d_psi0c, ipsi.data(), 3 * (size_t)L);
-#undef UP
-    upload_bytes = h->arena_off;
-    h->upload_bytes = upload_bytes;
-#define AL(field, n) dev_alloc(h, &d.field, (size_t)(n))
-    for (int b = 0; b < 2; ++b) { AL(pose[b], 7 * (size_t)P); AL(Rt[b], 12 * (size_t)P); AL(psi[b], 3 * (size_t)L); }
-    AL(e_obs_w, 3 * (size_t)ne); AL(e_w_w, 3 * (size_t)ne);
-    AL(W, 18 * (size_t)ns); AL(Dbl, 12 * (size_t)L); AL(chi_l, L); AL(chi_new_l, L); AL(scale_l, L);
-    {   // reduced system S | bp | bc | totals in ONE buffer: a sharded window sums it with a single all-reduce
-      double* sys = nullptr;
-      dev_alloc(h, &sys, 36 * (size_t)sy.nblk + 12 * (size_t)P + 4);
-      if (!h->measuring) { d.S = sys; d.bp = sys + 36 * (size_t)sy.nblk; d.bc = d.bp + 6 * (size_t)P; d.totals = d.bc + 6 * (size_t)P; }
-      h->sys_count = 36 * (size_t)sy.nblk + 12 * (size_t)P;
-    }
-    AL(x, 6 * (size_t)P); AL(Nrow, 36 * (size_t)std::max(sy.nblk - P, 1));
-    AL(chi_c, C); AL(chi_c_new, C); AL(Linv, 36 * (size_t)P); AL(ywork, 6 * (size_t)P);
-    AL(ctl, 1);
-    AL(part, 3 * (size_t)update_grid_blocks(L, C)); AL(ticket, 4); AL(dbg, 160 + 2 * (size_t)P + 2); AL(col_done, P);
-#undef AL
-  };
-  h->measuring = true;
-  lay();
-  h->measuring = false;
-  CK(grow(h->arena_off, &h->arena_cap, &h->arena));
-  CK(grow<char>(upload_bytes, &h->stage_cap, nullptr, &h->stage));
-  lay();
+  LaySrc s;
+  s.fixed = fx.data(); s.lm_eptr = lm_eptr.data(); s.lm_sptr = lm_sptr.data(); s.lm_anchor = lm_anchor.data();
+  s.lm_self = lm_self.data(); s.lm_user = h->lm_to_user.data(); s.e_pose = ie_pose.data(); s.edge_src = edge_src.data();
+  s.task_lm = task_lm.data(); s.task_cnt = task_cnt.data(); s.gen_lm = gen_lm.data(); s.long_lm = long_lm.data();
+  s.col_need = col_need.data(); s.c_i = c_i; s.c_j = c_j; s.c_T = c_T; s.c_Lam = c_Lambda; s.pose0 = T_qt; s.psi0 = ipsi.data();
+  if (int rc = lay_arena(h, sy, s)) return rc;
   lap("stage");
   h->worker.wait();   // its DMA is in the stream ahead of everything enqueued below
   if (side.err != cudaSuccess) return fail(h, SVS_ERR_CUDA, cudaGetErrorString(side.err));
-  h->d_pose0 = const_cast<double*>(d_pose0c);
-  h->d_psi0 = const_cast<double*>(d_psi0c);
-  d.e_obs = d.e_obs_w; d.e_w = d.e_w_w;
-  h->solve_col_branch = sy.max_col_branch; h->solve_col_sep = std::max(sy.max_col_sep, sy.max_row - 2);
-  d.nbranch = h->nbranch;
-  h->Kmax = Kmax;
-  h->Kmax_gen = Kmax_gen;
-  d.ntasks = (int)task_lm.size(); d.ngen = (int)gen_lm.size(); d.nlong = (int)long_lm.size();
-  h->has_problem = true;
-  h->k_P = P; h->k_L = L; h->k_E = E; h->k_C = C; h->k_flags = h->flags; h->k_extra = h->extra_pairs;
+  adopt_structure(h, sy, Kmax, Kmax_gen, P, L, E, C);
+  h->k_on_device = false;
+  h->lm_user_stale = false;
   h->k_ci.assign(c_i, c_i + C); h->k_cj.assign(c_j, c_j + C);
   h->k_fixed = fx;
   return finish_problem(h, 0, d_obs_info, true);
@@ -1011,6 +1053,142 @@ int svs_ba_set_problem(svs_ba* h, int P, const double* T_qt, const unsigned char
   if (h) h->L_full = 0;
   return set_problem_impl(h, P, T_qt, fixed, L, psi, E, e_point, e_pose, e_anchor, e_obs, e_info, C, c_i, c_j, c_T, c_Lambda,
                           cam, nullptr);
+}
+
+// set_problem_impl for a problem whose arrays all lie on the handle's device: the structure analysis runs there
+// (ba_structure.cu) and one readback brings the counts, the error bits and the pose pattern for the symbolic analysis.
+// d_obs_info: as for set_problem_impl; without it e_obs and e_info (device) are copied into the handle's raw buffer.
+static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi, int E,
+                           const int* e_point, const int* e_pose, const int* e_anchor, const double* e_obs,
+                           const double* e_info, int C, const int* c_i, const int* c_j, const double* c_T,
+                           const double* c_Lambda, const svs_cam* cam, const double* d_obs_info) {
+  cudaSetDevice(h->device);
+  CK(cudaStreamSynchronize(h->stream));   // the scratch and the staging buffer are about to be reused
+  const cudaStream_t st = h->stream;
+  const bool host_timing = getenv("SVS_HOST_TIMING") != nullptr;
+  if (E > 0 && !d_obs_info) CK(grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+  StructIn in{};
+  in.P = P; in.L = L; in.E = E; in.C = C;
+  in.chunk = build_chunk(L, sms);
+  in.pad = getenv("SVS_BUILD_NO_PAD") == nullptr && !h->extra_pairs_from_caller;
+  in.e_point = e_point; in.e_pose = e_pose; in.e_anchor = e_anchor; in.c_i = c_i; in.c_j = c_j; in.fixed = fixed; in.psi = psi;
+  // the same structure as the problem on the device, if the index arrays say so (compared on the device)
+  in.compare = h->has_problem && h->k_on_device && P == h->k_P && L == h->k_L && E == h->k_E && C == h->k_C &&
+               h->flags == h->k_flags && h->extra_pairs == h->k_extra;
+  const int* keep = reinterpret_cast<const int*>(h->d_keep);
+  in.k_epoint = keep; in.k_epose = keep + E; in.k_eanchor = keep + 2 * (size_t)E; in.k_ci = keep + 3 * (size_t)E;
+  in.k_cj = keep + 3 * (size_t)E + C; in.k_fixed = reinterpret_cast<const unsigned char*>(keep + 3 * (size_t)E + 2 * (size_t)C);
+  StructOut so{};
+  CK(grow(launch_structure(in, nullptr, &so, st), &h->scr_cap, &h->d_scr));
+  launch_structure(in, h->d_scr, &so, st);
+  CK(grow<char>(so.readback_bytes, &h->rb_cap, nullptr, &h->h_rb));
+  CK(cudaMemcpyAsync(h->h_rb, so.hdr, so.readback_bytes, cudaMemcpyDeviceToHost, st));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  const StructHdr hd = *reinterpret_cast<const StructHdr*>(h->h_rb);
+  BaDev& d = h->d;
+  if (hd.err & kStructPairRange) return fail(h, SVS_ERR_INVALID, "pose-pose edge index out of range");
+  if (hd.diff == 0) {   // ---- same structure: only the numbers travel, device to device
+    d.f = cam->f; d.px = cam->px; d.py = cam->py; d.b = cam->b;
+    CopyList cl;
+    if (!d_obs_info) { cl.add(e_obs, h->d_raw, 24 * (size_t)E); cl.add(e_info, h->d_raw + 3 * (size_t)E, 24 * (size_t)E); }
+    cl.add(c_T, const_cast<double*>(d.c_T), 56 * (size_t)C);
+    cl.add(c_Lambda, const_cast<double*>(d.c_Lam), 288 * (size_t)C);
+    cl.add(T_qt, h->d_pose0, 56 * (size_t)P);
+    launch_copies(cl, st);
+    launch_psi_gather(psi, d.lm_user, L, h->d_psi0, st);
+    ++h->reuse_hits;
+    if (host_timing) fprintf(stderr, "set_problem_device: structure reused (%d)\n", h->reuse_hits);
+    return finish_problem(h, h->upload_bytes, d_obs_info, false);
+  }
+  free_problem(h);
+  if (hd.err & kStructEdgeRange) return fail(h, SVS_ERR_INVALID, "observation edge index out of range");
+  if (hd.err & kStructDuplicate) return fail(h, SVS_ERR_UNSUPPORTED, "a point is observed twice by the same frame");
+  if (hd.err & kStructAnchor) return fail(h, SVS_ERR_UNSUPPORTED, "edges of one point name different anchor frames");
+  // ---- pose pattern: the device's bitset as the byte matrix of the host analysis, plus svs_ba_set_structure's pairs
+  {
+    auto& A = h->w_adj;
+    A.assign((size_t)P * P, 0);
+    const int W = (P + 31) / 32;
+    const unsigned* bits = reinterpret_cast<const unsigned*>(h->h_rb + (reinterpret_cast<char*>(so.adj) - reinterpret_cast<char*>(so.hdr)));
+    for (int i = 0; i < P; ++i)
+      for (int w = 0; w < W; ++w)
+        for (unsigned x = bits[(size_t)i * W + w]; x; x &= x - 1) A[(size_t)i * P + 32 * w + __builtin_ctz(x)] = 1;
+    for (size_t q = 0; q + 1 < h->extra_pairs.size(); q += 2) {
+      const int a = h->extra_pairs[q], b = h->extra_pairs[q + 1];
+      if (a < 0 || b < 0 || a >= P || b >= P) return fail(h, SVS_ERR_INVALID, "structure pair out of range");
+      if (a != b) { A[(size_t)a * P + b] = 1; A[(size_t)b * P + a] = 1; }
+    }
+  }
+  Symbolic sy;
+  if (int rc = analyse_pattern(h, P, sy)) return rc;
+  d.P = P; d.L = L; d.E = hd.ne; d.E_user = E; d.C = C; d.nslots = hd.ns; d.nblk = sy.nblk; d.flags = h->flags;
+  d.f = cam->f; d.px = cam->px; d.py = cam->py; d.b = cam->b;
+  d.ntasks = hd.ntasks; d.ngen = hd.ngen; d.nlong = hd.nlong;
+  if (int rc = lay_arena(h, sy, LaySrc{})) return rc;   // every array but the symbolic ones comes from the device
+  CK(cudaMemcpyAsync(h->arena + h->off_sym, h->stage + h->off_sym, h->off_sym_end - h->off_sym, cudaMemcpyHostToDevice, st));
+  // the device's results into the arena, and this structure's index arrays into the copy the next call compares with
+  const size_t keep_bytes = 4 * (3 * (size_t)E + 2 * (size_t)C) + P;
+  CK(grow(keep_bytes, &h->keep_cap, &h->d_keep));
+  int* kp = reinterpret_cast<int*>(h->d_keep);
+  CopyList cl;
+  auto I = [](const int* p) { return const_cast<int*>(p); };
+  cl.add(so.fixed, const_cast<unsigned char*>(d.fixed), P);
+  cl.add(so.lm_eptr, I(d.lm_eptr), 4 * ((size_t)L + 1)); cl.add(so.lm_sptr, I(d.lm_sptr), 4 * ((size_t)L + 1));
+  cl.add(so.lm_anchor, I(d.lm_anchor), 4 * (size_t)L); cl.add(so.lm_self, const_cast<unsigned char*>(d.lm_self), L);
+  cl.add(so.lm_user, I(d.lm_user), 4 * (size_t)L);
+  cl.add(so.e_pose, I(d.e_pose), 4 * (size_t)d.E); cl.add(so.edge_src, I(d.edge_src), 4 * (size_t)d.E);
+  cl.add(so.task_lm, I(d.task_lm), 4 * (size_t)d.ntasks); cl.add(so.task_cnt, I(d.task_cnt), 4 * (size_t)d.ntasks);
+  cl.add(so.gen_lm, I(d.gen_lm), 4 * (size_t)d.ngen); cl.add(so.long_lm, I(d.long_lm), 4 * (size_t)d.nlong);
+  cl.add(c_i, I(d.c_i), 4 * (size_t)C); cl.add(c_j, I(d.c_j), 4 * (size_t)C);
+  cl.add(c_T, const_cast<double*>(d.c_T), 56 * (size_t)C); cl.add(c_Lambda, const_cast<double*>(d.c_Lam), 288 * (size_t)C);
+  cl.add(T_qt, h->d_pose0, 56 * (size_t)P); cl.add(so.psi, h->d_psi0, 24 * (size_t)L);
+  cl.add(e_point, kp, 4 * (size_t)E); cl.add(e_pose, kp + E, 4 * (size_t)E); cl.add(e_anchor, kp + 2 * (size_t)E, 4 * (size_t)E);
+  cl.add(c_i, kp + 3 * (size_t)E, 4 * (size_t)C); cl.add(c_j, kp + 3 * (size_t)E + C, 4 * (size_t)C);
+  cl.add(so.fixed, kp + 3 * (size_t)E + 2 * (size_t)C, P);
+  if (!d_obs_info) { cl.add(e_obs, h->d_raw, 24 * (size_t)E); cl.add(e_info, h->d_raw + 3 * (size_t)E, 24 * (size_t)E); }
+  launch_copies(cl, st);
+  CK(cudaMemsetAsync(I(d.col_need), 0, sizeof(int) * (size_t)std::max(P, 1), st));
+  launch_col_need(so, L, C, c_i, c_j, d.pos, I(d.col_need), st);
+  adopt_structure(h, sy, hd.Kmax, hd.Kmax_gen, P, L, E, C);
+  h->k_on_device = true;
+  const unsigned char* fx = reinterpret_cast<const unsigned char*>(h->h_rb + (so.fixed - reinterpret_cast<unsigned char*>(so.hdr)));
+  h->k_fixed.assign(fx, fx + P);
+  h->lm_to_user.clear();
+  h->lm_user_stale = true;
+  return finish_problem(h, h->upload_bytes, d_obs_info, true);
+}
+
+// true when p is device (or managed) memory of the handle's device
+static bool on_handle_device(const svs_ba* h, const void* p) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
+}
+
+int svs_ba_set_problem_device(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi,
+                              int E, const int* e_point, const int* e_pose, const int* e_anchor, const double* e_obs,
+                              const double* e_info, int C, const int* c_i, const int* c_j, const double* c_T,
+                              const double* c_Lambda, const svs_cam* cam) {
+  svs::NvtxRange nvtx_("copyDataToG2o");
+  if (!h) return SVS_ERR_INVALID;
+  if (P < 0 || L < 0 || E < 0 || C < 0 || !cam) return fail(h, SVS_ERR_INVALID, "negative size or null camera");
+  if ((P && !T_qt) || (L && !psi) || (E && (!e_point || !e_pose || !e_anchor || !e_obs || !e_info)) ||
+      (C && (!c_i || !c_j || !c_T || !c_Lambda)))
+    return fail(h, SVS_ERR_INVALID, "null array");
+  const void* arrays[] = {P ? T_qt : nullptr, P ? fixed : nullptr, L ? psi : nullptr, E ? e_point : nullptr,
+                          E ? e_pose : nullptr, E ? e_anchor : nullptr, E ? e_obs : nullptr, E ? e_info : nullptr,
+                          C ? c_i : nullptr, C ? c_j : nullptr, C ? c_T : nullptr, C ? c_Lambda : nullptr};
+  cudaSetDevice(h->device);
+  for (const void* p : arrays)
+    if (p && !on_handle_device(h, p)) return fail(h, SVS_ERR_INVALID, "an array is not device memory of the handle's device");
+  h->L_full = 0;
+  const int rc = set_problem_dev(h, P, T_qt, P ? fixed : nullptr, L, psi, E, e_point, e_pose, e_anchor, e_obs, e_info, C,
+                                 c_i, c_j, c_T, c_Lambda, cam, nullptr);
+  if (rc == SVS_OK) CK(cudaStreamSynchronize(h->stream));   // the caller's arrays may be reused now
+  return rc;
 }
 
 int svs_ba_reset_state(svs_ba* h) {
@@ -1229,7 +1407,12 @@ int svs_ba_get_points(svs_ba* h, double* psi) {
   const int L = h->d.L;
   std::vector<double> tmp(3 * (size_t)L);
   if (L) CK(cudaMemcpyAsync(tmp.data(), h->d.psi[h->h_ctl->cur],3 * (size_t)L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (h->lm_user_stale) {   // a device set-up left the landmark order on the device only
+    h->lm_to_user.resize(L);
+    if (L) CK(cudaMemcpyAsync(h->lm_to_user.data(), h->d.lm_user, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  }
   CK(cudaStreamSynchronize(h->stream));
+  h->lm_user_stale = false;
   // a sharded window (svs_ba_set_problem_sharded) addresses the caller's full-size array: only this rank's entries are written
   const size_t mul = h->L_full ? (size_t)h->comm_size : 1, add = h->L_full ? (size_t)h->comm_rank : 0;
   for (int li = 0; li < L; ++li)
@@ -1642,8 +1825,9 @@ namespace svs {
 int ba_set_problem_device_obs(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi, int E,
                               const int* e_point, const int* e_pose, const int* e_anchor, const double* d_obs_info, int C,
                               const int* c_i, const int* c_j, const double* c_T, const double* c_Lambda, const svs_cam* cam) {
-  const int rc = set_problem_impl(h, P, T_qt, fixed, L, psi, E, e_point, e_pose, e_anchor, nullptr, nullptr, C, c_i, c_j, c_T,
-                                  c_Lambda, cam, d_obs_info);
+  h->L_full = 0;
+  const int rc = set_problem_dev(h, P, T_qt, fixed, L, psi, E, e_point, e_pose, e_anchor, nullptr, nullptr, C, c_i, c_j, c_T,
+                                 c_Lambda, cam, d_obs_info);
   if (rc == SVS_OK && cudaStreamSynchronize(h->stream) != cudaSuccess) return SVS_ERR_CUDA;   // d_obs_info may be reused now
   return rc;
 }

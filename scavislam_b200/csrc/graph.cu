@@ -285,9 +285,9 @@ struct svs_map {
   char* d_map = nullptr; size_t map_cap = 0;
   MapDev m{};
   char* d_work = nullptr; size_t work_cap = 0;
-  std::vector<int> h_ep, h_es, h_ea, h_winpos;
-  std::vector<double> h_pose, h_psi;
+  std::vector<int> h_winpos;
   const double* d_oi_last = nullptr;   // [E][3] observations, [E][3] weights of the last assembly
+  const int* d_ep_last = nullptr; const int* d_es_last = nullptr; const int* d_ea_last = nullptr;   // its index triples
   int last_E = 0;
   const int* d_win_last = nullptr; const int* d_act_last = nullptr; int last_P = 0, last_L = 0;   // the last assembled window
   char* d_upd = nullptr; size_t upd_cap = 0;   // staging of svs_map_update_*
@@ -470,6 +470,7 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   svs::NvtxRange nvtx_("copyDataToG2o");
   if (!ba || !h || P <= 0 || L < 0 || C < 0 || !window_vertex || (L && !active_point) || !cam || !h->d_map) return SVS_ERR_INVALID;
   if (svs::ba_device(ba) != h->device) { h->err = "map and bundle adjuster live on different devices"; return SVS_ERR_INVALID; }
+  if (C && (!c_i || !c_j || !c_T || !c_Lambda)) { h->err = "svs_ba_set_problem: null array"; return SVS_ERR_INVALID; }
   // window position of every vertex (-1 = outside the double window)
   h->h_winpos.assign(h->V, -1);
   for (int i = 0; i < P; ++i) {
@@ -495,6 +496,12 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   const size_t o_es = off; off += al256(sizeof(int) * emax);
   const size_t o_ea = off; off += al256(sizeof(int) * emax);
   const size_t o_oi = off; off += al256(sizeof(double) * 6 * emax);
+  // the caller's fixed flags and pose-pose constraints (host arrays) go up next to the window
+  const size_t o_fx = off; off += al256((size_t)P);
+  const size_t o_ci = off; off += al256(sizeof(int) * (size_t)C);
+  const size_t o_cj = off; off += al256(sizeof(int) * (size_t)C);
+  const size_t o_cT = off; off += al256(sizeof(double) * 7 * (size_t)C);
+  const size_t o_cL = off; off += al256(sizeof(double) * 36 * (size_t)C);
   GCK(cudaStreamSynchronize(h->stream));
   if (off > h->work_cap) {
     cudaFree(h->d_work); h->d_work = nullptr; h->work_cap = 0;
@@ -512,6 +519,13 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   GCK(cudaMemcpyAsync(d_win, window_vertex, sizeof(int) * (size_t)P, cudaMemcpyHostToDevice, h->stream));
   if (L) GCK(cudaMemcpyAsync(d_act, active_point, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
   GCK(cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream));
+  if (fixed) GCK(cudaMemcpyAsync(W + o_fx, fixed, (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  if (C) {
+    GCK(cudaMemcpyAsync(W + o_ci, c_i, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    GCK(cudaMemcpyAsync(W + o_cj, c_j, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    GCK(cudaMemcpyAsync(W + o_cT, c_T, sizeof(double) * 7 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    GCK(cudaMemcpyAsync(W + o_cL, c_Lambda, sizeof(double) * 36 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+  }
   int E = 0, bad = 0;
   if (L) {
     k_count<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, d_wp, d_act, L, d_cnt, d_bad);
@@ -525,22 +539,16 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   }
   k_gather_poses<<<(7 * P + 255) / 256, 256, 0, h->stream>>>(h->m, d_win, P, d_pose);
   GCK(cudaGetLastError());
-  // only the index triples, psi and the window's poses go back: structure analysis and initial state of the BA handle
-  h->h_ep.resize(std::max(E, 1)); h->h_es.resize(std::max(E, 1)); h->h_ea.resize(std::max(E, 1));
-  h->h_pose.resize(7 * (size_t)P); h->h_psi.resize(3 * (size_t)std::max(L, 1));
-  if (E) {
-    GCK(cudaMemcpyAsync(h->h_ep.data(), d_ep, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(h->h_es.data(), d_es, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(h->h_ea.data(), d_ea, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost, h->stream));
-  }
-  if (L) GCK(cudaMemcpyAsync(h->h_psi.data(), d_psi, sizeof(double) * 3 * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
-  GCK(cudaMemcpyAsync(h->h_pose.data(), d_pose, sizeof(double) * 7 * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
-  GCK(cudaStreamSynchronize(h->stream));
+  GCK(cudaStreamSynchronize(h->stream));   // the BA handle reads the window on its own stream
   if (num_edges) *num_edges = E;
   h->d_oi_last = d_oi; h->last_E = E;
+  h->d_ep_last = d_ep; h->d_es_last = d_es; h->d_ea_last = d_ea;
   h->d_win_last = d_win; h->d_act_last = d_act; h->last_P = P; h->last_L = L;
-  const int rc = svs::ba_set_problem_device_obs(ba, P, h->h_pose.data(), fixed, L, h->h_psi.data(), E, h->h_ep.data(), h->h_es.data(),
-                                                h->h_ea.data(), d_oi, C, c_i, c_j, c_T, c_Lambda, cam);
+  // the window goes to the BA handle device to device: its structure is analysed there (svs_ba_set_problem_device)
+  const int rc = svs::ba_set_problem_device_obs(ba, P, d_pose, fixed ? reinterpret_cast<const unsigned char*>(W + o_fx) : nullptr, L,
+                                                 d_psi, E, d_ep, d_es, d_ea, d_oi, C, reinterpret_cast<const int*>(W + o_ci),
+                                                 reinterpret_cast<const int*>(W + o_cj), reinterpret_cast<const double*>(W + o_cT),
+                                                 reinterpret_cast<const double*>(W + o_cL), cam);
   if (rc != SVS_OK) h->err = std::string("svs_ba_set_problem: ") + svs_last_error(ba);
   return rc;
 }
@@ -742,10 +750,10 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
 int svs_map_last_edges(svs_map* h, int E, int* e_point, int* e_pose, int* e_anchor, double* e_obs, double* e_info) {
   if (!h || E != h->last_E || !h->d_work) return SVS_ERR_INVALID;
   if (E == 0) return SVS_OK;
-  if (e_point) memcpy(e_point, h->h_ep.data(), sizeof(int) * (size_t)E);
-  if (e_pose) memcpy(e_pose, h->h_es.data(), sizeof(int) * (size_t)E);
-  if (e_anchor) memcpy(e_anchor, h->h_ea.data(), sizeof(int) * (size_t)E);
   cudaSetDevice(h->device);
+  if (e_point) GCK(cudaMemcpy(e_point, h->d_ep_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_pose) GCK(cudaMemcpy(e_pose, h->d_es_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_anchor) GCK(cudaMemcpy(e_anchor, h->d_ea_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
   if (e_obs) GCK(cudaMemcpy(e_obs, h->d_oi_last, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
   if (e_info) GCK(cudaMemcpy(e_info, h->d_oi_last + 3 * (size_t)E, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
   return SVS_OK;

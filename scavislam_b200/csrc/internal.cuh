@@ -6,8 +6,9 @@ namespace svs {
 // device-resident results of the last svs_match on this handle (n = number of candidate points)
 __attribute__((visibility("hidden"))) void matcher_device_results(svs_matcher* m, const svs_match_result** d_res, int* n,
                                                                    int* device);
-// svs_ba_set_problem with the observations [E][3] and weights [E][3] (one buffer, in this order) already on the
-// BA handle's device in the caller's edge order; returns after the handle has consumed the buffer
+// svs_ba_set_problem_device with the observations [E][3] and weights [E][3] in one buffer (in this order) on the BA
+// handle's device in the caller's edge order; every other array is on that device too (no pointer checks); returns
+// after the handle has consumed the arrays
 __attribute__((visibility("hidden"))) int ba_set_problem_device_obs(
     svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi, int E, const int* e_point,
     const int* e_pose, const int* e_anchor, const double* d_obs_info, int C, const int* c_i, const int* c_j, const double* c_T,
