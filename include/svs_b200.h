@@ -237,6 +237,41 @@ int svs_ba_covariance(svs_ba *h, int robust, double huber_delta, double lambda, 
                       const int *pair_i, const int *pair_j, double *pair_cov, double *point_cov,
                       svs_ba_cov_stats *stats);
 
+/* Gradient of a loss of the optimised window with respect to its observations and their weights (the adjoint of the
+ * minimiser), for a caller who trains observations or confidence weights through the back-end.
+ *   State: the handle's accepted state x*, which must be a stationary point of the cost: optimise to convergence first.
+ *   Notation: e_e = z_e - h_e(x) the stereo residual of edge e and J_e = de_e/dx; Omega_e = diag(e_info[e]); rho'_e the
+ *     Huber weight at x* when `robust` (huber_delta), else 1; the pose tangent is delta = (upsilon, omega) of
+ *     T <- exp(delta) T, psi is updated additively.  H = sum_e rho'_e J_e^T Omega_e J_e + the pose-pose blocks.
+ *   Given g = (dL/d delta_p, dL/d psi_l):  (H + lambda I) v = g over the free variables (fixed poses and landmarks
+ *     without edges are not variables, their v is 0), then per caller edge
+ *       dL_dobs[e]  = -rho'_e Omega_e (J_e v),      dL_dinfo[e][k] = -rho'_e e_{e,k} (J_e v)_k.
+ *   Conditions:
+ *   - rho'_e is held at its value at x*: no rho'' or residual-curvature terms.  This is the exact derivative of the
+ *     minimiser when the residuals vanish and its Gauss-Newton approximation otherwise.
+ *   - H never contains the self-anchor term of SURVEY.md B5, whatever the handle's flags (that term is not a derivative
+ *     of the cost: J_pose = -J_anchor when pose == anchor).  This is where the result deliberately differs from the H of
+ *     svs_ba_covariance.
+ *   - Not differentiated: the pose-pose constraints (they enter H, but get no gradient), the camera, the initial state.
+ *   - An edge whose three weights are all 0 gets 0 in both outputs; the zero-weight padding edges the library adds
+ *     produce nothing.  For a window from svs_ba_set_problem_from_map the caller's edge order is svs_map_last_edges'.
+ *   Arrays: dL_dpose [P][6] (upsilon, omega) and dL_dpsi [L][3] in the caller's orders, NULL = 0; dL_dobs, dL_dinfo
+ *   [E][3] in the caller's edge order, each may be NULL.  on_device != 0: all four are device pointers on the handle's
+ *   device, ready when the call is made.  The call returns after the outputs have been written.
+ *   Method: one build at x* and lambda, one factor and solve of the reduced system, and two light kernels.
+ *   Returns 0; 1 when the reduced system is not positive definite (outputs zeroed); SVS_ERR_STATE before a problem is
+ *   set; SVS_ERR_INVALID for lambda < 0 or not finite, lambda = 0 with no fixed pose (H is exactly singular, SURVEY.md
+ *   B2) and, with on_device, an array that is not memory of the handle's device -- all checked before anything is
+ *   enqueued; SVS_ERR_UNSUPPORTED when the handle has a communicator (sharded windows).  The Levenberg state is left
+ *   as it was found. */
+typedef struct {
+  int P, L, E, nnzb_L, nbranch, general;   /* as svs_ba_cov_stats; E = the caller's edges */
+  float ms;                                /* device time: build + factor + solve + adjoint kernels */
+} svs_ba_grad_stats;
+int svs_ba_observation_grad(svs_ba *h, int robust, double huber_delta, double lambda, const double *dL_dpose,
+                            const double *dL_dpsi, double *dL_dobs, double *dL_dinfo, int on_device,
+                            svs_ba_grad_stats *stats);
+
 /* ------------------------------------------------------------------ block Cholesky of a caller's 6x6-block system
  * g2o::LinearSolver<Matrix6d>::solve(A, x, b) as LinearSolverCSparse implements it (slam_graph.cpp:55-60), for a
  * caller that keeps g2o and hands its reduced camera system to the device (INTEGRATION.md).  The elimination order,

@@ -77,6 +77,14 @@ class SvsBaCovStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class SvsBaGradStats(C.Structure):
+    _fields_ = [("P", C.c_int), ("L", C.c_int), ("E", C.c_int), ("nnzb_L", C.c_int), ("nbranch", C.c_int),
+                ("general", C.c_int), ("ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SvsFastCell(C.Structure):
     _fields_ = [("u0", C.c_int), ("u1", C.c_int), ("v0", C.c_int), ("v1", C.c_int), ("thr", C.c_int)]
 
@@ -156,7 +164,7 @@ EXPORTS = [
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
-    "svs_ba_covariance", "svs_ba_set_problem_device",
+    "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad",
 ]
 
 
@@ -198,6 +206,8 @@ def lib():
     L.svs_ba_solve_reduced.argtypes = [vp, C.c_int, C.c_double, C.c_double, c_dp]
     L.svs_ba_covariance.argtypes = [vp, C.c_int, C.c_double, C.c_double, c_dp, C.c_int, c_ip, c_ip, c_dp, c_dp,
                                     C.POINTER(SvsBaCovStats)]
+    L.svs_ba_observation_grad.argtypes = [vp, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp, C.c_int,
+                                          C.POINTER(SvsBaGradStats)]
     L.svs_device_info.argtypes = [C.c_char_p, C.c_int]
     L.svs_ba_set_structure.argtypes = [vp, C.c_int, c_ip, c_ip]
     L.svs_ba_lm_begin.argtypes = [vp, C.c_double, C.c_int]
@@ -363,7 +373,7 @@ class BundleAdjuster:
         if rc != 0:
             raise SvsError(rc, "svs_ba_create failed (no CUDA device? there is no CPU fallback)")
         self._keep = None
-        self.P = self.L = 0
+        self.P = self.L = self.E = 0
 
     def close(self):
         if self._h:
@@ -412,7 +422,7 @@ class BundleAdjuster:
             k = self._arrays(pb)
             args, cam = self._prob_args(pb, k)
             self._check(lib().svs_ba_set_problem(self._h, *args))
-        self.P, self.L = pb.P, pb.L
+        self.P, self.L, self.E = pb.P, pb.L, pb.E
 
     def _set_problem_device(self, pb):
         import torch
@@ -496,6 +506,38 @@ class BundleAdjuster:
             self._check(rc)
         return pose, pair, point, rc, st.as_dict()
 
+    def observation_grad(self, dL_dpose=None, dL_dpsi=None, robust=True, huber_delta=1.0, lam=0.0):
+        """dL/d(observations, weights) of the optimised window at the accepted state (svs_ba_observation_grad) from
+        dL_dpose [P,6] (upsilon, omega) and dL_dpsi [L,3] (None = 0).  Returns (dL_dobs [E,3], dL_dinfo [E,3] in the
+        caller's edge order, rc, stats); rc = 1: not positive definite (outputs zeroed).  Numpy arrays in, numpy out;
+        CUDA float64 tensors on the handle's device in, tensors out (the current torch stream is synchronised first)."""
+        st = SvsBaGradStats()
+        if _is_torch_tensor(dL_dpose) or _is_torch_tensor(dL_dpsi):
+            import torch
+            ins = [t for t in (dL_dpose, dL_dpsi) if t is not None]
+            dev = ins[0].device
+            for t in ins:
+                if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.device == dev):
+                    raise TypeError("dL_dpose / dL_dpsi: CUDA float64 tensors on one device (or None)")
+            gp = None if dL_dpose is None else dL_dpose.detach().reshape(self.P, 6).contiguous()
+            gl = None if dL_dpsi is None else dL_dpsi.detach().reshape(self.L, 3).contiguous()
+            dobs = torch.empty((self.E, 3), dtype=torch.float64, device=dev)
+            dinfo = torch.empty((self.E, 3), dtype=torch.float64, device=dev)
+            torch.cuda.current_stream(dev).synchronize()   # the handle reads the arrays on its own stream
+            ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
+            rc = lib().svs_ba_observation_grad(self._h, int(robust), float(huber_delta), float(lam), ptr(gp), ptr(gl),
+                                               ptr(dobs), ptr(dinfo), 1, C.byref(st))
+        else:
+            gp = None if dL_dpose is None else np.ascontiguousarray(np.asarray(dL_dpose, np.float64).reshape(self.P, 6))
+            gl = None if dL_dpsi is None else np.ascontiguousarray(np.asarray(dL_dpsi, np.float64).reshape(self.L, 3))
+            dobs, dinfo = np.zeros((self.E, 3)), np.zeros((self.E, 3))
+            ptr = lambda a: a.ctypes.data if a is not None and a.size else None
+            rc = lib().svs_ba_observation_grad(self._h, int(robust), float(huber_delta), float(lam), ptr(gp), ptr(gl),
+                                               ptr(dobs), ptr(dinfo), 0, C.byref(st))
+        if rc < 0:
+            self._check(rc)
+        return dobs, dinfo, rc, st.as_dict()
+
     # ---- stepwise trial API (window split by landmarks across ranks, SURVEY.md 8e)
     def set_structure(self, pairs):
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
@@ -534,7 +576,7 @@ class BundleAdjuster:
         k = self._arrays(pb)
         args, cam = self._prob_args(pb, k)
         self._check(lib().svs_ba_set_problem_sharded(self._h, *args))
-        self.P, self.L = pb.P, pb.L
+        self.P, self.L, self.E = pb.P, pb.L, pb.E
 
     def points_all(self):
         out = np.zeros((self.L, 3))
@@ -557,7 +599,7 @@ class BundleAdjuster:
                                                    C.byref(st))
         if it <= -100:
             raise SvsError(it + 100, lib().svs_last_error(self._h).decode())
-        self.P, self.L = pb.P, pb.L
+        self.P, self.L, self.E = pb.P, pb.L, pb.E
         return it, k["pose_qt"], k["psi"], st.as_dict()
 
 
@@ -1231,7 +1273,7 @@ class DeviceMap:
         self._ck(lib().svs_ba_set_problem_from_map(ba._h, self._h, len(win), _ip(win),
                                                    None if fx is None else fx.ctypes.data_as(c_up), len(act), _ip(act),
                                                    len(ci), _ip(ci), _ip(cj), _dp(cT), _dp(cL), C.byref(cm), C.byref(E)))
-        ba.P, ba.L = len(win), len(act)
+        ba.P, ba.L, ba.E = len(win), len(act), E.value
         return E.value
 
     def last_edges(self, E):

@@ -151,7 +151,7 @@ struct svs_ba {
   int symbolic_hits = 0;
   std::vector<cudaEvent_t> tev;   // per-trial timing events
   // svs_ba_covariance: host copies of the analysis' table and positions (fetched once per structure), the selected
-  // inversion's scratch, the requested blocks | landmark blocks
+  // inversion's scratch, the requested blocks | landmark blocks (svs_ba_observation_grad stages host arrays there too)
   std::vector<int> cov_tbl, cov_pos;
   bool cov_tables = false;
   InvScratch inv;
@@ -1617,6 +1617,81 @@ int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, 
   if (stats) {
     stats->P = P; stats->L = L; stats->nnzb_L = d.nblk; stats->nbranch = d.nbranch; stats->general = general;
     stats->n_pairs_in_pattern = in_pattern - ndiag; stats->n_cols_solved = ncols;
+    cudaEventElapsedTime(&stats->ms, h->ev[0], h->ev[1]);
+  }
+  return failed ? 1 : 0;
+}
+
+int svs_ba_observation_grad(svs_ba* h, int robust, double huber_delta, double lambda, const double* dL_dpose,
+                            const double* dL_dpsi, double* dL_dobs, double* dL_dinfo, int on_device,
+                            svs_ba_grad_stats* stats) {
+  svs::NvtxRange nvtx_("observationGrad");
+  if (int rc = need_problem(h)) return rc;
+  if (stats) memset(stats, 0, sizeof *stats);
+  const std::string fn = "svs_ba_observation_grad: ";
+  BaDev& d = h->d;
+  const int P = d.P, L = d.L, E = d.E_user;
+  if (h->comm) return fail(h, SVS_ERR_UNSUPPORTED, fn + "the handle has a communicator (sharded windows are not supported)");
+  if (!std::isfinite(lambda) || lambda < 0.) return fail(h, SVS_ERR_INVALID, fn + "lambda must be finite and >= 0");
+  cudaSetDevice(h->device);
+  if (on_device)
+    for (const void* p : {(const void*)dL_dpose, (const void*)dL_dpsi, (const void*)dL_dobs, (const void*)dL_dinfo})
+      if (p && !on_handle_device(h, p)) return fail(h, SVS_ERR_INVALID, fn + "an array is not device memory of the handle's device");
+  if (P == 0) return 0;   // no poses, hence no edges: nothing to write
+  const unsigned char* fx = h->k_fixed.data();
+  if (lambda == 0. && std::none_of(fx, fx + P, [](unsigned char f) { return f != 0; }))
+    return fail(h, SVS_ERR_INVALID, fn + "H is singular with no fixed pose and lambda = 0 (every edge is invariant under one "
+                                         "global SE3): fix a pose or pass lambda > 0");
+  int rc;
+  // host arrays go through the pinned / device scratch of svs_ba_covariance: g_pose | g_psi | dL_dobs | dL_dinfo
+  const size_t o_psi = 6 * (size_t)P, o_obs = o_psi + 3 * (size_t)L, o_info = o_obs + 3 * (size_t)E;
+  const double* gp = dL_dpose; const double* gl = dL_dpsi;
+  double* go = dL_dobs; double* gw = dL_dinfo;
+  if (!on_device) {
+    CK(grow(o_info + 3 * (size_t)E, &h->cov_cap, &h->d_cov, &h->h_cov));
+    if (dL_dpose) memcpy(h->h_cov, dL_dpose, o_psi * sizeof(double));
+    if (dL_dpsi) memcpy(h->h_cov + o_psi, dL_dpsi, 3 * (size_t)L * sizeof(double));
+    if (dL_dpose || dL_dpsi) CK(cudaMemcpyAsync(h->d_cov, h->h_cov, o_obs * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    gp = dL_dpose ? h->d_cov : nullptr;
+    gl = dL_dpsi ? h->d_cov + o_psi : nullptr;
+    go = dL_dobs ? h->d_cov + o_obs : nullptr;
+    gw = dL_dinfo ? h->d_cov + o_info : nullptr;
+  }
+  // the kernels run unconditionally at this lambda; the control block is put back as it was found at the end
+  if ((rc = read_ctl(h))) return rc;
+  const LmCtl saved = *h->h_ctl;
+  h->h_ctl->lambda = lambda;
+  h->h_ctl->max_iters = 0;
+  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  if ((rc = clear_system(h))) return rc;
+  CK(cudaEventRecord(h->ev[0], h->stream));
+  // H is the Hessian of the cost: never the self-anchor term of SURVEY.md B5, whatever the handle's flags
+  BaDev db = d;
+  db.flags |= SVS_BA_SKIP_SELF_ANCHOR_HESSIAN;
+  launch_build(db, h->Kmax_gen, robust, huber_delta, h->stream);
+  // the build summed its own right-hand side into bp / bc: k_grad_rhs overwrites bp and accumulates into bc
+  CK(cudaMemsetAsync(d.bc, 0, 6 * (size_t)P * sizeof(double), h->stream));
+  launch_grad_rhs(d, gp, gl, lambda, h->stream);
+  const int general = solve(h) ? 1 : 0;
+  launch_grad_edges(d, gl, lambda, robust, huber_delta, go, gw, h->stream);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(h->ev[1], h->stream));
+  if (!on_device && E) {
+    if (dL_dobs) CK(cudaMemcpyAsync(h->h_cov + o_obs, go, 3 * (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    if (dL_dinfo) CK(cudaMemcpyAsync(h->h_cov + o_info, gw, 3 * (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  }
+  if ((rc = read_ctl(h))) return rc;
+  const int failed = h->h_ctl->chol_fail;
+  if ((rc = clear_system(h))) return rc;
+  *h->h_ctl = saved;
+  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (!on_device) {
+    if (dL_dobs) memcpy(dL_dobs, h->h_cov + o_obs, 3 * (size_t)E * sizeof(double));
+    if (dL_dinfo) memcpy(dL_dinfo, h->h_cov + o_info, 3 * (size_t)E * sizeof(double));
+  }
+  if (stats) {
+    stats->P = P; stats->L = L; stats->E = E; stats->nnzb_L = d.nblk; stats->nbranch = d.nbranch; stats->general = general;
     cudaEventElapsedTime(&stats->ms, h->ev[0], h->ev[1]);
   }
   return failed ? 1 : 0;

@@ -28,4 +28,9 @@ void launch_export(const BaDev& d, double* out, cudaStream_t st);
 // landmark blocks of (H + lambda I)^-1 into out [L][9] (caller's landmark order) from Z = S^-1 on the factor's pattern
 // and the build's W / Dbl at the same lambda (ba_cov.cu)
 void launch_point_cov(const BaDev& d, const double* Z, double lambda, double* out, cudaStream_t st);
+// adjoint solve of svs_ba_observation_grad (ba_grad.cu): bp / bc of (H + lambda I) v = g from the build's W / Dbl, then,
+// after the solve, v_l and dL/d(observations, weights) [E_user][3] in the caller's edge order (either may be nullptr)
+void launch_grad_rhs(const BaDev& d, const double* g_pose, const double* g_psi, double lambda, cudaStream_t st);
+void launch_grad_edges(const BaDev& d, const double* g_psi, double lambda, int robust, double delta, double* dobs,
+                       double* dinfo, cudaStream_t st);
 }  // namespace svs
