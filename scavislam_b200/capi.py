@@ -811,9 +811,18 @@ class DenseTracker:
         self._ck(lib().svs_dt_set_intrinsics(self._h, level, f, px, py))
 
     def set_images(self, level, prev=None, cur=None, dx=None, dy=None):
-        arrs = [None if a is None else np.ascontiguousarray(a, np.float32) for a in (prev, cur, dx, dy)]
-        w = self.w0 >> level
-        self._ck(lib().svs_dt_set_images(self._h, level, *[self._fp(a) for a in arrs], w))
+        """Level images as 2-D float32 arrays of at least (h0 >> level, w0 >> level); the tracker reads that top-left
+        window with each array's own row stride (a pyramid that rounds its sizes up, like cv2.pyrDown, is wider)."""
+        w, h = self.w0 >> level, self.h0 >> level
+        for k, a in enumerate((prev, cur, dx, dy)):
+            if a is None:
+                continue
+            a = np.ascontiguousarray(a, np.float32)
+            if a.ndim != 2 or a.shape[0] < h or a.shape[1] < w:
+                raise SvsError(-1, f"level {level} image of shape {a.shape} is smaller than ({h}, {w})")
+            planes = [None] * 4
+            planes[k] = self._fp(a)
+            self._ck(lib().svs_dt_set_images(self._h, level, *planes, a.shape[1]))
 
     def set_images_device(self, level, prev=None, cur=None, dx=None, dy=None, stride=0):
         self._ck(lib().svs_dt_set_images_device(self._h, level, prev, cur, dx, dy, stride))

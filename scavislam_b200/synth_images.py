@@ -28,11 +28,12 @@ def _value_noise(u, v, seed, octaves=5):
     return out / tot
 
 
-def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H):
+def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H, cam=None):
     """Render the left image (uint8) and disparity (float32) seen from camera centre t_wc (x,y,z)
     with heading yaw (rotation about the y axis).  Scene: ground plane y = 1.5 m (y down) and a far
-    wall z = 25 m, plus a few boxes (fronto-parallel quads) -- all textured with value noise."""
-    f, px, py, b = CAM_F, CAM_PX, CAM_PY, CAM_B
+    wall z = 25 m, plus a few boxes (fronto-parallel quads) -- all textured with value noise.
+    cam = (f, px, py, baseline) of the left camera; None is the default 640x480 camera of synth."""
+    f, px, py, b = (CAM_F, CAM_PX, CAM_PY, CAM_B) if cam is None else cam
     uu, vv = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
     dx = (uu - px) / f; dy = (vv - py) / f; dz = np.ones_like(dx)
     c, s = np.cos(yaw), np.sin(yaw)
@@ -83,14 +84,15 @@ def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H):
 
 
 def _render_job(args):
-    pos, yaw, seed = args
-    img, disp = render_frame(np.asarray(pos), yaw, seed)
+    pos, yaw, seed, w, h, cam = args
+    img, disp = render_frame(np.asarray(pos), yaw, seed, w, h, cam)
     return img, disp
 
 
-def sequence(n_frames=8, seed=77, step=0.02, dyaw=np.deg2rad(0.2), workers=1):
+def sequence(n_frames=8, seed=77, step=0.02, dyaw=np.deg2rad(0.2), workers=1, w=CAM_W, h=CAM_H, cam=None):
     """Frames along a gentle arc: 2 cm / 0.2 deg inter-frame motion.  `workers` > 1 renders the frames in a process
-    pool (the renderer is plain numpy, about a second per 640x480 frame): same images, bit for bit."""
+    pool (the renderer is plain numpy, about a second per 640x480 frame): same images, bit for bit.  (w, h, cam) give
+    another image size and camera (f, px, py, baseline), as in render_frame."""
     poses = []
     pos = np.array([0.0, 0.0, 0.0]); yaw = 0.0
     for i in range(n_frames):
@@ -100,7 +102,7 @@ def sequence(n_frames=8, seed=77, step=0.02, dyaw=np.deg2rad(0.2), workers=1):
     if workers > 1 and n_frames > 2:
         import multiprocessing as mp
         with mp.get_context("fork").Pool(min(workers, n_frames)) as pool:
-            rendered = pool.map(_render_job, [(p.tolist(), y, seed) for p, y in poses])
+            rendered = pool.map(_render_job, [(p.tolist(), y, seed, w, h, cam) for p, y in poses])
     else:
-        rendered = [render_frame(p, y, seed) for p, y in poses]
+        rendered = [render_frame(p, y, seed, w, h, cam) for p, y in poses]
     return [dict(img=im, disp=dp, pos=p, yaw=y) for (im, dp), (p, y) in zip(rendered, poses)]
