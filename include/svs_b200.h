@@ -252,7 +252,8 @@ int svs_ba_covariance(svs_ba *h, int robust, double huber_delta, double lambda, 
  *   - H never contains the self-anchor term of SURVEY.md B5, whatever the handle's flags (that term is not a derivative
  *     of the cost: J_pose = -J_anchor when pose == anchor).  This is where the result deliberately differs from the H of
  *     svs_ba_covariance.
- *   - Not differentiated: the pose-pose constraints (they enter H, but get no gradient), the camera, the initial state.
+ *   - Not differentiated here: the pose-pose constraints (they enter H, but get no gradient), the camera, the initial
+ *     state.  svs_ba_window_grad below adds the constraints and the camera.
  *   - An edge whose three weights are all 0 gets 0 in both outputs; the zero-weight padding edges the library adds
  *     produce nothing.  For a window from svs_ba_set_problem_from_map the caller's edge order is svs_map_last_edges'.
  *   Arrays: dL_dpose [P][6] (upsilon, omega) and dL_dpsi [L][3] in the caller's orders, NULL = 0; dL_dobs, dL_dinfo
@@ -271,6 +272,39 @@ typedef struct {
 int svs_ba_observation_grad(svs_ba *h, int robust, double huber_delta, double lambda, const double *dL_dpose,
                             const double *dL_dpsi, double *dL_dobs, double *dL_dinfo, int on_device,
                             svs_ba_grad_stats *stats);
+
+/* svs_ba_observation_grad extended to the pose-pose constraints and the stereo camera, from the same v (one build, one
+ * factor, one solve; State, Notation and Conditions as above, except that the constraints and the camera are now
+ * differentiated), for a caller who learns constraint information, constraint measurements or the calibration.
+ *   Pose-pose constraint c (G2oEdgeSE3, i = c_i[c], j = c_j[c]): e_c = log(T_ji T_i T_j^-1), cost e_c^T Lambda_c e_c,
+ *     J_i = third(T_ji, e_c), J_j = -third(I, -e_c) (anchored_points.cpp:207-215; zero for a fixed pose) and
+ *     w_c = J_i v_i + J_j v_j.  Then
+ *       dL_dcLambda[c][a][b] = -(w_{c,a} e_{c,b} + w_{c,b} e_{c,a}) / 2   the gradient of each entry as the cost uses
+ *                                                                        it (symmetric; on the diagonal the form of
+ *                                                                        dL_dinfo)
+ *       dL_dcT[c]            = -X_c^T Lambda_c w_c,  X_c = third(I, e_c)  in the tangent (upsilon, omega) of
+ *                                                                        T_ji <- exp(delta) T_ji
+ *     A constraint whose two poses are fixed gets exactly 0.  Every row of the caller's constraint arrays is its own
+ *     input (the reference adds each pair in both orders, SURVEY.md B4).
+ *   Camera (svs_cam): e_e is linear in z_e, so dL_dcam[k] = sum_e (de_e/dcam_k)^T dL_dobs[e] with y the point in the
+ *     observing camera: de/df = -(y0, y1, y0 - b) / y2, de/dpx = -(1, 0, 1), de/dpy = -(0, 1, 0), de/db = (0, 0, f / y2).
+ *     Self-anchored edges count (their J v is the psi block alone); edges with all-zero weights add nothing.  The sum
+ *     runs in a fixed order without atomics: the same bits on every call.
+ *   Like dL_dinfo, dL_dcLambda and dL_dcT are first order in the residual where the residuals do not vanish.
+ *   Arrays: as svs_ba_observation_grad, the outputs in *out (out or any member may be NULL: that output is neither
+ *   computed nor written).  dL_dcT [C][6] and dL_dcLambda [C][36] (row-major) are in the caller's constraint order --
+ *   for a window from svs_ba_set_problem_from_map, the order of the arrays passed to it; dL_dcam [4] is (f, px, py, b).
+ *   Returns: as svs_ba_observation_grad (1: every requested output zeroed), with the same checks in the same order.
+ *   Not differentiated: fixed-pose values and the initial state (zero at a stationary point); sharded windows give
+ *   SVS_ERR_UNSUPPORTED. */
+typedef struct {
+  double *dL_dobs, *dL_dinfo; /* [E][3], the caller's edge order (as svs_ba_observation_grad) */
+  double *dL_dcT;             /* [C][6]  tangent (upsilon, omega) of T_ji <- exp(d) T_ji, the caller's constraint order */
+  double *dL_dcLambda;        /* [C][36] row-major, symmetric */
+  double *dL_dcam;            /* [4]     f, px, py, b */
+} svs_ba_grad_out;            /* any member may be NULL */
+int svs_ba_window_grad(svs_ba *h, int robust, double huber_delta, double lambda, const double *dL_dpose,
+                       const double *dL_dpsi, const svs_ba_grad_out *out, int on_device, svs_ba_grad_stats *stats);
 
 /* ------------------------------------------------------------------ block Cholesky of a caller's 6x6-block system
  * g2o::LinearSolver<Matrix6d>::solve(A, x, b) as LinearSolverCSparse implements it (slam_graph.cpp:55-60), for a

@@ -85,6 +85,11 @@ class SvsBaGradStats(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class SvsBaGradOut(C.Structure):
+    _fields_ = [("dL_dobs", C.c_void_p), ("dL_dinfo", C.c_void_p), ("dL_dcT", C.c_void_p), ("dL_dcLambda", C.c_void_p),
+                ("dL_dcam", C.c_void_p)]
+
+
 class SvsFastCell(C.Structure):
     _fields_ = [("u0", C.c_int), ("u1", C.c_int), ("v0", C.c_int), ("v1", C.c_int), ("thr", C.c_int)]
 
@@ -164,7 +169,7 @@ EXPORTS = [
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
-    "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad",
+    "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad", "svs_ba_window_grad",
 ]
 
 
@@ -208,6 +213,8 @@ def lib():
                                     C.POINTER(SvsBaCovStats)]
     L.svs_ba_observation_grad.argtypes = [vp, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp, C.c_int,
                                           C.POINTER(SvsBaGradStats)]
+    L.svs_ba_window_grad.argtypes = [vp, C.c_int, C.c_double, C.c_double, vp, vp, C.POINTER(SvsBaGradOut), C.c_int,
+                                     C.POINTER(SvsBaGradStats)]
     L.svs_device_info.argtypes = [C.c_char_p, C.c_int]
     L.svs_ba_set_structure.argtypes = [vp, C.c_int, c_ip, c_ip]
     L.svs_ba_lm_begin.argtypes = [vp, C.c_double, C.c_int]
@@ -373,7 +380,7 @@ class BundleAdjuster:
         if rc != 0:
             raise SvsError(rc, "svs_ba_create failed (no CUDA device? there is no CPU fallback)")
         self._keep = None
-        self.P = self.L = self.E = 0
+        self.P = self.L = self.E = self.C = 0
 
     def close(self):
         if self._h:
@@ -422,7 +429,7 @@ class BundleAdjuster:
             k = self._arrays(pb)
             args, cam = self._prob_args(pb, k)
             self._check(lib().svs_ba_set_problem(self._h, *args))
-        self.P, self.L, self.E = pb.P, pb.L, pb.E
+        self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
 
     def _set_problem_device(self, pb):
         import torch
@@ -538,6 +545,51 @@ class BundleAdjuster:
             self._check(rc)
         return dobs, dinfo, rc, st.as_dict()
 
+    # outputs of window_grad: name -> (svs_ba_grad_out member, trailing shape)
+    _GRAD_OUT = {"obs": ("dL_dobs", (3,)), "info": ("dL_dinfo", (3,)), "cT": ("dL_dcT", (6,)),
+                 "cLambda": ("dL_dcLambda", (36,)), "cam": ("dL_dcam", ())}
+
+    def window_grad(self, dL_dpose=None, dL_dpsi=None, robust=True, huber_delta=1.0, lam=0.0,
+                    want=("obs", "info", "cT", "cLambda", "cam")):
+        """svs_ba_window_grad: observation_grad extended to the pose-pose constraints and the camera, from one adjoint
+        solve.  `want` names the outputs to compute, any of "obs" / "info" [E,3] (caller's edge order), "cT" [C,6]
+        (tangent (upsilon, omega) of T_ji <- exp(d) T_ji), "cLambda" [C,36] (row-major, symmetric), "cam" [4]
+        (f, px, py, b); the others are neither computed nor written.  Returns (dict name -> array for the names in
+        `want`, rc, stats); rc = 1: not positive definite (outputs zeroed).  Numpy arrays in, numpy out; CUDA float64
+        tensors on the handle's device in, tensors out (the current torch stream is synchronised first)."""
+        bad = [w for w in want if w not in self._GRAD_OUT]
+        if bad:
+            raise ValueError(f"want: unknown outputs {bad} (choose from {list(self._GRAD_OUT)})")
+        rows = {"obs": self.E, "info": self.E, "cT": self.C, "cLambda": self.C}
+        shape = lambda w: (4,) if w == "cam" else (rows[w],) + self._GRAD_OUT[w][1]
+        st, out = SvsBaGradStats(), SvsBaGradOut()
+        if _is_torch_tensor(dL_dpose) or _is_torch_tensor(dL_dpsi):
+            import torch
+            ins = [t for t in (dL_dpose, dL_dpsi) if t is not None]
+            dev = ins[0].device
+            for t in ins:
+                if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float64 and t.device == dev):
+                    raise TypeError("dL_dpose / dL_dpsi: CUDA float64 tensors on one device (or None)")
+            gp = None if dL_dpose is None else dL_dpose.detach().reshape(self.P, 6).contiguous()
+            gl = None if dL_dpsi is None else dL_dpsi.detach().reshape(self.L, 3).contiguous()
+            res = {w: torch.empty(shape(w), dtype=torch.float64, device=dev) for w in want}
+            torch.cuda.current_stream(dev).synchronize()   # the handle reads the arrays on its own stream
+            ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
+            on_device = 1
+        else:
+            gp = None if dL_dpose is None else np.ascontiguousarray(np.asarray(dL_dpose, np.float64).reshape(self.P, 6))
+            gl = None if dL_dpsi is None else np.ascontiguousarray(np.asarray(dL_dpsi, np.float64).reshape(self.L, 3))
+            res = {w: np.zeros(shape(w)) for w in want}
+            ptr = lambda a: a.ctypes.data if a is not None and a.size else None
+            on_device = 0
+        for w, a in res.items():
+            setattr(out, self._GRAD_OUT[w][0], ptr(a))
+        rc = lib().svs_ba_window_grad(self._h, int(robust), float(huber_delta), float(lam), ptr(gp), ptr(gl),
+                                      C.byref(out), on_device, C.byref(st))
+        if rc < 0:
+            self._check(rc)
+        return res, rc, st.as_dict()
+
     # ---- stepwise trial API (window split by landmarks across ranks, SURVEY.md 8e)
     def set_structure(self, pairs):
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
@@ -576,7 +628,7 @@ class BundleAdjuster:
         k = self._arrays(pb)
         args, cam = self._prob_args(pb, k)
         self._check(lib().svs_ba_set_problem_sharded(self._h, *args))
-        self.P, self.L, self.E = pb.P, pb.L, pb.E
+        self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
 
     def points_all(self):
         out = np.zeros((self.L, 3))
@@ -599,7 +651,7 @@ class BundleAdjuster:
                                                    C.byref(st))
         if it <= -100:
             raise SvsError(it + 100, lib().svs_last_error(self._h).decode())
-        self.P, self.L, self.E = pb.P, pb.L, pb.E
+        self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
         return it, k["pose_qt"], k["psi"], st.as_dict()
 
 
@@ -1282,7 +1334,7 @@ class DeviceMap:
         self._ck(lib().svs_ba_set_problem_from_map(ba._h, self._h, len(win), _ip(win),
                                                    None if fx is None else fx.ctypes.data_as(c_up), len(act), _ip(act),
                                                    len(ci), _ip(ci), _ip(cj), _dp(cT), _dp(cL), C.byref(cm), C.byref(E)))
-        ba.P, ba.L, ba.E = len(win), len(act), E.value
+        ba.P, ba.L, ba.E, ba.C = len(win), len(act), E.value, len(ci)
         return E.value
 
     def last_edges(self, E):

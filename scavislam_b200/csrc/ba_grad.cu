@@ -8,6 +8,11 @@
 //                 state, dL/dz_e = -rho' Omega_e (J_e v) and dL/domega_e = -rho' e_e (.) (J_e v), written at edge_src[e].
 // Fixed poses have Hpl = 0 and x = 0 and add exactly nothing.  The self edge (pose == anchor) has J_pose = -J_anchor, so
 // only its psi block acts on v.  Each caller edge is written by exactly one lane and every sum runs in a fixed order.
+// svs_ba_window_grad adds, from the same v:
+//   k_grad_edges<., true>  also the camera term per landmark, sum over its edges of (de_e/dcam)^T dL/dz_e (e is linear in
+//                          z, so dL/dcam is the contraction of dL/dz), one partial [4] per landmark
+//   k_grad_cam             the L partials summed in a fixed order by one CTA: no atomics, the same bits on every run
+//   k_grad_constraints     one thread per pose-pose constraint: w_c = J_i v_i + J_j v_j, dL/dLambda_c, dL/d delta_c
 #include "ba_dev.cuh"
 #include "ba_kernels.cuh"
 
@@ -52,11 +57,12 @@ k_grad_rhs(BaDev d, const double* __restrict__ g_pose, const double* __restrict_
 
 // One group of LANES lanes per landmark of `list` (nullptr: landmark idx) whose slot count falls on this instance's
 // side of kShortTrack.  Lane `sub` takes the slots and then the edges sub, sub + LANES, ...; the slot sums are reduced
-// over the group by a butterfly, which leaves the same bits on every lane.
-template <int LANES>
+// over the group by a butterfly, which leaves the same bits on every lane.  kCam: the group's camera sums are reduced
+// by the same butterfly and lane 0 writes cam_part[li] (0 for a landmark without edges).
+template <int LANES, bool kCam>
 __global__ void __launch_bounds__(kGradThreads)
 k_grad_edges(BaDev d, const int* __restrict__ list, int n, const double* __restrict__ g_psi, double lambda, int robust,
-             double delta, double* __restrict__ dobs, double* __restrict__ dinfo) {
+             double delta, double* __restrict__ dobs, double* __restrict__ dinfo, double* __restrict__ cam_part) {
   const int lane = threadIdx.x & 31, sub = lane & (LANES - 1);
   const int idx = (int)((blockIdx.x * (unsigned)kGradThreads + threadIdx.x) / LANES);
   if (idx >= n) return;   // whole groups leave together
@@ -65,7 +71,12 @@ k_grad_edges(BaDev d, const int* __restrict__ list, int n, const double* __restr
   if ((K > kShortTrack) != (LANES == 32)) return;   // the other instance's landmark
   const unsigned gmask = LANES == 32 ? 0xffffffffu : ((1u << LANES) - 1u) << (lane & ~(LANES - 1));
   const int e0 = __ldg(d.lm_eptr + li), k = __ldg(d.lm_eptr + li + 1) - e0;
-  if (k == 0) return;
+  if (k == 0) {
+    if (kCam && sub == 0)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) cam_part[4 * (size_t)li + q] = 0.;
+    return;
+  }
   const bool failed = d.ctl->chol_fail;
   const int off = __ldg(d.lm_self + li) ? 0 : 1, ia = __ldg(d.lm_anchor + li);
   const size_t ns = (size_t)d.nslots;
@@ -107,6 +118,7 @@ k_grad_edges(BaDev d, const int* __restrict__ list, int n, const double* __restr
   double va[6];
 #pragma unroll
   for (int r = 0; r < 6; ++r) va[r] = x[6 * ia + r];
+  double gc[4] = {0., 0., 0., 0.};   // kCam: dL/d(f, px, py, b) of this lane's edges
   for (int i = sub; i < k; i += LANES) {
     const int e = e0 + i, src = __ldg(d.edge_src + e);
     if (src < 0) continue;   // zero-weight padding edge
@@ -141,6 +153,13 @@ k_grad_edges(BaDev d, const int* __restrict__ list, int n, const double* __restr
         go[q] = -r1 * om[q] * jv;
         gw[q] = -r1 * er[q] * jv;
       }
+      if (kCam) {   // de/df = -(y0, y1, y0 - b) / y2, de/dpx = -(1, 0, 1), de/dpy = -(0, 1, 0), de/db = (0, 0, f / y2)
+        const double iz = 1. / y[2];
+        gc[0] -= (y[0] * go[0] + y[1] * go[1] + (y[0] - d.b) * go[2]) * iz;
+        gc[1] -= go[0] + go[2];
+        gc[2] -= go[1];
+        gc[3] += d.f * iz * go[2];
+      }
     }
 #pragma unroll
     for (int q = 0; q < 3; ++q) {
@@ -148,15 +167,101 @@ k_grad_edges(BaDev d, const int* __restrict__ list, int n, const double* __restr
       if (dinfo) dinfo[3 * (size_t)src + q] = gw[q];
     }
   }
+  if (kCam) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int s = LANES / 2; s > 0; s >>= 1) gc[q] += __shfl_xor_sync(gmask, gc[q], s);
+    if (sub == 0)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) cam_part[4 * (size_t)li + q] = gc[q];
+  }
+}
+
+// One CTA: out[q] = sum over landmarks of part[l][q], each thread over a fixed stride of landmarks, then a fixed tree.
+__global__ void __launch_bounds__(kGradThreads) k_grad_cam(const double* __restrict__ part, int L, double* __restrict__ out) {
+  __shared__ double sh[4][kGradThreads];
+  const int t = threadIdx.x;
+  double s[4] = {0., 0., 0., 0.};
+  for (int l = t; l < L; l += kGradThreads)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) s[q] += __ldg(part + 4 * (size_t)l + q);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) sh[q][t] = s[q];
+  __syncthreads();
+  for (int w = kGradThreads / 2; w > 0; w >>= 1) {
+    if (t < w)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) sh[q][t] += sh[q][t + w];
+    __syncthreads();
+  }
+  if (t < 4) out[t] = sh[t][0];
+}
+
+// One thread per pose-pose constraint c (G2oEdgeSE3, e_c = log(T_ji T_i T_j^-1), cost e_c^T Lambda_c e_c), with the
+// Jacobians of constraint_build: J_i = third(T_ji, e_c), J_j = -third(I, -e_c), zero for a fixed pose.  w = J_i v_i + J_j v_j;
+//   dL/dLambda_c[a][b] = -(w_a e_b + w_b e_a) / 2   (symmetric: the cost sees Lambda_ab and Lambda_ba together)
+//   dL/d delta_c       = -X^T Lambda_c w,  X = third(I, e_c) = de_c/d delta_c for T_ji <- exp(delta_c) T_ji
+// X is the factor J_i already contains: third(T_ji, e) = third(I, e) Ad(T_ji), since T_ji exp(d) = exp(Ad(T_ji) d) T_ji
+// puts a change of T_i in front of T_ji.  Both outputs of c are written by this thread alone.
+__global__ void __launch_bounds__(kGradThreads)
+k_grad_constraints(BaDev d, double* __restrict__ dcT, double* __restrict__ dcLam) {
+  const int c = (int)(blockIdx.x * (unsigned)kGradThreads + threadIdx.x);
+  if (c >= d.C) return;
+  double w[6] = {0., 0., 0., 0., 0., 0.}, err[6] = {0., 0., 0., 0., 0., 0.};
+  if (!d.ctl->chol_fail) {
+    const double* pose = d.pose[d.ctl->cur];
+    const int i = d.c_i[c], j = d.c_j[c];
+    constraint_error(d, pose, c, err);
+    const double I7[7] = {0, 0, 0, 1, 0, 0, 0};
+    double J[36];
+    if (!d.fixed[i]) {
+      double T21[7];
+      for (int k = 0; k < 7; ++k) T21[k] = d.c_T[7 * (size_t)c + k];
+      third(T21, err, J);
+      for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < 6; ++b) w[a] += J[a * 6 + b] * d.x[6 * i + b];
+    }
+    if (!d.fixed[j]) {
+      double md[6];
+      for (int k = 0; k < 6; ++k) md[k] = -err[k];
+      third(I7, md, J);
+      for (int a = 0; a < 6; ++a)
+        for (int b = 0; b < 6; ++b) w[a] -= J[a * 6 + b] * d.x[6 * j + b];
+    }
+    if (dcT) {
+      const double* Lm = d.c_Lam + 36 * (size_t)c;
+      double u[6];
+      for (int a = 0; a < 6; ++a) {
+        double s = 0.;
+        for (int b = 0; b < 6; ++b) s += Lm[a * 6 + b] * w[b];
+        u[a] = s;
+      }
+      third(I7, err, J);
+      for (int b = 0; b < 6; ++b) {
+        double s = 0.;
+        for (int a = 0; a < 6; ++a) s += J[a * 6 + b] * u[a];
+        dcT[6 * (size_t)c + b] = -s;
+      }
+    }
+  } else if (dcT) {
+    for (int b = 0; b < 6; ++b) dcT[6 * (size_t)c + b] = 0.;
+  }
+  if (dcLam)
+    for (int a = 0; a < 6; ++a)
+      for (int b = 0; b < 6; ++b) dcLam[36 * (size_t)c + 6 * a + b] = -0.5 * (w[a] * err[b] + w[b] * err[a]);
 }
 
 template <int LANES>
 void launch_edges(const BaDev& d, const int* list, int n, const double* g_psi, double lambda, int robust, double delta,
-                  double* dobs, double* dinfo, cudaStream_t st) {
+                  double* dobs, double* dinfo, double* cam_part, cudaStream_t st) {
   if (n <= 0) return;
   const long long threads = (long long)n * LANES;
-  k_grad_edges<LANES><<<(unsigned)((threads + kGradThreads - 1) / kGradThreads), kGradThreads, 0, st>>>(
-      d, list, n, g_psi, lambda, robust, delta, dobs, dinfo);
+  const unsigned grid = (unsigned)((threads + kGradThreads - 1) / kGradThreads);
+  if (cam_part)
+    k_grad_edges<LANES, true><<<grid, kGradThreads, 0, st>>>(d, list, n, g_psi, lambda, robust, delta, dobs, dinfo, cam_part);
+  else
+    k_grad_edges<LANES, false><<<grid, kGradThreads, 0, st>>>(d, list, n, g_psi, lambda, robust, delta, dobs, dinfo, nullptr);
 }
 
 }  // namespace
@@ -169,11 +274,18 @@ void launch_grad_rhs(const BaDev& d, const double* g_pose, const double* g_psi, 
 
 // Tracks of up to kShortTrack slots: kShortLanes lanes each, over all landmarks; the longer ones (gen_lm: 9..32 slots
 // or no observations, long_lm: more than 32) one warp each.
+// cam_part [L][4] (nullptr: no camera term) holds each landmark's camera partial; dcam [4] their sum.
 void launch_grad_edges(const BaDev& d, const double* g_psi, double lambda, int robust, double delta, double* dobs,
-                       double* dinfo, cudaStream_t st) {
-  launch_edges<kShortLanes>(d, nullptr, d.L, g_psi, lambda, robust, delta, dobs, dinfo, st);
-  launch_edges<32>(d, d.gen_lm, d.ngen, g_psi, lambda, robust, delta, dobs, dinfo, st);
-  launch_edges<32>(d, d.long_lm, d.nlong, g_psi, lambda, robust, delta, dobs, dinfo, st);
+                       double* dinfo, double* cam_part, double* dcam, cudaStream_t st) {
+  launch_edges<kShortLanes>(d, nullptr, d.L, g_psi, lambda, robust, delta, dobs, dinfo, cam_part, st);
+  launch_edges<32>(d, d.gen_lm, d.ngen, g_psi, lambda, robust, delta, dobs, dinfo, cam_part, st);
+  launch_edges<32>(d, d.long_lm, d.nlong, g_psi, lambda, robust, delta, dobs, dinfo, cam_part, st);
+  if (cam_part) k_grad_cam<<<1, kGradThreads, 0, st>>>(cam_part, d.L, dcam);
+}
+
+void launch_grad_constraints(const BaDev& d, double* dcT, double* dcLam, cudaStream_t st) {
+  if (d.C == 0 || (!dcT && !dcLam)) return;
+  k_grad_constraints<<<(unsigned)((d.C + kGradThreads - 1) / kGradThreads), kGradThreads, 0, st>>>(d, dcT, dcLam);
 }
 
 }  // namespace svs

@@ -1622,41 +1622,61 @@ int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, 
   return failed ? 1 : 0;
 }
 
-int svs_ba_observation_grad(svs_ba* h, int robust, double huber_delta, double lambda, const double* dL_dpose,
-                            const double* dL_dpsi, double* dL_dobs, double* dL_dinfo, int on_device,
-                            svs_ba_grad_stats* stats) {
-  svs::NvtxRange nvtx_("observationGrad");
+// svs_ba_observation_grad and svs_ba_window_grad: one build, factor and solve at x*, then the kernels of the requested
+// outputs only
+static int window_grad(svs_ba* h, const char* name, int robust, double huber_delta, double lambda, const double* dL_dpose,
+                       const double* dL_dpsi, const svs_ba_grad_out& out, int on_device, svs_ba_grad_stats* stats) {
   if (int rc = need_problem(h)) return rc;
   if (stats) memset(stats, 0, sizeof *stats);
-  const std::string fn = "svs_ba_observation_grad: ";
+  const std::string fn = std::string(name) + ": ";
   BaDev& d = h->d;
-  const int P = d.P, L = d.L, E = d.E_user;
+  const int P = d.P, L = d.L, E = d.E_user, C = d.C;
   if (h->comm) return fail(h, SVS_ERR_UNSUPPORTED, fn + "the handle has a communicator (sharded windows are not supported)");
   if (!std::isfinite(lambda) || lambda < 0.) return fail(h, SVS_ERR_INVALID, fn + "lambda must be finite and >= 0");
   cudaSetDevice(h->device);
   if (on_device)
-    for (const void* p : {(const void*)dL_dpose, (const void*)dL_dpsi, (const void*)dL_dobs, (const void*)dL_dinfo})
+    for (const void* p : {(const void*)dL_dpose, (const void*)dL_dpsi, (const void*)out.dL_dobs, (const void*)out.dL_dinfo,
+                          (const void*)out.dL_dcT, (const void*)out.dL_dcLambda, (const void*)out.dL_dcam})
       if (p && !on_handle_device(h, p)) return fail(h, SVS_ERR_INVALID, fn + "an array is not device memory of the handle's device");
-  if (P == 0) return 0;   // no poses, hence no edges: nothing to write
+  if (P == 0) {   // no poses, hence no edges and no constraints: only the camera's zero gradient to write
+    if (out.dL_dcam && on_device) {
+      CK(cudaMemsetAsync(out.dL_dcam, 0, 4 * sizeof(double), h->stream));
+      CK(cudaStreamSynchronize(h->stream));
+    } else if (out.dL_dcam) {
+      std::fill(out.dL_dcam, out.dL_dcam + 4, 0.);
+    }
+    return 0;
+  }
   const unsigned char* fx = h->k_fixed.data();
   if (lambda == 0. && std::none_of(fx, fx + P, [](unsigned char f) { return f != 0; }))
     return fail(h, SVS_ERR_INVALID, fn + "H is singular with no fixed pose and lambda = 0 (every edge is invariant under one "
                                          "global SE3): fix a pose or pass lambda > 0");
   int rc;
-  // host arrays go through the pinned / device scratch of svs_ba_covariance: g_pose | g_psi | dL_dobs | dL_dinfo
+  // host arrays go through the pinned / device scratch of svs_ba_covariance:
+  //   g_pose | g_psi | dL_dobs | dL_dinfo | dL_dcT | dL_dcLambda | dL_dcam | the camera's per-landmark partials
+  // (device arrays: the partials alone)
   const size_t o_psi = 6 * (size_t)P, o_obs = o_psi + 3 * (size_t)L, o_info = o_obs + 3 * (size_t)E;
+  const size_t o_cT = o_info + 3 * (size_t)E, o_cLam = o_cT + 6 * (size_t)C, o_cam = o_cLam + 36 * (size_t)C;
+  const size_t o_part = on_device ? 0 : o_cam + 4, n_part = out.dL_dcam ? 4 * (size_t)L : 0;
   const double* gp = dL_dpose; const double* gl = dL_dpsi;
-  double* go = dL_dobs; double* gw = dL_dinfo;
+  double* go = out.dL_dobs; double* gw = out.dL_dinfo;
+  double* gcT = out.dL_dcT; double* gcL = out.dL_dcLambda; double* gcam = out.dL_dcam;
   if (!on_device) {
-    CK(grow(o_info + 3 * (size_t)E, &h->cov_cap, &h->d_cov, &h->h_cov));
+    CK(grow(o_part + n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
     if (dL_dpose) memcpy(h->h_cov, dL_dpose, o_psi * sizeof(double));
     if (dL_dpsi) memcpy(h->h_cov + o_psi, dL_dpsi, 3 * (size_t)L * sizeof(double));
     if (dL_dpose || dL_dpsi) CK(cudaMemcpyAsync(h->d_cov, h->h_cov, o_obs * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     gp = dL_dpose ? h->d_cov : nullptr;
     gl = dL_dpsi ? h->d_cov + o_psi : nullptr;
-    go = dL_dobs ? h->d_cov + o_obs : nullptr;
-    gw = dL_dinfo ? h->d_cov + o_info : nullptr;
+    go = go ? h->d_cov + o_obs : nullptr;
+    gw = gw ? h->d_cov + o_info : nullptr;
+    gcT = gcT ? h->d_cov + o_cT : nullptr;
+    gcL = gcL ? h->d_cov + o_cLam : nullptr;
+    gcam = gcam ? h->d_cov + o_cam : nullptr;
+  } else if (n_part) {
+    CK(grow(n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
   }
+  double* part = n_part ? h->d_cov + o_part : nullptr;
   // the kernels run unconditionally at this lambda; the control block is put back as it was found at the end
   if ((rc = read_ctl(h))) return rc;
   const LmCtl saved = *h->h_ctl;
@@ -1673,28 +1693,50 @@ int svs_ba_observation_grad(svs_ba* h, int robust, double huber_delta, double la
   CK(cudaMemsetAsync(d.bc, 0, 6 * (size_t)P * sizeof(double), h->stream));
   launch_grad_rhs(d, gp, gl, lambda, h->stream);
   const int general = solve(h) ? 1 : 0;
-  launch_grad_edges(d, gl, lambda, robust, huber_delta, go, gw, h->stream);
+  launch_grad_edges(d, gl, lambda, robust, huber_delta, go, gw, part, gcam, h->stream);
+  launch_grad_constraints(d, gcT, gcL, h->stream);
   CK(cudaGetLastError());
   CK(cudaEventRecord(h->ev[1], h->stream));
-  if (!on_device && E) {
-    if (dL_dobs) CK(cudaMemcpyAsync(h->h_cov + o_obs, go, 3 * (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    if (dL_dinfo) CK(cudaMemcpyAsync(h->h_cov + o_info, gw, 3 * (size_t)E * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  }
+  // host arrays: each requested output comes back from its place in the scratch
+  struct Back { const double* dst; size_t off, n; };
+  const Back back[] = {{out.dL_dobs, o_obs, 3 * (size_t)E}, {out.dL_dinfo, o_info, 3 * (size_t)E},
+                       {out.dL_dcT, o_cT, 6 * (size_t)C}, {out.dL_dcLambda, o_cLam, 36 * (size_t)C}, {out.dL_dcam, o_cam, 4}};
+  if (!on_device)
+    for (const Back& k : back)
+      if (k.dst && k.n)
+        CK(cudaMemcpyAsync(h->h_cov + k.off, h->d_cov + k.off, k.n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = read_ctl(h))) return rc;
   const int failed = h->h_ctl->chol_fail;
   if ((rc = clear_system(h))) return rc;
   *h->h_ctl = saved;
   CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
-  if (!on_device) {
-    if (dL_dobs) memcpy(dL_dobs, h->h_cov + o_obs, 3 * (size_t)E * sizeof(double));
-    if (dL_dinfo) memcpy(dL_dinfo, h->h_cov + o_info, 3 * (size_t)E * sizeof(double));
-  }
+  if (!on_device)
+    for (const Back& k : back)
+      if (k.dst && k.n) memcpy(const_cast<double*>(k.dst), h->h_cov + k.off, k.n * sizeof(double));
   if (stats) {
     stats->P = P; stats->L = L; stats->E = E; stats->nnzb_L = d.nblk; stats->nbranch = d.nbranch; stats->general = general;
     cudaEventElapsedTime(&stats->ms, h->ev[0], h->ev[1]);
   }
   return failed ? 1 : 0;
+}
+
+int svs_ba_observation_grad(svs_ba* h, int robust, double huber_delta, double lambda, const double* dL_dpose,
+                            const double* dL_dpsi, double* dL_dobs, double* dL_dinfo, int on_device,
+                            svs_ba_grad_stats* stats) {
+  svs::NvtxRange nvtx_("observationGrad");
+  svs_ba_grad_out out{};
+  out.dL_dobs = dL_dobs;
+  out.dL_dinfo = dL_dinfo;
+  return window_grad(h, "svs_ba_observation_grad", robust, huber_delta, lambda, dL_dpose, dL_dpsi, out, on_device, stats);
+}
+
+int svs_ba_window_grad(svs_ba* h, int robust, double huber_delta, double lambda, const double* dL_dpose,
+                       const double* dL_dpsi, const svs_ba_grad_out* out, int on_device, svs_ba_grad_stats* stats) {
+  svs::NvtxRange nvtx_("windowGrad");
+  const svs_ba_grad_out none{};
+  return window_grad(h, "svs_ba_window_grad", robust, huber_delta, lambda, dL_dpose, dL_dpsi, out ? *out : none, on_device,
+                     stats);
 }
 
 // ---- one window sharded by landmarks across GPUs, driven inside the library (SURVEY.md 8e, BASELINE config C5)

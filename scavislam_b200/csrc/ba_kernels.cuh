@@ -31,6 +31,10 @@ void launch_point_cov(const BaDev& d, const double* Z, double lambda, double* ou
 // adjoint solve of svs_ba_observation_grad (ba_grad.cu): bp / bc of (H + lambda I) v = g from the build's W / Dbl, then,
 // after the solve, v_l and dL/d(observations, weights) [E_user][3] in the caller's edge order (either may be nullptr)
 void launch_grad_rhs(const BaDev& d, const double* g_pose, const double* g_psi, double lambda, cudaStream_t st);
+// svs_ba_window_grad also: with cam_part (scratch [L][4]) the camera gradient into dcam [4], summed in a fixed order;
+// nullptr launches the kernels svs_ba_observation_grad uses and nothing else
 void launch_grad_edges(const BaDev& d, const double* g_psi, double lambda, int robust, double delta, double* dobs,
-                       double* dinfo, cudaStream_t st);
+                       double* dinfo, double* cam_part, double* dcam, cudaStream_t st);
+// after the solve: dL/d delta_c [C][6] and dL/dLambda_c [C][36] of every pose-pose constraint (either may be nullptr)
+void launch_grad_constraints(const BaDev& d, double* dcT, double* dcLam, cudaStream_t st);
 }  // namespace svs
