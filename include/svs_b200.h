@@ -600,6 +600,52 @@ int svs_calcFastMotionOnly(svs_pose *h, int n, const int *obs_point_id, const do
  * obs / xyz_actkey): no host trip between matching and pose refinement. */
 int svs_calcFastMotionOnly_matched(svs_pose *h, svs_matcher *m, const svs_cam *cam, const svs_pose_params *params,
                                    double T_frame[7], svs_pose_stats *stats);
+/* svs_calcFastMotionOnly for a track that already lies in GPU memory: obs_point_id, obs_uvu and point_xyz are device
+ * pointers on the handle's device (cam, params and T_frame stay host memory).  They are copied device to device into
+ * the handle's buffers; the point_id range is checked on the device and reported with the same code and message.  The
+ * result is bit-identical to svs_calcFastMotionOnly's on the same numbers.  A host pointer or memory of another
+ * device gives SVS_ERR_INVALID before anything is enqueued.  The arrays are read on the handle's stream, which does
+ * not wait for other streams: the caller must have finished producing them; they may be reused once the call returns. */
+int svs_calcFastMotionOnly_device(svs_pose *h, int n, const int *obs_point_id, const double *obs_uvu, int npoints,
+                                  const double *point_xyz, const svs_cam *cam, const svs_pose_params *params,
+                                  double T_frame[7], svs_pose_stats *stats);
+
+/* Gradient of a loss of the refined pose with respect to the observations, the points and the camera of the last
+ * calcFastMotionOnly (the adjoint of the refinement), for a caller who trains keypoints, a matcher or the map's points
+ * through the tracked pose.
+ *   State: the inputs, parameters and returned pose T* of the last successful svs_calcFastMotionOnly or
+ *     svs_calcFastMotionOnly_device call on this handle, which must have converged.
+ *   Notation: f_i = z_i - pi(T X_{p_i}) the stereo residual of observation i (z_i = obs_uvu[i], X_p = point_xyz[p],
+ *     p_i = obs_point_id[i]); J_i = df_i/d delta (SE3XYZ_STEREO::frameJac) for T <- exp(delta) T, delta = (upsilon,
+ *     omega); r_i = max(1e-10, |f_i|), b = kernel_param and w_i = sqrt(rho(r_i)) / r_i the reweighting of
+ *     pose_optimizer.h:224-231 (w_i = 1 without robust_kernel).
+ *   What is differentiated: the LM stops where its right-hand side vanishes, so T* is the root of
+ *     F(T) = sum_i J_i^T w_i f_i -- not the minimiser of sum_i rho(r_i), which differs on tracks with outliers.  With
+ *     W_i = d(w_i f_i)/df_i = I for r_i < b (or without robust_kernel) and w_i (I - (r_i - b)/(2 r_i - b) f^_i f^_i^T)
+ *     beyond, H = sum_i J_i^T W_i J_i, and (H + lambda I) v = dL_dT:
+ *       dL_dobs[i] = -W_i J_i v
+ *       dL_dxyz[p] = sum_{i: p_i = p} (dpi_i/dX)^T W_i J_i v             (0 for a point nobody observes)
+ *       dL_dcam    = sum_i (dpi_i/d(f, px, py, b))^T W_i J_i v
+ *   Conditions:
+ *   - The derivatives of J_i are dropped (Gauss-Newton, as in svs_ba_observation_grad); the reweighting's derivative
+ *     W_i is kept exactly.  T_init is not differentiated: the root does not depend on the start.
+ *   - lambda > 0 is needed when H is singular (n <= 2 observations).
+ *   - The sums over a point's observations and over all observations run in a fixed order without atomics: repeated
+ *     calls give the same bits.  The call leaves the forward state alone: a later forward call gives the same bits
+ *     whether or not this one ran in between.  Its buffers are allocated on its first call.
+ *   Arrays: dL_dT [6] (upsilon, omega), NULL = 0; dL_dobs [n][3], dL_dxyz [npoints][3], dL_dcam [4] (f, px, py, b), in
+ *   the forward's orders; a NULL output is neither computed nor written.  on_device != 0: every array is device memory
+ *   of the handle's device, ready when the call is made.  The call returns after the outputs have been written.
+ *   Returns 0; 1 when H + lambda I is not positive definite (the requested outputs zeroed); SVS_ERR_STATE before any
+ *   successful forward call, after a failed one and after svs_calcFastMotionOnly_matched (gradients with respect to
+ *   the matcher's buffers are not provided); SVS_ERR_INVALID for lambda < 0 or not finite and, with on_device, an
+ *   array that is not memory of the handle's device -- all checked before anything is enqueued. */
+typedef struct {
+  int num_obs, npoints;
+  float ms;   /* device time of the gradient kernels (the once-per-problem sort by point is not included) */
+} svs_pose_grad_stats;
+int svs_pose_grad(svs_pose *h, double lambda, const double dL_dT[6], double *dL_dobs, double *dL_dxyz, double *dL_dcam,
+                  int on_device, svs_pose_grad_stats *stats);
 
 /* ------------------------------------------------------------------ pose-pose constraint weights
  * ("next" row, SURVEY.md 8f-4).  SlamGraph::computeConstraint (slam_graph.cpp:785-846) for a batch of pose

@@ -13,6 +13,11 @@ that state is stationary: optimise to convergence.  Robust weights are held at t
 the initial state (its gradient is zero at a stationary point) and the values of fixed poses are not differentiated.
 The handle keeps the window between the two passes: nothing may be loaded into or optimised on `ba` before backward()
 runs.
+
+The front end's motion-only pose refinement is differentiable the same way (svs_pose_grad):
+
+    T = track_pose(po, obs_point_id, obs_uvu, point_xyz, cam, T_init, True, 2.0, 15)
+    loss(T).backward()                   # fills obs_uvu.grad, point_xyz.grad and cam.grad
 """
 from __future__ import annotations
 
@@ -118,6 +123,57 @@ class _OptimiseWindow(torch.autograd.Function):
         for name, like in zip(("obs", "info", "cT", "cLambda", "cam"), ctx.like):
             grads.append(None if like is None else res[name].reshape(like[2]).to(like[1], like[0]))
         return (*grads, None, None, None, None, None, None, None)
+
+
+class _TrackPose(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, obs_uvu, point_xyz, cam, po, obs_point_id, T_init, robust_kernel, kernel_param, num_iter, initial_mu,
+                grad_lambda):
+        dev = obs_uvu.device
+        host = lambda a: a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)
+        if dev.type == "cuda":   # the track stays on the device (svs_calcFastMotionOnly_device)
+            pid = torch.as_tensor(obs_point_id).to(dev, torch.int32)
+            obs, xyz = obs_uvu.detach(), torch.as_tensor(point_xyz).detach().to(dev)
+        else:
+            pid, obs, xyz = host(obs_point_id), host(obs_uvu), host(point_xyz)
+        cam_t = tuple(float(x) for x in host(cam).reshape(4))
+        T, _ = po.calc_fast_motion_only(pid, obs, xyz, cam_t, host(T_init).astype(np.float64).reshape(7), robust_kernel,
+                                        kernel_param, num_iter, initial_mu)
+        T = torch.as_tensor(T, dtype=torch.float64, device=dev)
+        ctx.po, ctx.grad_lambda = po, grad_lambda
+        ctx.like = [(a.dtype, a.device, a.shape) if isinstance(a, torch.Tensor) else None for a in (obs_uvu, point_xyz, cam)]
+        ctx.save_for_backward(T)
+        return T
+
+    @staticmethod
+    def backward(ctx, g_T):
+        (T,) = ctx.saved_tensors
+        names = ("obs", "xyz", "cam")
+        want = [w for w, like, need in zip(names, ctx.like, ctx.needs_input_grad[:3]) if like is not None and need]
+        none = (None,) * 8
+        if not want:
+            return (None, None, None, *none)
+        g = pose_grad_to_tangent(T[None], g_T.to(torch.float64)[None])[0].contiguous()
+        res, rc, _ = ctx.po.grad(g if g.is_cuda else g.numpy(), ctx.grad_lambda, want)
+        if rc != 0:
+            raise RuntimeError(f"svs_pose_grad: H + lambda I is not positive definite (rc = {rc}); pass grad_lambda > 0")
+        grads = []
+        for w, like in zip(names, ctx.like):
+            grads.append(torch.as_tensor(res[w]).reshape(like[2]).to(like[1], like[0]) if w in res else None)
+        return (*grads, *none)
+
+
+def track_pose(po, obs_point_id, obs_uvu, point_xyz, cam, T_init, robust_kernel=True, kernel_param=1.0, num_iter=50,
+               initial_mu=-1.0, grad_lambda=0.0):
+    """Refine the frame pose with the PoseOptimizer `po` (calcFastMotionOnly) on the observations obs_uvu [n,3] of the
+    points point_xyz [npoints,3] (obs_point_id [n] indexes them), with cam (f, px, py, b) and the start T_init [7], and
+    return the pose T [7] (qx, qy, qz, qw, tx, ty, tz) as a float64 tensor on obs_uvu's device.  CUDA tensors stay on
+    the device (po must live on theirs).  backward() fills obs_uvu.grad, point_xyz.grad and cam.grad where they are
+    tensors that require it (svs_pose_grad, one solve at H + grad_lambda I; grad_lambda > 0 for n <= 2).  The gradient
+    is that of the root the LM converges to, so run it to convergence; T_init gets none.  The handle keeps the track
+    between the two passes: nothing may be refined on `po` before backward() runs."""
+    return _TrackPose.apply(obs_uvu, point_xyz, cam, po, obs_point_id, T_init, robust_kernel, kernel_param, num_iter,
+                            initial_mu, grad_lambda)
 
 
 def optimise_window(ba, pb, e_obs, e_info, num_iters, robust=True, huber_delta=1.0, lambda_init=50.0, grad_lambda=0.0,

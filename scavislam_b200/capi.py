@@ -118,6 +118,13 @@ class SvsPoseStats(C.Structure):
                 ("iterations", C.c_int), ("trials", C.c_int), ("ms", C.c_float)]
 
 
+class SvsPoseGradStats(C.Structure):
+    _fields_ = [("num_obs", C.c_int), ("npoints", C.c_int), ("ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SvsMatchLevel(C.Structure):
     _fields_ = [("w", C.c_int), ("h", C.c_int), ("f", C.c_double), ("px", C.c_double), ("py", C.c_double)]
 
@@ -158,7 +165,7 @@ EXPORTS = [
     "svs_prep_get_u8", "svs_prep_get_f32", "svs_dt_set_images_device", "svs_dt_swap_prev_cur",
     "svs_matcher_set_pyramid_device",
     "svs_pose_create", "svs_pose_destroy", "svs_pose_last_error", "svs_calcFastMotionOnly",
-    "svs_calcFastMotionOnly_matched",
+    "svs_calcFastMotionOnly_matched", "svs_calcFastMotionOnly_device", "svs_pose_grad",
     "svs_dtc_create", "svs_dtc_destroy", "svs_dtc_last_error", "svs_dtc_set_prev_u8", "svs_dtc_set_cur",
     "svs_dtc_set_disparity", "svs_computeDensePointCloudCpu", "svs_dtc_get_point_cloud", "svs_dtc_set_point_cloud",
     "svs_denseTrackingCpu",
@@ -327,6 +334,9 @@ def lib():
                                          C.POINTER(SvsPoseParams), c_dp, C.POINTER(SvsPoseStats)]
     L.svs_calcFastMotionOnly_matched.argtypes = [vp, vp, C.POINTER(SvsCam), C.POINTER(SvsPoseParams), c_dp,
                                                  C.POINTER(SvsPoseStats)]
+    L.svs_calcFastMotionOnly_device.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, C.POINTER(SvsCam),
+                                                C.POINTER(SvsPoseParams), c_dp, C.POINTER(SvsPoseStats)]
+    L.svs_pose_grad.argtypes = [vp, C.c_double, vp, vp, vp, vp, C.c_int, C.POINTER(SvsPoseGradStats)]
     ucpp = C.POINTER(C.POINTER(C.c_ubyte))
     L.svs_matcher_create.argtypes = [C.c_int, C.c_int, C.POINTER(SvsMatchLevel), C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
     L.svs_matcher_destroy.argtypes = [vp]
@@ -1095,17 +1105,71 @@ class PoseOptimizer:
 
     def calc_fast_motion_only(self, obs_point_id, obs_uvu, point_xyz, cam, T_frame, robust_kernel=True,
                               kernel_param=1.0, num_iter=50, initial_mu=-1.0):
-        """Returns (T_frame_new, stats); cam = (f, px, py, baseline)."""
-        pid = np.ascontiguousarray(obs_point_id, np.int32)
-        obs = np.ascontiguousarray(obs_uvu, np.float64).reshape(-1, 3)
-        xyz = np.ascontiguousarray(point_xyz, np.float64).reshape(-1, 3)
+        """Returns (T_frame_new, stats); cam = (f, px, py, baseline).  obs_point_id, obs_uvu and point_xyz are numpy
+        arrays, or CUDA torch tensors on the handle's device (then svs_calcFastMotionOnly_device reads them where they
+        are; the current torch stream is synchronised first).  T_frame and the returned pose are host arrays [7]."""
         T = np.array(T_frame, np.float64).copy()
         c = SvsCam(*[float(x) for x in cam])
         p = self._params(robust_kernel, kernel_param, num_iter, initial_mu)
         st = SvsPoseStats()
-        self._ck(lib().svs_calcFastMotionOnly(self._h, len(pid), _ip(pid), _dp(obs), len(xyz), _dp(xyz), C.byref(c),
-                                              C.byref(p), _dp(T), C.byref(st)))
+        if any(_is_torch_tensor(a) for a in (obs_point_id, obs_uvu, point_xyz)):
+            import torch
+            arrs = []
+            for name, a, dt in (("obs_point_id", obs_point_id, torch.int32), ("obs_uvu", obs_uvu, torch.float64),
+                                ("point_xyz", point_xyz, torch.float64)):
+                if not (isinstance(a, torch.Tensor) and a.is_cuda):
+                    raise TypeError(f"{name}: a CUDA tensor (all three arrays of a device track are)")
+                arrs.append(a.detach().to(dt).contiguous())
+            pid, obs, xyz = arrs[0].reshape(-1), arrs[1].reshape(-1, 3), arrs[2].reshape(-1, 3)
+            if not (pid.device == obs.device == xyz.device):
+                raise ValueError("obs_point_id, obs_uvu and point_xyz: tensors on one device")
+            torch.cuda.current_stream(pid.device).synchronize()   # the handle reads the arrays on its own stream
+            self._ck(lib().svs_calcFastMotionOnly_device(self._h, pid.numel(), pid.data_ptr(), obs.data_ptr(), len(xyz),
+                                                         xyz.data_ptr(), C.byref(c), C.byref(p), _dp(T), C.byref(st)))
+        else:
+            pid = np.ascontiguousarray(obs_point_id, np.int32)
+            obs = np.ascontiguousarray(obs_uvu, np.float64).reshape(-1, 3)
+            xyz = np.ascontiguousarray(point_xyz, np.float64).reshape(-1, 3)
+            self._ck(lib().svs_calcFastMotionOnly(self._h, len(pid), _ip(pid), _dp(obs), len(xyz), _dp(xyz), C.byref(c),
+                                                  C.byref(p), _dp(T), C.byref(st)))
+        self.n, self.npoints = len(pid), len(xyz)
         return T, self._stats(st)
+
+    # outputs of grad: name -> (trailing shape)
+    _GRAD_OUT = {"obs": (3,), "xyz": (3,), "cam": ()}
+
+    def grad(self, dL_dT, lam=0.0, want=("obs", "xyz", "cam")):
+        """svs_pose_grad: dL/d(observations, points, camera) of the pose the last calc_fast_motion_only returned, from
+        dL_dT [6] in the tangent (upsilon, omega) of T <- exp(delta) T (None = 0).  `want` names the outputs to compute,
+        any of "obs" [n,3], "xyz" [npoints,3], "cam" [4] (f, px, py, b); the others are neither computed nor written.
+        Returns (dict name -> array for the names in `want`, rc, stats); rc = 1: H + lam I is not positive definite
+        (outputs zeroed).  Numpy in, numpy out; a CUDA float64 tensor on the handle's device in, tensors out (the current
+        torch stream is synchronised first)."""
+        bad = [w for w in want if w not in self._GRAD_OUT]
+        if bad:
+            raise ValueError(f"want: unknown outputs {bad} (choose from {list(self._GRAD_OUT)})")
+        n, npts = getattr(self, "n", 0), getattr(self, "npoints", 0)
+        shape = {"obs": (n, 3), "xyz": (npts, 3), "cam": (4,)}
+        st = SvsPoseGradStats()
+        if _is_torch_tensor(dL_dT):
+            import torch
+            if not (dL_dT.is_cuda and dL_dT.dtype == torch.float64):
+                raise TypeError("dL_dT: a CUDA float64 tensor (or numpy, or None)")
+            g = dL_dT.detach().reshape(6).contiguous()
+            res = {w: torch.empty(shape[w], dtype=torch.float64, device=g.device) for w in want}
+            torch.cuda.current_stream(g.device).synchronize()   # the handle reads the arrays on its own stream
+            ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None
+            on_device = 1
+        else:
+            g = None if dL_dT is None else np.ascontiguousarray(np.asarray(dL_dT, np.float64).reshape(6))
+            res = {w: np.zeros(shape[w]) for w in want}
+            ptr = lambda a: a.ctypes.data if a is not None and a.size else None
+            on_device = 0
+        rc = lib().svs_pose_grad(self._h, float(lam), ptr(g), ptr(res.get("obs")), ptr(res.get("xyz")),
+                                 ptr(res.get("cam")), on_device, C.byref(st))
+        if rc < 0:
+            self._ck(rc)
+        return res, rc, st.as_dict()
 
     def calc_fast_motion_only_matched(self, matcher, cam, T_frame, robust_kernel=True, kernel_param=1.0, num_iter=50,
                                       initial_mu=-1.0):

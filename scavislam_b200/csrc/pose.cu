@@ -11,12 +11,16 @@
 // and a rejected step costs one pass plus a 6x6 solve; the reference recomputes A and B from the
 // unchanged frame after a rejection, which gives the same numbers.  Sums are FP64, reduced in a fixed
 // tree order (deterministic).  There is no host round trip inside the loop.
+//
+// svs_calcFastMotionOnly_device runs the same kernel on a track handed over in GPU memory; svs_pose_grad differentiates
+// the returned pose with respect to the observations, points and camera (the kernels after k_pose_lm).
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <string>
 
 #include <cooperative_groups.h>
+#include <cub/cub.cuh>
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
@@ -33,6 +37,7 @@ constexpr double kEps = 0.0000000001;   // global.h:106
 
 struct PoseCtl {
   double T[7];
+  int bad_pid;   // device input: some obs.point_id lies outside [0, npoints) (k_pose_ingest); uploaded with T
   double initial_chi2, chi2, max_err;
   int num_obs, iterations, trials, nan_error;
 };
@@ -321,6 +326,289 @@ __global__ void __launch_bounds__(kThreads) k_pose_lm(PoseArgs a, PoseCtl* ctl) 
   }
 }
 
+// Device input: obs.point_id into the handle's buffer, an id outside [0, npoints) flagged in ctl->bad_pid and replaced
+// by 0 so that the LM kernel that follows on the stream reads only inside point_list (its result is then discarded).
+__global__ void __launch_bounds__(256) k_pose_ingest(const int* __restrict__ src, int n, int npoints, int* __restrict__ dst,
+                                                     PoseCtl* ctl) {
+  const int i = (int)(blockIdx.x * 256u + threadIdx.x);
+  if (i >= n) return;
+  const int p = src[i];
+  const bool bad = p < 0 || p >= npoints;
+  dst[i] = bad ? 0 : p;
+  if (bad) ctl->bad_pid = 1;
+}
+
+// ---------------------------------------------------------------- svs_pose_grad: the derivative of the LM's root
+// The pose the LM returns is the root of F(T) = sum_i J_i^T w_i f_i (its normal equations' right-hand side), with
+// f_i = z_i - pi(T X_{p_i}) and w_i = sqrt(rho(r_i)) / r_i the pseudo-Huber reweighting.  Implicit differentiation,
+// dropping the derivatives of J_i (Gauss-Newton): H = sum_i J_i^T W_i J_i with W_i = d(w_i f_i)/df_i, v = (H + lambda I)^-1 g,
+// u_i = W_i J_i v, and then dL/dz_i = -u_i, dL/dX_p = sum_{i: p_i = p} (dpi_i/dX)^T u_i, dL/dcam = sum_i (dpi_i/dcam)^T u_i.
+//   k_pose_grad_h       H at T* on the forward's launch shape, then (H + lambda I) v = g by Cholesky with a
+//                       positive-definiteness test (one thread)
+//   k_pose_grad_obs     one thread per observation: dL/dz_i, and its point and camera partials
+//   k_pose_grad_points  one thread per point: its partials in ascending observation order (a stable sort by point)
+//   k_pose_grad_cam     one CTA: the camera partials in a fixed order
+// Every sum runs in a fixed order without atomics: repeated calls give the same bits.
+
+struct PoseGradCtl {
+  double g[6];          // dL/d delta from host memory
+  double v[6];          // (H + lambda I)^-1 g
+  double R[9], t[3];    // T* as the forward's last sweep evaluated it
+  int fail;             // H + lambda I not positive definite
+};
+
+// Observation i at (R, t): the point in the camera, f (unweighted), J = df/d delta and W = w (I - c f f^T)
+struct ObsLin {
+  double x, y, z, f[3], J0[6], J1[6], J2[6], w, c;
+};
+
+__device__ __forceinline__ void linearise(const PoseArgs& a, const double R[9], const double t[3], int i, ObsLin& o) {
+  const int p = a.pid ? a.pid[i] : i;
+  const double* X = reinterpret_cast<const double*>(a.xyz + (size_t)p * a.xyz_stride);
+  const double* ob = reinterpret_cast<const double*>(a.obs + (size_t)i * a.obs_stride);
+  const double X0 = X[0], X1 = X[1], X2 = X[2];
+  const double x = R[0] * X0 + R[1] * X1 + R[2] * X2 + t[0];
+  const double y = R[3] * X0 + R[4] * X1 + R[5] * X2 + t[1];
+  const double z = R[6] * X0 + R[7] * X1 + R[8] * X2 + t[2];
+  o.x = x; o.y = y; o.z = z;
+  o.f[0] = ob[0] - (a.f * (x / z) + a.px);
+  o.f[1] = ob[1] - (a.f * (y / z) + a.py);
+  o.f[2] = ob[2] - ((x - a.b) / z * a.f + a.px);
+  // d(w f)/df: w = 1 inside the kernel's quadratic branch; beyond it (r >= b) w = sqrt(2 b r - b^2) / r and
+  // W = w (I - (r - b) / (2 r - b) f^ f^T), written with the unnormalised f: c = (r - b) / ((2 r - b) r^2)
+  o.w = 1; o.c = 0;
+  if (a.robust) {
+    const double r = fmax(kEps, sqrt(o.f[0] * o.f[0] + o.f[1] * o.f[1] + o.f[2] * o.f[2]));
+    const double b = a.kernel_param;
+    if (!(r < b)) {
+      o.w = sqrt(pseudo_huber(r, b)) / r;
+      o.c = (r - b) / ((2 * r - b) * r * r);
+    }
+  }
+  // SE3XYZ_STEREO::frameJac, as in pass()
+  const double one_b_z = 1. / z, one_b_z_sq = 1. / (z * z);
+  const double A = -a.f * one_b_z, B = -a.f * one_b_z;
+  const double C = a.f * x * one_b_z_sq, D = a.f * y * one_b_z_sq, E = a.f * (x - a.b) * one_b_z_sq;
+  const double J0[6] = {A, 0, C, y * C, z * A - x * C, -y * A};
+  const double J1[6] = {0, B, D, -z * B + y * D, -x * D, x * B};
+  const double J2[6] = {A, 0, E, y * E, z * A - x * E, -y * A};
+#pragma unroll
+  for (int k = 0; k < 6; ++k) { o.J0[k] = J0[k]; o.J1[k] = J1[k]; o.J2[k] = J2[k]; }
+}
+
+// e <- W e
+__device__ __forceinline__ void apply_w(const ObsLin& o, double e[3]) {
+  const double fe = o.c * (o.f[0] * e[0] + o.f[1] * e[1] + o.f[2] * e[2]);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) e[k] = o.w * (e[k] - fe * o.f[k]);
+}
+
+// (U + lambda I) v = g, U given by its upper triangle in row order, by Cholesky; false when not positive definite
+__device__ bool chol_solve6(const double* U21, double lambda, const double* g, double v[6]) {
+  double A[6][6], L[6][6], y[6];
+  int k = 0;
+  for (int r = 0; r < 6; ++r)
+    for (int c = r; c < 6; ++c) { A[r][c] = A[c][r] = U21[k++]; }
+  for (int r = 0; r < 6; ++r) A[r][r] += lambda;
+  for (int j = 0; j < 6; ++j) {
+    double d = A[j][j];
+    for (int q = 0; q < j; ++q) d -= L[j][q] * L[j][q];
+    if (!(d > 0)) return false;      // also NaN
+    L[j][j] = sqrt(d);
+    for (int i = j + 1; i < 6; ++i) {
+      double s = A[i][j];
+      for (int q = 0; q < j; ++q) s -= L[i][q] * L[j][q];
+      L[i][j] = s / L[j][j];
+    }
+  }
+  for (int i = 0; i < 6; ++i) {
+    double s = g ? g[i] : 0.;
+    for (int q = 0; q < i; ++q) s -= L[i][q] * y[q];
+    y[i] = s / L[i][i];
+  }
+  for (int i = 5; i >= 0; --i) {
+    double s = y[i];
+    for (int q = i + 1; q < 6; ++q) s -= L[q][i] * v[q];
+    v[i] = s / L[i][i];
+  }
+  bool finite = true;
+  for (int i = 0; i < 6; ++i) finite = finite && isfinite(v[i]);
+  return finite;
+}
+
+template <int kThreads, bool kCluster>
+struct GradShared {
+  double part[kThreads / 32][21];
+  double sum[21];   // this CTA's share (on a cluster read by CTA 0 through DSMEM)
+  double tot[21];
+  double R[9], t[3];
+};
+
+// H at T* summed as k_pose_lm sums J^T J (one CTA, or kCl CTAs added in rank order), then the solve on CTA 0, thread 0
+template <int kThreads, bool kCluster>
+__global__ void __launch_bounds__(kThreads) k_pose_grad_h(PoseArgs a, const PoseCtl* ctl, const double* g, double lambda,
+                                                          PoseGradCtl* gc) {
+  using Cluster = cg::cluster_group;
+  constexpr int kWarps = kThreads / 32;
+  __shared__ GradShared<kThreads, kCluster> sh;
+  int rank = 0, nr = 1;
+  if constexpr (kCluster) { rank = (int)Cluster::block_rank(); nr = (int)Cluster::num_blocks(); }
+  if (threadIdx.x == 0) {
+    double T[7];
+    for (int k = 0; k < 7; ++k) T[k] = ctl->T[k];
+    svs::quat_to_R(T, sh.R);
+    sh.t[0] = T[4]; sh.t[1] = T[5]; sh.t[2] = T[6];
+  }
+  __syncthreads();
+  double R[9], t[3];
+  for (int k = 0; k < 9; ++k) R[k] = sh.R[k];
+  for (int k = 0; k < 3; ++k) t[k] = sh.t[k];
+  double acc[21];
+#pragma unroll
+  for (int k = 0; k < 21; ++k) acc[k] = 0;
+  for (int i = rank * kThreads + (int)threadIdx.x; i < a.n; i += nr * kThreads) {
+    ObsLin o;
+    linearise(a, R, t, i, o);
+    double M0[6], M1[6], M2[6];   // W J, column by column
+#pragma unroll
+    for (int c = 0; c < 6; ++c) {
+      double e[3] = {o.J0[c], o.J1[c], o.J2[c]};
+      apply_w(o, e);
+      M0[c] = e[0]; M1[c] = e[1]; M2[c] = e[2];
+    }
+    int k = 0;
+#pragma unroll
+    for (int r = 0; r < 6; ++r)
+#pragma unroll
+      for (int c = r; c < 6; ++c) acc[k++] += o.J0[r] * M0[c] + o.J1[r] * M1[c] + o.J2[r] * M2[c];
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 21; ++k) {
+    const double s = wsum(acc[k]);
+    if (lane == 0) sh.part[w][k] = s;
+  }
+  __syncthreads();
+  if (threadIdx.x < 21) {
+    double s = 0;
+    for (int q = 0; q < kWarps; ++q) s += sh.part[q][threadIdx.x];
+    sh.sum[threadIdx.x] = s;
+  }
+  const double* tot = sh.sum;
+  if constexpr (kCluster) {
+    Cluster::sync();   // every CTA's share is in its sh.sum
+    if (rank == 0 && threadIdx.x < 21) {   // fixed order: rank 0, 1, ..., nr - 1
+      double s = 0;
+      for (int r = 0; r < nr; ++r) s += Cluster::map_shared_rank(sh.sum, r)[threadIdx.x];
+      sh.tot[threadIdx.x] = s;
+    }
+    tot = sh.tot;
+  }
+  __syncthreads();
+  if (rank == 0 && threadIdx.x == 0) {
+    double v[6];
+    const bool ok = chol_solve6(tot, lambda, g, v);
+    for (int k = 0; k < 6; ++k) gc->v[k] = ok ? v[k] : 0.;
+    for (int k = 0; k < 9; ++k) gc->R[k] = R[k];
+    for (int k = 0; k < 3; ++k) gc->t[k] = t[k];
+    gc->fail = ok ? 0 : 1;
+  }
+  if constexpr (kCluster) Cluster::sync();   // nobody reads a remote sh.sum any more
+}
+
+constexpr int kGradThreads = 256;
+
+// One thread per observation: u = W J v; dobs[i] = -u, the point partial q[i] = (dpi/dX)^T u = R^T (dpi/dy)^T u and
+// the camera partial c[i] = (dpi/d(f, px, py, b))^T u (any of the three may be nullptr)
+__global__ void __launch_bounds__(kGradThreads) k_pose_grad_obs(PoseArgs a, const PoseGradCtl* __restrict__ gc,
+                                                                double* __restrict__ dobs, double* __restrict__ q,
+                                                                double* __restrict__ c) {
+  const int i = (int)(blockIdx.x * (unsigned)kGradThreads + threadIdx.x);
+  if (i >= a.n) return;
+  double R[9], t[3], v[6];
+  for (int k = 0; k < 9; ++k) R[k] = gc->R[k];
+  for (int k = 0; k < 3; ++k) t[k] = gc->t[k];
+  for (int k = 0; k < 6; ++k) v[k] = gc->v[k];
+  const bool fail = gc->fail != 0;
+  ObsLin o;
+  linearise(a, R, t, i, o);
+  double u[3] = {0, 0, 0};
+#pragma unroll
+  for (int k = 0; k < 6; ++k) { u[0] += o.J0[k] * v[k]; u[1] += o.J1[k] * v[k]; u[2] += o.J2[k] * v[k]; }
+  apply_w(o, u);
+  if (dobs)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) dobs[3 * (size_t)i + k] = fail ? 0. : -u[k];
+  const double iz = 1. / o.z;
+  if (q) {
+    // dpi/dy = -J[:, 0:3]
+    const double gy[3] = {-(o.J0[0] * u[0] + o.J2[0] * u[2]), -(o.J1[1] * u[1]),
+                          -(o.J0[2] * u[0] + o.J1[2] * u[1] + o.J2[2] * u[2])};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) q[3 * (size_t)i + k] = R[k] * gy[0] + R[3 + k] * gy[1] + R[6 + k] * gy[2];
+  }
+  if (c) {
+    c[4 * (size_t)i + 0] = (o.x * u[0] + o.y * u[1] + (o.x - a.b) * u[2]) * iz;
+    c[4 * (size_t)i + 1] = u[0] + u[2];
+    c[4 * (size_t)i + 2] = u[1];
+    c[4 * (size_t)i + 3] = -a.f * iz * u[2];
+  }
+}
+
+// One thread per point: the partials of its observations in ascending observation order
+__global__ void __launch_bounds__(kGradThreads) k_pose_grad_points(const int* __restrict__ order, const int* __restrict__ start,
+                                                                   const int* __restrict__ end, const double* __restrict__ q,
+                                                                   int npoints, const PoseGradCtl* __restrict__ gc,
+                                                                   double* __restrict__ dxyz) {
+  const int p = (int)(blockIdx.x * (unsigned)kGradThreads + threadIdx.x);
+  if (p >= npoints) return;
+  double s[3] = {0, 0, 0};
+  for (int k = start[p]; k < end[p]; ++k) {
+    const int i = order[k];
+#pragma unroll
+    for (int j = 0; j < 3; ++j) s[j] += q[3 * (size_t)i + j];
+  }
+  const bool fail = gc->fail != 0;
+#pragma unroll
+  for (int j = 0; j < 3; ++j) dxyz[3 * (size_t)p + j] = fail ? 0. : s[j];
+}
+
+// One CTA: out[k] = sum over observations of c[i][k], each thread over a fixed stride, then a fixed tree
+__global__ void __launch_bounds__(kGradThreads) k_pose_grad_cam(const double* __restrict__ c, int n,
+                                                                const PoseGradCtl* __restrict__ gc, double* __restrict__ out) {
+  __shared__ double sh[4][kGradThreads];
+  const int t = threadIdx.x;
+  double s[4] = {0., 0., 0., 0.};
+  for (int i = t; i < n; i += kGradThreads)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s[k] += c[4 * (size_t)i + k];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) sh[k][t] = s[k];
+  __syncthreads();
+  for (int w = kGradThreads / 2; w > 0; w >>= 1) {
+    if (t < w)
+#pragma unroll
+      for (int k = 0; k < 4; ++k) sh[k][t] += sh[k][t + w];
+    __syncthreads();
+  }
+  if (t < 4) out[t] = gc->fail ? 0. : sh[t][0];
+}
+
+__global__ void __launch_bounds__(kGradThreads) k_iota(int n, int* __restrict__ out) {
+  const int i = (int)(blockIdx.x * (unsigned)kGradThreads + threadIdx.x);
+  if (i < n) out[i] = i;
+}
+
+// start[p] / end[p] of point p's run in the sorted keys (both 0 for a point without observations: memset first)
+__global__ void __launch_bounds__(kGradThreads) k_point_ranges(const int* __restrict__ key, int n, int* __restrict__ start,
+                                                               int* __restrict__ end) {
+  const int s = (int)(blockIdx.x * (unsigned)kGradThreads + threadIdx.x);
+  if (s >= n) return;
+  const int k = key[s];
+  if (s == 0 || key[s - 1] != k) start[k] = s;
+  if (s == n - 1 || key[s + 1] != k) end[k] = s + 1;
+}
+
 }  // namespace
 
 struct svs_pose {
@@ -333,6 +621,21 @@ struct svs_pose {
   double* d_xyz = nullptr;
   PoseCtl* d_ctl = nullptr;
   PoseCtl* h_ctl = nullptr;   // pinned
+  // the last successful svs_calcFastMotionOnly / _device call, which svs_pose_grad differentiates: its inputs stay in
+  // d_pid / d_obs / d_xyz, its pose in d_ctl->T
+  bool have_problem = false;
+  PoseArgs last{};
+  int npoints = 0;
+  bool sorted = false;          // order / start / end describe last's point ids
+  // svs_pose_grad's buffers, allocated on its first call at the handle's capacity
+  PoseGradCtl* d_gctl = nullptr;
+  double* d_gout = nullptr;     // host outputs: dobs [max_obs][3] | dxyz [max_obs][3] | dcam [4]
+  double* h_gout = nullptr;     // pinned: the same | a PoseGradCtl
+  double* d_q = nullptr;        // [max_obs][3] point partials
+  double* d_c = nullptr;        // [max_obs][4] camera partials
+  int* d_sort = nullptr;        // keys | iota | order | start | end, max_obs each
+  void* d_cub = nullptr;
+  size_t cub_bytes = 0;
 };
 
 #define QCK(call)                                                       \
@@ -344,13 +647,31 @@ struct svs_pose {
     }                                                                   \
   } while (0)
 
+// true when p is device (or managed) memory of the handle's device
+static bool on_handle_device(const svs_pose* h, const void* p) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
+}
+
+// after a successful array or device call: the problem svs_pose_grad differentiates
+static void keep_problem(svs_pose* h, const PoseArgs& a, int npoints) {
+  h->last = a;
+  h->npoints = npoints;
+  h->sorted = false;
+  h->have_problem = true;
+}
+
+// src_pid (device input): the caller's obs.point_id, checked against npoints on the device on its way into h->d_pid
 static int run(svs_pose* h, PoseArgs& a, const svs_cam* cam, const svs_pose_params* p, double T[7],
-               svs_pose_stats* stats) {
+               svs_pose_stats* stats, const int* src_pid = nullptr, int npoints = 0) {
   a.f = cam->f; a.px = cam->px; a.py = cam->py; a.b = cam->b;
   a.robust = p->robust_kernel; a.num_iter = p->num_iter; a.kernel_param = p->kernel_param;
   a.initial_mu = p->initial_mu; a.tau = p->tau;
   memcpy(h->h_ctl->T, T, sizeof(double) * 7);
-  QCK(cudaMemcpyAsync(h->d_ctl, h->h_ctl, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+  h->h_ctl->bad_pid = 0;
+  QCK(cudaMemcpyAsync(h->d_ctl, h->h_ctl, offsetof(PoseCtl, bad_pid) + sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  if (src_pid) k_pose_ingest<<<(unsigned)((a.n + 255) / 256), 256, 0, h->stream>>>(src_pid, a.n, npoints, h->d_pid, h->d_ctl);
   QCK(cudaEventRecord(h->ev0, h->stream));
   if (a.n > kClusterMinObs) {
     cudaLaunchConfig_t cfg = {};
@@ -375,6 +696,7 @@ static int run(svs_pose* h, PoseArgs& a, const svs_cam* cam, const svs_pose_para
   QCK(cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PoseCtl), cudaMemcpyDeviceToHost, h->stream));
   QCK(cudaStreamSynchronize(h->stream));
   const PoseCtl& c = *h->h_ctl;
+  if (c.bad_pid) { h->err = "obs.point_id outside point_list"; return SVS_ERR_INVALID; }
   if (c.nan_error) { h->err = "Res is NaN!"; return SVS_ERR_NUMERIC; }
   memcpy(T, c.T, sizeof(double) * 7);
   if (stats) {
@@ -413,6 +735,8 @@ void svs_pose_destroy(svs_pose* h) {
   cudaSetDevice(h->device);
   if (h->stream) cudaStreamSynchronize(h->stream);
   cudaFree(h->d_pid); cudaFree(h->d_obs); cudaFree(h->d_xyz); cudaFree(h->d_ctl);
+  cudaFree(h->d_gctl); cudaFree(h->d_gout); cudaFree(h->d_q); cudaFree(h->d_c); cudaFree(h->d_sort); cudaFree(h->d_cub);
+  if (h->h_gout) cudaFreeHost(h->h_gout);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -426,7 +750,9 @@ int svs_calcFastMotionOnly(svs_pose* h, int n, const int* obs_point_id, const do
                            const double* point_xyz, const svs_cam* cam, const svs_pose_params* params, double T_frame[7],
                            svs_pose_stats* stats) {
   svs::NvtxRange nvtx_("match");
-  if (!h || n <= 0 || !obs_point_id || !obs_uvu || npoints <= 0 || !point_xyz || !cam || !params || !T_frame)
+  if (!h) return SVS_ERR_INVALID;
+  h->have_problem = false;
+  if (n <= 0 || !obs_point_id || !obs_uvu || npoints <= 0 || !point_xyz || !cam || !params || !T_frame)
     return SVS_ERR_INVALID;                       // the reference asserts obs_list.size() > 0
   if (n > h->max_obs || npoints > h->max_obs) { h->err = "more observations/points than the handle's capacity"; return SVS_ERR_INVALID; }
   for (int i = 0; i < n; ++i)
@@ -439,13 +765,152 @@ int svs_calcFastMotionOnly(svs_pose* h, int n, const int* obs_point_id, const do
   memset(&a, 0, sizeof a);
   a.pid = h->d_pid; a.obs = reinterpret_cast<const char*>(h->d_obs); a.xyz = reinterpret_cast<const char*>(h->d_xyz);
   a.obs_stride = a.xyz_stride = 3 * sizeof(double); a.n = n;
-  return run(h, a, cam, params, T_frame, stats);
+  const int rc = run(h, a, cam, params, T_frame, stats);
+  if (rc == SVS_OK) keep_problem(h, a, npoints);
+  return rc;
+}
+
+int svs_calcFastMotionOnly_device(svs_pose* h, int n, const int* obs_point_id, const double* obs_uvu, int npoints,
+                                  const double* point_xyz, const svs_cam* cam, const svs_pose_params* params,
+                                  double T_frame[7], svs_pose_stats* stats) {
+  svs::NvtxRange nvtx_("match");
+  if (!h) return SVS_ERR_INVALID;
+  h->have_problem = false;
+  if (n <= 0 || !obs_point_id || !obs_uvu || npoints <= 0 || !point_xyz || !cam || !params || !T_frame)
+    return SVS_ERR_INVALID;
+  if (n > h->max_obs || npoints > h->max_obs) { h->err = "more observations/points than the handle's capacity"; return SVS_ERR_INVALID; }
+  for (const void* p : {(const void*)obs_point_id, (const void*)obs_uvu, (const void*)point_xyz})
+    if (!on_handle_device(h, p)) {
+      h->err = "svs_calcFastMotionOnly_device: an array is not device memory of the handle's device";
+      return SVS_ERR_INVALID;
+    }
+  cudaSetDevice(h->device);
+  QCK(cudaMemcpyAsync(h->d_obs, obs_uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
+  QCK(cudaMemcpyAsync(h->d_xyz, point_xyz, sizeof(double) * 3 * (size_t)npoints, cudaMemcpyDeviceToDevice, h->stream));
+  PoseArgs a;
+  memset(&a, 0, sizeof a);
+  a.pid = h->d_pid; a.obs = reinterpret_cast<const char*>(h->d_obs); a.xyz = reinterpret_cast<const char*>(h->d_xyz);
+  a.obs_stride = a.xyz_stride = 3 * sizeof(double); a.n = n;
+  const int rc = run(h, a, cam, params, T_frame, stats, obs_point_id, npoints);   // obs_point_id is checked on its way in
+  if (rc == SVS_OK) keep_problem(h, a, npoints);
+  return rc;
+}
+
+int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_dobs, double* dL_dxyz, double* dL_dcam,
+                  int on_device, svs_pose_grad_stats* stats) {
+  svs::NvtxRange nvtx_("poseGrad");
+  if (!h) return SVS_ERR_INVALID;
+  if (stats) memset(stats, 0, sizeof *stats);
+  if (!h->have_problem) {
+    h->err = "svs_pose_grad: no problem to differentiate (call svs_calcFastMotionOnly or _device first; a failed call "
+             "and svs_calcFastMotionOnly_matched leave none)";
+    return SVS_ERR_STATE;
+  }
+  if (!std::isfinite(lambda) || lambda < 0.) { h->err = "svs_pose_grad: lambda must be finite and >= 0"; return SVS_ERR_INVALID; }
+  if (on_device)
+    for (const void* p : {(const void*)dL_dT, (const void*)dL_dobs, (const void*)dL_dxyz, (const void*)dL_dcam})
+      if (p && !on_handle_device(h, p)) {
+        h->err = "svs_pose_grad: on_device = 1 but an array is not device memory of the handle's device";
+        return SVS_ERR_INVALID;
+      }
+  cudaSetDevice(h->device);
+  const int n = h->last.n, np = h->npoints, cap = h->max_obs;
+  const size_t o_xyz = 3 * (size_t)cap, o_cam = 6 * (size_t)cap, o_ctl = o_cam + 4;   // offsets in d_gout / h_gout
+  if (!h->d_gctl) {   // first gradient call on this handle (d_gctl last: it marks the set complete)
+    if (!h->d_gout) QCK(cudaMalloc(&h->d_gout, sizeof(double) * o_ctl));
+    if (!h->h_gout) QCK(cudaMallocHost(&h->h_gout, sizeof(double) * o_ctl + sizeof(PoseGradCtl)));
+    if (!h->d_q) QCK(cudaMalloc(&h->d_q, sizeof(double) * 3 * (size_t)cap));
+    if (!h->d_c) QCK(cudaMalloc(&h->d_c, sizeof(double) * 4 * (size_t)cap));
+    if (!h->d_sort) QCK(cudaMalloc(&h->d_sort, sizeof(int) * 5 * (size_t)cap));
+    QCK(cudaMalloc(&h->d_gctl, sizeof(PoseGradCtl)));
+  }
+  PoseGradCtl* h_gctl = reinterpret_cast<PoseGradCtl*>(h->h_gout + o_ctl);
+  int* keys = h->d_sort; int* iota = keys + cap; int* order = iota + cap; int* start = order + cap; int* end = start + cap;
+  const unsigned nblk = (unsigned)((n + kGradThreads - 1) / kGradThreads);
+  // the stable sort of the observations by point, once per problem (only dL/dxyz needs it)
+  if (dL_dxyz && !h->sorted) {
+    int bits = 1;
+    while (bits < 31 && (1 << bits) < np) ++bits;
+    size_t need = 0;
+    QCK(cub::DeviceRadixSort::SortPairs(nullptr, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
+    if (need > h->cub_bytes) {
+      QCK(cudaFree(h->d_cub));
+      h->d_cub = nullptr; h->cub_bytes = 0;
+      QCK(cudaMalloc(&h->d_cub, need));
+      h->cub_bytes = need;
+    }
+    k_iota<<<nblk, kGradThreads, 0, h->stream>>>(n, iota);
+    QCK(cub::DeviceRadixSort::SortPairs(h->d_cub, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
+    QCK(cudaMemsetAsync(start, 0, sizeof(int) * 2 * (size_t)cap, h->stream));   // start | end
+    k_point_ranges<<<nblk, kGradThreads, 0, h->stream>>>(keys, n, start, end);
+    QCK(cudaGetLastError());
+    h->sorted = true;
+  }
+  const double* g = dL_dT;
+  double* go = dL_dobs; double* gx = dL_dxyz; double* gcam = dL_dcam;
+  if (!on_device) {
+    if (dL_dT) {
+      memcpy(h_gctl->g, dL_dT, 6 * sizeof(double));
+      QCK(cudaMemcpyAsync(h->d_gctl->g, h_gctl->g, 6 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+      g = h->d_gctl->g;
+    }
+    go = go ? h->d_gout : nullptr;
+    gx = gx ? h->d_gout + o_xyz : nullptr;
+    gcam = gcam ? h->d_gout + o_cam : nullptr;
+  }
+  QCK(cudaEventRecord(h->ev0, h->stream));
+  const PoseArgs& a = h->last;
+  if (n > kClusterMinObs) {   // the forward's launch shapes
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(kCl, 1, 1);
+    cfg.blockDim = dim3(kClThreads, 1, 1);
+    cfg.stream = h->stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = kCl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    if (cudaLaunchKernelEx(&cfg, k_pose_grad_h<kClThreads, true>, a, (const PoseCtl*)h->d_ctl, g, lambda, h->d_gctl) !=
+        cudaSuccess) {
+      (void)cudaGetLastError();   // as in run(): the one-CTA shape
+      k_pose_grad_h<kCtaThreads, false><<<1, kCtaThreads, 0, h->stream>>>(a, h->d_ctl, g, lambda, h->d_gctl);
+    }
+  } else {
+    k_pose_grad_h<kCtaThreads, false><<<1, kCtaThreads, 0, h->stream>>>(a, h->d_ctl, g, lambda, h->d_gctl);
+  }
+  if (go || gx || gcam)
+    k_pose_grad_obs<<<nblk, kGradThreads, 0, h->stream>>>(a, h->d_gctl, go, gx ? h->d_q : nullptr, gcam ? h->d_c : nullptr);
+  if (gx)
+    k_pose_grad_points<<<(unsigned)((np + kGradThreads - 1) / kGradThreads), kGradThreads, 0, h->stream>>>(
+        order, start, end, h->d_q, np, h->d_gctl, gx);
+  if (gcam) k_pose_grad_cam<<<1, kGradThreads, 0, h->stream>>>(h->d_c, n, h->d_gctl, gcam);
+  QCK(cudaGetLastError());
+  QCK(cudaEventRecord(h->ev1, h->stream));
+  if (!on_device) {
+    if (go) QCK(cudaMemcpyAsync(h->h_gout, go, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
+    if (gx) QCK(cudaMemcpyAsync(h->h_gout + o_xyz, gx, sizeof(double) * 3 * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
+    if (gcam) QCK(cudaMemcpyAsync(h->h_gout + o_cam, gcam, sizeof(double) * 4, cudaMemcpyDeviceToHost, h->stream));
+  }
+  QCK(cudaMemcpyAsync(h_gctl, h->d_gctl, sizeof(PoseGradCtl), cudaMemcpyDeviceToHost, h->stream));
+  QCK(cudaStreamSynchronize(h->stream));
+  if (!on_device) {
+    if (dL_dobs) memcpy(dL_dobs, h->h_gout, sizeof(double) * 3 * (size_t)n);
+    if (dL_dxyz) memcpy(dL_dxyz, h->h_gout + o_xyz, sizeof(double) * 3 * (size_t)np);
+    if (dL_dcam) memcpy(dL_dcam, h->h_gout + o_cam, sizeof(double) * 4);
+  }
+  if (stats) {
+    stats->num_obs = n; stats->npoints = np;
+    cudaEventElapsedTime(&stats->ms, h->ev0, h->ev1);
+  }
+  return h_gctl->fail ? 1 : 0;
 }
 
 int svs_calcFastMotionOnly_matched(svs_pose* h, svs_matcher* m, const svs_cam* cam, const svs_pose_params* params,
                                    double T_frame[7], svs_pose_stats* stats) {
   svs::NvtxRange nvtx_("match");
-  if (!h || !m || !cam || !params || !T_frame) return SVS_ERR_INVALID;
+  if (!h) return SVS_ERR_INVALID;
+  h->have_problem = false;   // svs_pose_grad does not differentiate through the matcher's buffers
+  if (!m || !cam || !params || !T_frame) return SVS_ERR_INVALID;
   const svs_match_result* d_res = nullptr;
   int n = 0, dev = -1;
   svs::matcher_device_results(m, &d_res, &n, &dev);
