@@ -728,6 +728,81 @@ int svs_map_add_keyframe(svs_map *h, int oldkey, const double *T_newkey_from_old
 /* the edge list of the last assembly (any output may be NULL); E must equal *num_edges */
 int svs_map_last_edges(svs_map *h, int E, int *e_point, int *e_pose, int *e_anchor, double *e_obs, double *e_info);
 
+/* ------------------------------------------------------------------ place recognition
+ * PlaceRecognizer::addLocation (placerecognizer.cpp:206-324) after the caller's SURF step: vocabulary words, TF-IDF
+ * loop candidates (calcLoopStatistics, :131-172) and geometricCheck (:175-202) = BFMatcher(NORM_L2).match +
+ * RanSaC<SE3Model>::compute (ransac.cpp:29-137, ransac_models.cpp:27-181), one call per keyframe with no host round
+ * trip between the stages.  The handle keeps the vocabulary, the stereo camera and the database of places on its
+ * device; SURF detection / description, interpolateDisparity and the monitor's queue policy stay with the caller.
+ *
+ *   Distance.  Both nearest-neighbour searches use d = fp32 sum over dimensions 0..63 in order of
+ *     d = fmaf(q - t, q - t, d) from 0.  OpenCV sums in a vectorised order, so indices equal OpenCV's except at
+ *     near-ties.
+ *   Words.  Row r gets the word with the smallest d (ties to the lowest index) when that d < 0.1f, else none (-1):
+ *     FLANN's L2<float> is squared and radiusSearch(.., 0.1, ..) with one result slot keeps the nearest word.
+ *     DEVIATION: the search is exhaustive; the reference's k-means tree (default SearchParams) is approximate, so a
+ *     row may receive a closer word than the reference found.  Whether FLANN's radius test is < or <= is unverified;
+ *     this is <.  number_of_words of a place = its rows that received a word.
+ *   Scores (bit-exact in float, as the reference computes them).  L = places stored before the call.  Rows r of the
+ *     new keyframe in order; for word w of r, every stored place k not in the exclude set holding w gets
+ *       score[k] += (float(n_w(k)) / float(nwords(k))) * (float(L) / float(c_w(r)))
+ *     rounded per product and summed in r order without contraction; c_w(r) = places holding w, counting the new
+ *     keyframe once an earlier row of it took w (the reference inserts into inverted_index_ per descriptor).
+ *     Only with do_loop_detection; the place is inserted in every case.  best = the largest score > 2, ties to the
+ *     smallest keyframe id (the reference's tie order is unordered_map iteration: unspecified).
+ *   Match.  Every query row is matched to the candidate's row with the smallest d (ties to the lowest index,
+ *     BFMatcher::match with crossCheck = false); dist = sqrtf(d).
+ *   RANSAC.  Query observations = the new uvu; train points = the candidate's xyz = unmap_uvu(uvu), computed at
+ *     insertion with the handle's camera.  Hypothesis h draws match indices from its own SplitMix64 stream (state
+ *     seed ^ (0xD1B54A32D192ED03 * (h + 1)); per draw state += 0x9E3779B97F4A7C15 and the standard finaliser;
+ *     index ((z >> 32) * nmatch) >> 32) with the reference's redraw rules (an index equal to an earlier one of the
+ *     triple is redrawn; a repeated query or train index restarts the triple).  DEVIATION: a hypothesis is void
+ *     after 64 draws (the reference loops forever with fewer than three distinct train indices).  calc_motion =
+ *     Kabsch with H = sum p1 p0^T on the centred triple and the determinant fix (rank(H) <= 2: U's third column is
+ *     u1 x u2; a collinear triple gives NaN and no inliers); belowThreshold on map_uvu in double, T applied as its
+ *     rotation matrix.  The kept hypothesis has the most inliers, ties to the lowest h; with none, T = identity
+ *     (the reference's default SE3) and the inliers are those of the identity, as in the reference's last loop.
+ *     nmatch < 3: 0 inliers and the identity.  Inliers are listed in match (query row) order.  A row with
+ *     u == u_right gives NaN and poisons only the hypotheses that draw it.
+ *   Refused with SVS_ERR_INVALID before anything is enqueued, the database untouched: a keyframe id already stored
+ *     (DEVIATION: the reference would count the repeated keyframe's words in the inverted index again and keep
+ *     the first place), n < 0, a NULL array with n > 0, n_exclude < 0 or
+ *     a NULL exclude_ids with n_exclude > 0, num_ransac < 0, pixel_thr <= 0 or not finite.
+ *   Arrays: words [W][64], desc [n][64], uvu [n][3] = (u, v, u - disparity); inlier_query / inlier_train receive
+ *   num_inliers entries (room for n; NULL = not written).  p = NULL takes SVS_PLACE_PARAMS_DEFAULT. */
+typedef struct svs_place svs_place;
+typedef struct {
+  int num_ransac;
+  double pixel_thr;
+  unsigned long long seed;
+} svs_place_params;
+#define SVS_PLACE_PARAMS_DEFAULT {100, 2.5, 0}
+typedef struct {
+  int best_keyframe_id;      /* argmax of the TF-IDF score, -1 if no score > 2 (or no loop detection) */
+  float best_score;
+  int num_matches, num_inliers;
+  int loop_found;            /* num_inliers > 30: geometricCheck would call monitor.addLoop */
+  double T_query_from_loop[7];
+  float ms;                  /* device time of the call */
+} svs_place_result;
+int svs_place_create(int device, int num_words, const float *words, const svs_cam *cam, svs_place **out);
+void svs_place_destroy(svs_place *h);
+const char *svs_place_last_error(const svs_place *h);
+int svs_place_add_location(svs_place *h, int keyframe_id, int n, const float *desc, const double *uvu,
+                           int do_loop_detection, int n_exclude, const int *exclude_ids, const svs_place_params *p,
+                           svs_place_result *res, int *inlier_query, int *inlier_train);
+/* number of stored places */
+int svs_place_num_places(const svs_place *h);
+/* Read-back of the last call's intermediates, for tests and callers who keep their own policy.  Each returns a
+ * count or a negative SVS_ERR_*.  words: [n], -1 = no word.  scores: the places that received a contribution, in
+ * insertion order (at most cap written; the count is returned).  matches: [num_matches] (0 without a candidate).
+ * hypotheses: triple [cap][3] of match indices (-1 for a void hypothesis) and inliers [cap] (-1 = void); *best = the
+ * kept hypothesis or -1; returns the number run. */
+int svs_place_last_words(const svs_place *h, int *word);
+int svs_place_last_scores(const svs_place *h, int cap, int *keyframe_id, float *score);
+int svs_place_last_matches(const svs_place *h, int *train_idx, float *dist);
+int svs_place_last_hypotheses(const svs_place *h, int cap, int *triple, int *inliers, int *best);
+
 /* Library/device info: writes "name;sm;SMs;..." into buf. */
 int svs_device_info(char *buf, int buflen);
 

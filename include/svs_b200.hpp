@@ -459,6 +459,55 @@ class ConstraintBuilder {
   bool ok_ = false;
 };
 
+// PlaceRecognizer::addLocation (placerecognizer.cpp:206-324) after the caller's SURF step; semantics: svs_place
+struct DetectedLoop {   // placerecognizer.h
+  int query_keyframe_id = -1, loop_keyframe_id = -1;
+  SE3d T_query_from_loop;
+};
+
+class PlaceRecognizer {
+ public:
+  // words [W][64] (the vocabulary the reference reads from surfwords10000.png), cam = the stereo camera
+  PlaceRecognizer(const std::vector<float>& words, const svs_cam& cam, int device = -1) {
+    ok_ = words.size() >= 64 && svs_place_create(device, (int)(words.size() / 64), words.data(), &cam, &h_) == SVS_OK;
+  }
+  ~PlaceRecognizer() { if (h_) svs_place_destroy(h_); }
+  PlaceRecognizer(const PlaceRecognizer&) = delete;
+  PlaceRecognizer& operator=(const PlaceRecognizer&) = delete;
+  bool valid() const { return ok_; }
+  const char* last_error() const { return h_ ? svs_place_last_error(h_) : "no handle"; }
+  svs_place_params params = SVS_PLACE_PARAMS_DEFAULT;
+  const svs_place_result& last_result() const { return res_; }
+
+  // descriptors [n][64], uvu [n][3] = (u, v, u - disparity) of the rows with a disparity.  Returns false on a refused
+  // input or a device error; *loop is written when the check finds a loop (more than 30 inliers), as
+  // geometricCheck's monitor.addLoop would receive it.
+  bool addLocation(int keyframe_id, const std::vector<float>& descriptors, const std::vector<double>& uvu,
+                   const std::vector<int>& exclude_set, bool do_loop_detection, DetectedLoop* loop,
+                   std::vector<int>* inlier_query = nullptr, std::vector<int>* inlier_train = nullptr) {
+    const int n = (int)(descriptors.size() / 64);
+    if (!ok_ || descriptors.size() != 64 * (size_t)n || uvu.size() != 3 * (size_t)n) return false;
+    std::vector<int> iq((size_t)std::max(n, 1)), it((size_t)std::max(n, 1));
+    if (svs_place_add_location(h_, keyframe_id, n, descriptors.data(), uvu.data(), do_loop_detection ? 1 : 0,
+                               (int)exclude_set.size(), exclude_set.data(), &params, &res_, iq.data(), it.data()) != SVS_OK)
+      return false;
+    if (inlier_query) inlier_query->assign(iq.begin(), iq.begin() + res_.num_inliers);
+    if (inlier_train) inlier_train->assign(it.begin(), it.begin() + res_.num_inliers);
+    if (loop && res_.loop_found) {
+      loop->query_keyframe_id = keyframe_id;
+      loop->loop_keyframe_id = res_.best_keyframe_id;
+      std::memcpy(loop->T_query_from_loop.q, res_.T_query_from_loop, sizeof(double) * 4);
+      std::memcpy(loop->T_query_from_loop.t, res_.T_query_from_loop + 4, sizeof(double) * 3);
+    }
+    return true;
+  }
+
+ private:
+  svs_place* h_ = nullptr;
+  bool ok_ = false;
+  svs_place_result res_{};
+};
+
 // The part of SlamGraph the optimiser reads, kept on the device; copyDataToG2o as kernels (slam_graph.cpp:907-1032)
 class DeviceMap {
  public:

@@ -147,6 +147,16 @@ MATCH_POINT_DTYPE = np.dtype([("keyframe", "i4"), ("anchor_level", "i4"), ("xyz_
                               ("anchor_obs_pyr", "f8", 2)])
 
 
+class SvsPlaceParams(C.Structure):
+    _fields_ = [("num_ransac", C.c_int), ("pixel_thr", C.c_double), ("seed", C.c_ulonglong)]
+
+
+class SvsPlaceResult(C.Structure):
+    _fields_ = [("best_keyframe_id", C.c_int), ("best_score", C.c_float), ("num_matches", C.c_int),
+                ("num_inliers", C.c_int), ("loop_found", C.c_int), ("T_query_from_loop", C.c_double * 7),
+                ("ms", C.c_float)]
+
+
 EXPORTS = [
     "svs_ba_create", "svs_ba_destroy", "svs_last_error", "svs_ba_set_problem", "svs_ba_optimize",
     "svs_ba_get_poses", "svs_ba_get_points", "svs_ba_reset_state", "svs_optimiseInnerAndOuterWindow",
@@ -177,6 +187,8 @@ EXPORTS = [
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
     "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad", "svs_ba_window_grad",
+    "svs_place_create", "svs_place_destroy", "svs_place_last_error", "svs_place_add_location", "svs_place_num_places",
+    "svs_place_last_words", "svs_place_last_scores", "svs_place_last_matches", "svs_place_last_hypotheses",
 ]
 
 
@@ -349,6 +361,18 @@ def lib():
     L.svs_matcher_set_features_from_fast.argtypes = [vp, C.c_int, vp]
     L.svs_match.argtypes = [vp, c_dp, c_dp, C.POINTER(SvsMatchPoint), C.c_int, C.c_int, C.c_int, C.c_int,
                             C.POINTER(SvsMatchResult)]
+    L.svs_place_create.argtypes = [C.c_int, C.c_int, c_fp, C.POINTER(SvsCam), C.POINTER(vp)]
+    L.svs_place_destroy.argtypes = [vp]
+    L.svs_place_destroy.restype = None
+    L.svs_place_last_error.argtypes = [vp]
+    L.svs_place_last_error.restype = C.c_char_p
+    L.svs_place_add_location.argtypes = [vp, C.c_int, C.c_int, c_fp, c_dp, C.c_int, C.c_int, c_ip,
+                                         C.POINTER(SvsPlaceParams), C.POINTER(SvsPlaceResult), c_ip, c_ip]
+    L.svs_place_num_places.argtypes = [vp]
+    L.svs_place_last_words.argtypes = [vp, c_ip]
+    L.svs_place_last_scores.argtypes = [vp, C.c_int, c_ip, c_fp]
+    L.svs_place_last_matches.argtypes = [vp, c_ip, c_fp]
+    L.svs_place_last_hypotheses.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip]
     _LIB = L
     return L
 
@@ -1406,3 +1430,93 @@ class DeviceMap:
         obs, info = np.zeros((E, 3)), np.zeros((E, 3))
         self._ck(lib().svs_map_last_edges(self._h, E, _ip(ep), _ip(es), _ip(ea), _dp(obs), _dp(info)))
         return ep, es, ea, obs, info
+
+
+def load_surf_vocabulary(path):
+    """The reference's vocabulary file (surfwords10000.png: every float stored as four uint8 of an 8-bit image,
+    placerecognizer.cpp:91-100) as float32 [W][64]."""
+    import cv2
+    img = cv2.imread(str(path), -1)
+    if img is None or img.dtype != np.uint8 or img.ndim != 2 or img.shape[1] % 4:
+        raise ValueError(f"{path}: not a single-channel 8-bit image with a multiple of 4 columns")
+    return np.ascontiguousarray(img).view(np.float32).copy()
+
+
+class PlaceRecognizer:
+    """PlaceRecognizer::addLocation (reference placerecognizer.cpp:206-324) on the device: words, TF-IDF loop
+    candidates, brute-force match and the RANSAC check.  Semantics: include/svs_b200.h (svs_place)."""
+
+    def __init__(self, words, cam, device=-1):
+        words = np.ascontiguousarray(words, np.float32).reshape(-1, 64)
+        self._h = C.c_void_p()
+        rc = lib().svs_place_create(device, len(words), words.ctypes.data_as(C.POINTER(C.c_float)),
+                                    C.byref(SvsCam(*[float(x) for x in cam])), C.byref(self._h))
+        if rc != 0:
+            raise SvsError(rc, "svs_place_create failed (no CUDA device? there is no CPU fallback)")
+        self._last_n = 0
+
+    def close(self):
+        if self._h:
+            lib().svs_place_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _ck(self, rc):
+        if rc < 0:
+            raise SvsError(rc, lib().svs_place_last_error(self._h).decode())
+        return rc
+
+    @property
+    def num_places(self):
+        return self._ck(lib().svs_place_num_places(self._h))
+
+    def add_location(self, keyframe_id, desc, uvu, do_loop_detection=True, exclude=(), num_ransac=100, pixel_thr=2.5,
+                     seed=0):
+        """Returns dict(best_keyframe_id, best_score, num_matches, num_inliers, loop_found, T_query_from_loop[7], ms,
+        inlier_query, inlier_train)."""
+        desc = np.ascontiguousarray(desc, np.float32).reshape(-1, 64)
+        uvu = np.ascontiguousarray(uvu, np.float64).reshape(-1, 3)
+        if len(uvu) != len(desc):
+            raise ValueError("desc and uvu need one row per descriptor")
+        n = len(desc)
+        ex = np.ascontiguousarray(list(exclude), np.int32)
+        p = SvsPlaceParams(int(num_ransac), float(pixel_thr), int(seed) & (2 ** 64 - 1))
+        r = SvsPlaceResult()
+        iq, it = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        self._ck(lib().svs_place_add_location(self._h, int(keyframe_id), n, desc.ctypes.data_as(C.POINTER(C.c_float)),
+                                              _dp(uvu), int(bool(do_loop_detection)), len(ex), _ip(ex), C.byref(p),
+                                              C.byref(r), _ip(iq), _ip(it)))
+        self._last_n = n
+        ni = r.num_inliers
+        return dict(best_keyframe_id=r.best_keyframe_id, best_score=r.best_score, num_matches=r.num_matches,
+                    num_inliers=ni, loop_found=bool(r.loop_found), T_query_from_loop=np.array(r.T_query_from_loop[:]),
+                    ms=r.ms, inlier_query=iq[:ni].copy(), inlier_train=it[:ni].copy())
+
+    def last_words(self):
+        w = np.zeros(max(self._last_n, 1), np.int32)
+        n = self._ck(lib().svs_place_last_words(self._h, _ip(w)))
+        return w[:n].copy()
+
+    def last_scores(self):
+        cap = max(self.num_places, 1)
+        ids, sc = np.zeros(cap, np.int32), np.zeros(cap, np.float32)
+        n = self._ck(lib().svs_place_last_scores(self._h, cap, _ip(ids), sc.ctypes.data_as(C.POINTER(C.c_float))))
+        return ids[:n].copy(), sc[:n].copy()
+
+    def last_matches(self):
+        t, d = np.zeros(max(self._last_n, 1), np.int32), np.zeros(max(self._last_n, 1), np.float32)
+        n = self._ck(lib().svs_place_last_matches(self._h, _ip(t), d.ctypes.data_as(C.POINTER(C.c_float))))
+        return t[:n].copy(), d[:n].copy()
+
+    def last_hypotheses(self):
+        """(triple[H, 3], inliers[H], best): -1 marks a void hypothesis; best = -1 when none had an inlier."""
+        b = C.c_int()
+        H = self._ck(lib().svs_place_last_hypotheses(self._h, 0, None, None, C.byref(b)))
+        tri, inl = np.zeros((max(H, 1), 3), np.int32), np.zeros(max(H, 1), np.int32)
+        self._ck(lib().svs_place_last_hypotheses(self._h, H, _ip(tri), _ip(inl), C.byref(b)))
+        return tri[:H].copy(), inl[:H].copy(), b.value
