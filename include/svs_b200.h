@@ -692,7 +692,11 @@ int svs_map_update_points(svs_map *h, int n, const int *point, const double *xyz
 int svs_map_get(svs_map *h, double *T_me_from_world, double *xyz_anchor);
 /* SlamGraph::restoreDataFromG2o (slam_graph.cpp:1037-1058) device to device: after svs_ba_optimize on the window
  * svs_ba_set_problem_from_map assembled last, the vertex poses and xyz_anchor = invert_depth(psi) of its points go
- * back into the map without touching the host */
+ * back into the map without touching the host.
+ * Refused with SVS_ERR_STATE, the map unchanged, unless `ba` still holds the very problem this map's last successful
+ * svs_ba_set_problem_from_map loaded into it: after svs_map_set or svs_map_add_keyframe, after a refused
+ * svs_ba_set_problem_from_map, and after any later set-up of `ba` (svs_ba_set_problem*, another map's assembly, a
+ * failed set-up), even one of the same P and L, there is no window to absorb. */
 int svs_map_absorb(svs_map *h, svs_ba *ba);
 /* = svs_ba_set_problem on the window assembled from the map; *num_edges receives E */
 int svs_ba_set_problem_from_map(svs_ba *ba, svs_map *map, int P, const int *window_vertex, const unsigned char *fixed,

@@ -93,6 +93,7 @@ struct svs_ba {
   cudaStream_t stream = nullptr;
   std::string err;
   bool has_problem = false;
+  unsigned long long serial = 0;   // problem serial (svs::ba_problem_serial): a new value at the start of every set-up
   double* d_raw = nullptr; double* h_raw = nullptr; size_t raw_cap = 0;   // user-order observations + weights (6 doubles per edge)
   Worker worker;
   SpinPool pool;   // the per-landmark / per-edge host loops of set_problem
@@ -210,6 +211,12 @@ int dev_upload(svs_ba* h, const T** p, const T* src, size_t n) {
 }
 template <typename T>
 int dev_upload(svs_ba* h, const T** p, const std::vector<T>& v) { return dev_upload(h, p, v.data(), v.size()); }
+
+// process-wide, so that no two set-ups on any two handles share a serial (a destroyed handle's address can come back)
+unsigned long long next_serial() {
+  static std::atomic<unsigned long long> n{0};
+  return ++n;
+}
 
 void free_problem(svs_ba* h) {
   h->has_problem = false;
@@ -655,6 +662,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   for (int c = 0; c < C; ++c)
     if (c_i[c] < 0 || c_i[c] >= P || c_j[c] < 0 || c_j[c] >= P || c_i[c] == c_j[c])
       return fail(h, SVS_ERR_INVALID, "pose-pose edge index out of range");
+  h->serial = next_serial();   // whatever happens below, a window recorded under the old serial is gone
   cudaSetDevice(h->device);
   h->pool.begin();   // the host loops below run on a few spinning threads until this call returns
   struct PoolEnd { SpinPool* p; ~PoolEnd() { p->end(); } } pool_end{&h->pool};
@@ -1062,6 +1070,7 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
                            const int* e_point, const int* e_pose, const int* e_anchor, const double* e_obs,
                            const double* e_info, int C, const int* c_i, const int* c_j, const double* c_T,
                            const double* c_Lambda, const svs_cam* cam, const double* d_obs_info) {
+  h->serial = next_serial();
   cudaSetDevice(h->device);
   CK(cudaStreamSynchronize(h->stream));   // the scratch and the staging buffer are about to be reused
   const cudaStream_t st = h->stream;
@@ -1979,5 +1988,6 @@ int ba_state_on_device(svs_ba* h, const double* const** pose, const double* cons
   *pose = h->d.pose; *psi = h->d.psi; *lm_user = h->d.lm_user; *cur = &h->d.ctl->cur; *stream = h->stream; *P = h->d.P; *L = h->d.L;
   return SVS_OK;
 }
+unsigned long long ba_problem_serial(const svs_ba* h) { return h && h->has_problem ? h->serial : 0; }
 }  // namespace svs
 

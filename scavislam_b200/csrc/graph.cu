@@ -289,7 +289,10 @@ struct svs_map {
   const double* d_oi_last = nullptr;   // [E][3] observations, [E][3] weights of the last assembly
   const int* d_ep_last = nullptr; const int* d_es_last = nullptr; const int* d_ea_last = nullptr;   // its index triples
   int last_E = 0;
-  const int* d_win_last = nullptr; const int* d_act_last = nullptr; int last_P = 0, last_L = 0;   // the last assembled window
+  // the last assembled window and the serial of the BA problem it became (svs::ba_problem_serial); d_win_last = nullptr
+  // when there is none: the map was reloaded or grew, or the last assembly was refused
+  const int* d_win_last = nullptr; const int* d_act_last = nullptr; int last_P = 0, last_L = 0;
+  unsigned long long last_serial = 0;
   char* d_upd = nullptr; size_t upd_cap = 0;   // staging of svs_map_update_*
   char* d_graph = nullptr; size_t graph_cap = 0; GraphDev g{}; int nnzN = 0;   // svs_map_set_graph
   char* d_sel = nullptr; size_t sel_cap = 0;   // work buffers of svs_map_select_window
@@ -378,6 +381,7 @@ int svs_map_set(svs_map* h, int V, const double* T_me_from_world, int Np, const 
   const size_t o_pose = lo.o_pose, o_anch = lo.o_anch, o_xyz = lo.o_xyz, o_vptr = lo.o_vptr, o_vpose = lo.o_vpose, o_cen = lo.o_cen,
                o_lvl = lo.o_lvl;
   GCK(cudaStreamSynchronize(h->stream));
+  h->d_win_last = nullptr;   // a window assembled from the previous map names its rows, not this map's
   if (off > h->map_cap) {
     cudaFree(h->d_map); h->d_map = nullptr; h->map_cap = 0;
     GCK(cudaMalloc(&h->d_map, off + off / 4));
@@ -447,10 +451,12 @@ int svs_map_get(svs_map* h, double* T_me_from_world, double* xyz_anchor) {
 // svs_ba_set_problem_from_map from THIS map) goes back into the map, device to device
 int svs_map_absorb(svs_map* h, svs_ba* ba) {
   svs::NvtxRange nvtx_("restoreDataFromG2o");
-  if (!h || !ba || !h->d_map || !h->d_win_last) return SVS_ERR_INVALID;
+  if (!h || !ba || !h->d_map) return SVS_ERR_INVALID;
+  if (!h->d_win_last) { h->err = "no window of this map is waiting to be absorbed"; return SVS_ERR_STATE; }
   if (svs::ba_device(ba) != h->device) { h->err = "map and bundle adjuster live on different devices"; return SVS_ERR_INVALID; }
   const double* const* pose; const double* const* psi; const int* lm_user; const int* cur; cudaStream_t st; int P, L;
-  if (svs::ba_state_on_device(ba, &pose, &psi, &lm_user, &cur, &st, &P, &L) != SVS_OK || P != h->last_P || L != h->last_L) {
+  if (svs::ba_state_on_device(ba, &pose, &psi, &lm_user, &cur, &st, &P, &L) != SVS_OK || P != h->last_P || L != h->last_L ||
+      svs::ba_problem_serial(ba) != h->last_serial) {
     h->err = "the bundle adjuster does not hold the window this map assembled last";
     return SVS_ERR_STATE;
   }
@@ -470,6 +476,7 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   svs::NvtxRange nvtx_("copyDataToG2o");
   if (!ba || !h || P <= 0 || L < 0 || C < 0 || !window_vertex || (L && !active_point) || !cam || !h->d_map) return SVS_ERR_INVALID;
   if (svs::ba_device(ba) != h->device) { h->err = "map and bundle adjuster live on different devices"; return SVS_ERR_INVALID; }
+  h->d_win_last = nullptr;   // recorded again below once the BA handle has accepted this window
   if (C && (!c_i || !c_j || !c_T || !c_Lambda)) { h->err = "svs_ba_set_problem: null array"; return SVS_ERR_INVALID; }
   // window position of every vertex (-1 = outside the double window)
   h->h_winpos.assign(h->V, -1);
@@ -504,6 +511,7 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   const size_t o_cL = off; off += al256(sizeof(double) * 36 * (size_t)C);
   GCK(cudaStreamSynchronize(h->stream));
   if (off > h->work_cap) {
+    h->last_E = 0; h->d_oi_last = nullptr; h->d_ep_last = h->d_es_last = h->d_ea_last = nullptr;   // they lay in the old arena
     cudaFree(h->d_work); h->d_work = nullptr; h->work_cap = 0;
     GCK(cudaMalloc(&h->d_work, off + off / 4));
     h->work_cap = off + off / 4;
@@ -543,14 +551,15 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   if (num_edges) *num_edges = E;
   h->d_oi_last = d_oi; h->last_E = E;
   h->d_ep_last = d_ep; h->d_es_last = d_es; h->d_ea_last = d_ea;
-  h->d_win_last = d_win; h->d_act_last = d_act; h->last_P = P; h->last_L = L;
   // the window goes to the BA handle device to device: its structure is analysed there (svs_ba_set_problem_device)
   const int rc = svs::ba_set_problem_device_obs(ba, P, d_pose, fixed ? reinterpret_cast<const unsigned char*>(W + o_fx) : nullptr, L,
                                                  d_psi, E, d_ep, d_es, d_ea, d_oi, C, reinterpret_cast<const int*>(W + o_ci),
                                                  reinterpret_cast<const int*>(W + o_cj), reinterpret_cast<const double*>(W + o_cT),
                                                  reinterpret_cast<const double*>(W + o_cL), cam);
-  if (rc != SVS_OK) h->err = std::string("svs_ba_set_problem: ") + svs_last_error(ba);
-  return rc;
+  if (rc != SVS_OK) { h->err = std::string("svs_ba_set_problem: ") + svs_last_error(ba); return rc; }
+  h->d_win_last = d_win; h->d_act_last = d_act; h->last_P = P; h->last_L = L;
+  h->last_serial = svs::ba_problem_serial(ba);
+  return SVS_OK;
 }
 
 

@@ -29,6 +29,11 @@ __attribute__((visibility("hidden"))) void ba_forget_symbolic(svs_ba* h);
 // lm_user[L] (internal -> caller's landmark), *cur = index of the accepted buffers, the handle's stream
 __attribute__((visibility("hidden"))) int ba_state_on_device(svs_ba* h, const double* const** pose, const double* const** psi,
                                                              const int** lm_user, const int** cur, cudaStream_t* stream, int* P, int* L);
+// serial number of the problem the handle holds, 0 when it holds none.  A fresh value is drawn from one process-wide
+// counter at the start of every set-up (svs_ba_set_problem, _device, _sharded, _from_map; same-structure reuse too),
+// so two set-ups never share one and a caller that recorded it after its own set-up can tell whether that problem is
+// still the one the handle holds
+__attribute__((visibility("hidden"))) unsigned long long ba_problem_serial(const svs_ba* h);
 // keypoints of the last svs_fast_detect* call on this handle, on its device: xy [n][2] in cell order, cell_off [ncells + 1]
 __attribute__((visibility("hidden"))) void fast_device_results(svs_fast* f, const int** d_xy, const int** d_cell_off, int* ncells,
                                                                 int* n, int* device);
