@@ -732,6 +732,60 @@ int svs_map_add_keyframe(svs_map *h, int oldkey, const double *T_newkey_from_old
 /* the edge list of the last assembly (any output may be NULL); E must equal *num_edges */
 int svs_map_last_edges(svs_map *h, int E, int *e_point, int *e_pose, int *e_anchor, double *e_obs, double *e_info);
 
+/* ------------------------------------------------------------------ metric loop verification
+ * Backend::globalLoopClosure (backend.cpp:830-1001) with matchAndAlign (:726-784) on a loop that place recognition
+ * proposed, from the device map, the matcher's keyframe slots and the motion-only LM, and on success
+ * SlamGraph::addLoopClosure's addNewObsToOldPoints on the loop vertex (slam_graph.cpp:220, 400-420).
+ *   Inputs.  query, loop: map vertex indices; T_query_from_loop: the proposal (svs_place_result).  window_vertex[P]: the
+ *     double window (svs_map_select_window).  vertex_slot[V]: the matcher slot holding each vertex's keyframe pyramid,
+ *     -1 = none.  The matcher's current frame must be the loop keyframe: its pyramid, its disparity and its FAST
+ *     corners (recomputeFastCorners, backend.cpp:453-469).  cam: the level-0 stereo camera of the LM and the gate.
+ *   1 Candidates (:844-893).  T_loop_from_world = T_query_from_loop^-1 * T_query_from_world, composed on the device
+ *     from the map.  Every point the query observes whose anchor is in the window, with anchor_level and anchor_obs_pyr
+ *     = centre / 2^level taken from the anchor's own observation of it, whose projection (int)(cam_vec[level].map(
+ *     T_loop_from_world T_anchor^-1 xyz_anchor)) lies in the level image (border 0), in ascending point index (the
+ *     reference's unordered_map order is unspecified).  Every slot then receives its vertex's map pose, loop's slot
+ *     T_loop_from_world (the reference's vertex_table); the slots keep these poses after the call.
+ *   2 matchAndAlign.  svs_match at radius 10 (thr_mean 22, thr_std 10) with T_cur_from_actkey = identity and
+ *     T_actkey_from_w = T_loop_from_world; fewer than covis_thr matches: stage 1.  calcFastMotionOnly on the matches
+ *     with PoseOptimizerParams(true, 2, 25) -> T_align1; svs_match at radius 4 from T_align1; the LM with
+ *     (true, 2, 15) -> T_newloop_from_oldloop; fewer than covis_thr matches: stage 2.  A NaN residual gives
+ *     SVS_ERR_NUMERIC (the reference throws).
+ *   3 Gate (:904-961).  Each match is reprojected with T_newloop_from_oldloop (the projection of the LM); it becomes
+ *     a track when |du|, |dv| < 2 * 2^anchor_level and |du_right| < 6.  ASSUMPTION: `abs` in backend.cpp is read as
+ *     the floating-point overload; nothing in the reference tree confirms which std::abs is selected.  A track counts
+ *     right when u > w/2 (else left) and lower when v > h/2 (else upper), w and h of the matcher's level 0.  Fewer
+ *     than covis_thr tracks: stage 3; a quadrant with fewer than covis_thr / 2 (integer division): stage 4.
+ *   4 Commit, only when verified: T_newloop_from_w = T_newloop_from_oldloop * T_query_from_loop^-1 *
+ *     T_query_from_world, and each track (point, uvu at level 0, anchor_level) becomes an observation of `loop` at
+ *     its ascending-vertex position in the point's list; where loop already observes the point its observation stays
+ *     (std::map::insert), the track is still listed and counted.  Like svs_map_add_keyframe this forgets the last
+ *     assembled window; the pose graph stays (V is unchanged).  The neighbour lists, the edge and the loop constraint
+ *     stay with the caller (svs_computeConstraint_batch with loop placed at T_newloop_from_w, INTEGRATION.md).
+ *   Output.  res: the counts of every stage reached; tracks: track_point / track_uvu [.][3] / track_level, in match
+ *     order, whenever the gate ran (cap >= n_candidates always suffices).  Returns SVS_OK whether or not the loop
+ *     was verified.  Device-side findings come back through one control word; the host reads counts, poses and
+ *     the track list only.
+ *   Refused with SVS_ERR_INVALID, the map and the slots as they were: a NULL argument, an index outside [0, V),
+ *     query == loop, covis_thr < 1, a window vertex listed twice, a slot outside the matcher or used twice, handles
+ *     on different devices, a candidate whose anchor has no slot, no observation of the point or a level the matcher
+ *     lacks, more candidates than the matcher's max_points or the pose handle's max_obs, and cap < n_tracks (the
+ *     sizes needed are in res).  The message is in svs_map_last_error. */
+typedef struct {
+  int verified;                  /* the map was updated */
+  int stage;                     /* 0 verified; 1 first match < covis_thr; 2 second match < covis_thr;
+                                    3 gated tracks < covis_thr; 4 a quadrant < covis_thr / 2 */
+  int n_candidates, n_matched1, n_matched2, n_tracks;
+  int num_left, num_right, num_upper, num_lower;
+  double T_align1[7];            /* T_newloop_from_oldloop after the first LM */
+  double T_newloop_from_oldloop[7], T_newloop_from_w[7];   /* defined when verified */
+  svs_pose_stats lm[2];
+} svs_loop_result;
+int svs_globalLoopClosure(svs_map *map, svs_matcher *m, svs_pose *po, const svs_cam *cam, int covis_thr, int query,
+                          int loop, const double T_query_from_loop[7], int P, const int *window_vertex,
+                          const int *vertex_slot, svs_loop_result *res, int cap, int *track_point, double *track_uvu,
+                          int *track_level);
+
 /* ------------------------------------------------------------------ place recognition
  * PlaceRecognizer::addLocation (placerecognizer.cpp:206-324) after the caller's SURF step: vocabulary words, TF-IDF
  * loop candidates (calcLoopStatistics, :131-172) and geometricCheck (:175-202) = BFMatcher(NORM_L2).match +

@@ -377,6 +377,7 @@ class BA_SE3_XYZ_STEREO {
   BA_SE3_XYZ_STEREO(const BA_SE3_XYZ_STEREO&) = delete;
   BA_SE3_XYZ_STEREO& operator=(const BA_SE3_XYZ_STEREO&) = delete;
   bool valid() const { return ok_; }
+  svs_pose* handle() { return h_; }
   // calcFastMotionOnly(obs_list, prediction(cam), ba_params, &frame, &point_list); throws where the reference does
   OptimizerStatistics calcFastMotionOnly(const std::vector<int>& obs_point_id, const std::vector<double>& obs_uvu,
                                          const svs_cam& cam, const PoseOptimizerParams& ba_params, SE3d* frame,
@@ -589,6 +590,35 @@ class DeviceMap {
     if (rc != SVS_OK) return rc;
     V_ += 1; Np_ += (int)new_anchor.size(); nn_ = 0;
     return v;
+  }
+  // Backend::globalLoopClosure (backend.cpp:830-1001) on this map; semantics: svs_globalLoopClosure.  The matcher holds
+  // the loop keyframe as its current frame and the keyframe pyramids in the slots vertex_slot names.  Returns true when
+  // the loop was verified and the map grew; *res (when given) holds the counts of every stage reached, *tracks the gated
+  // tracks.  Throws std::runtime_error on a refused call and where the reference throws (a NaN residual).
+  struct LoopTracks { std::vector<int> point, level; std::vector<double> uvu; };
+  bool globalLoopClosure(GuidedMatcher& matcher, BA_SE3_XYZ_STEREO& ba, const svs_cam& cam, int covis_thr, int query_id,
+                         int loop_id, const SE3d& T_query_from_loop, const std::vector<int>& window_vertex,
+                         const std::vector<int>& vertex_slot, svs_loop_result* res = nullptr, LoopTracks* tracks = nullptr) {
+    if (!ok_) throw std::runtime_error("no CUDA device");
+    if ((int)vertex_slot.size() != V_) throw std::runtime_error("vertex_slot must name a slot (or -1) for every vertex");
+    const double T[7] = {T_query_from_loop.q[0], T_query_from_loop.q[1], T_query_from_loop.q[2], T_query_from_loop.q[3],
+                         T_query_from_loop.t[0], T_query_from_loop.t[1], T_query_from_loop.t[2]};
+    const int cap = Np_ > 0 ? Np_ : 1;   // tracks <= candidates <= points
+    std::vector<int> tp(cap), tl(cap);
+    std::vector<double> tu(3 * (size_t)cap);
+    svs_loop_result r{};
+    const int rc = svs_globalLoopClosure(h_, matcher.handle(), ba.handle(), &cam, covis_thr, query_id, loop_id, T,
+                                         (int)window_vertex.size(), window_vertex.data(), vertex_slot.data(), &r, cap, tp.data(),
+                                         tu.data(), tl.data());
+    if (res) *res = r;
+    if (rc != SVS_OK) throw std::runtime_error(svs_map_last_error(h_));
+    if (tracks) {
+      const int n = (r.stage == 0 || r.stage >= 3) ? r.n_tracks : 0;
+      tracks->point.assign(tp.begin(), tp.begin() + n);
+      tracks->level.assign(tl.begin(), tl.begin() + n);
+      tracks->uvu.assign(tu.begin(), tu.begin() + 3 * (size_t)n);
+    }
+    return r.verified != 0;
   }
   bool get(std::vector<double>* T_me_from_world, std::vector<double>* xyz_anchor) {
     T_me_from_world->resize(7 * (size_t)V_); xyz_anchor->resize(3 * (size_t)(Np_ > 0 ? Np_ : 1));

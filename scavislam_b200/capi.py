@@ -157,6 +157,14 @@ class SvsPlaceResult(C.Structure):
                 ("ms", C.c_float)]
 
 
+class SvsLoopResult(C.Structure):
+    _fields_ = [("verified", C.c_int), ("stage", C.c_int), ("n_candidates", C.c_int), ("n_matched1", C.c_int),
+                ("n_matched2", C.c_int), ("n_tracks", C.c_int), ("num_left", C.c_int), ("num_right", C.c_int),
+                ("num_upper", C.c_int), ("num_lower", C.c_int), ("T_align1", C.c_double * 7),
+                ("T_newloop_from_oldloop", C.c_double * 7), ("T_newloop_from_w", C.c_double * 7),
+                ("lm", SvsPoseStats * 2)]
+
+
 EXPORTS = [
     "svs_ba_create", "svs_ba_destroy", "svs_last_error", "svs_ba_set_problem", "svs_ba_optimize",
     "svs_ba_get_poses", "svs_ba_get_points", "svs_ba_reset_state", "svs_optimiseInnerAndOuterWindow",
@@ -189,6 +197,7 @@ EXPORTS = [
     "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad", "svs_ba_window_grad",
     "svs_place_create", "svs_place_destroy", "svs_place_last_error", "svs_place_add_location", "svs_place_num_places",
     "svs_place_last_words", "svs_place_last_scores", "svs_place_last_matches", "svs_place_last_hypotheses",
+    "svs_globalLoopClosure",
 ]
 
 
@@ -318,6 +327,8 @@ def lib():
     L.svs_ba_set_problem_from_map.argtypes = [vp, vp, C.c_int, c_ip, c_up, C.c_int, c_ip, C.c_int, c_ip, c_ip, c_dp, c_dp,
                                               C.POINTER(SvsCam), c_ip]
     L.svs_map_last_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp]
+    L.svs_globalLoopClosure.argtypes = [vp, vp, vp, C.POINTER(SvsCam), C.c_int, C.c_int, C.c_int, c_dp, C.c_int, c_ip, c_ip,
+                                        C.POINTER(SvsLoopResult), C.c_int, c_ip, c_dp, c_ip]
     L.svs_constraints_create.argtypes = [C.c_int, C.POINTER(vp)]
     L.svs_constraints_destroy.argtypes = [vp]
     L.svs_constraints_destroy.restype = None
@@ -1430,6 +1441,32 @@ class DeviceMap:
         obs, info = np.zeros((E, 3)), np.zeros((E, 3))
         self._ck(lib().svs_map_last_edges(self._h, E, _ip(ep), _ip(es), _ip(ea), _dp(obs), _dp(info)))
         return ep, es, ea, obs, info
+
+    def global_loop_closure(self, matcher, pose, cam, covis_thr, query, loop, T_query_from_loop, window_vertex, vertex_slot,
+                            cap=None):
+        """Backend::globalLoopClosure on the device (svs_globalLoopClosure): `matcher` (a GuidedMatcher) holds the loop
+        keyframe as its current frame and the keyframe pyramids in the slots vertex_slot names, `pose` is a
+        PoseOptimizer.  Returns (result dict, tracks dict(point, uvu, level)); a verified loop has grown the map."""
+        win = np.ascontiguousarray(window_vertex, np.int32)
+        slot = np.ascontiguousarray(vertex_slot, np.int32)
+        Tq = np.ascontiguousarray(T_query_from_loop, np.float64).reshape(7)
+        cap = max(self.Np, 1) if cap is None else int(cap)
+        tp, tu, tl = np.zeros(max(cap, 1), np.int32), np.zeros((max(cap, 1), 3)), np.zeros(max(cap, 1), np.int32)
+        r = SvsLoopResult()
+        cm = SvsCam(*[float(x) for x in cam])
+        rc = lib().svs_globalLoopClosure(self._h, matcher._h, pose._h, C.byref(cm), int(covis_thr), int(query), int(loop),
+                                         _dp(Tq), len(win), _ip(win), _ip(slot), C.byref(r), cap, _ip(tp), _dp(tu), _ip(tl))
+        out = {f: getattr(r, f) for f in ("verified", "stage", "n_candidates", "n_matched1", "n_matched2", "n_tracks",
+                                          "num_left", "num_right", "num_upper", "num_lower")}
+        for f in ("T_align1", "T_newloop_from_oldloop", "T_newloop_from_w"):
+            out[f] = np.array(getattr(r, f)[:])
+        out["lm"] = [PoseOptimizer._stats(r.lm[k]) for k in range(2)]
+        if rc != 0:
+            err = SvsError(rc, lib().svs_map_last_error(self._h).decode())
+            err.result = out
+            raise err
+        n = out["n_tracks"] if out["stage"] in (0, 3, 4) else 0
+        return out, dict(point=tp[:n].copy(), uvu=tu[:n].copy(), level=tl[:n].copy())
 
 
 def load_surf_vocabulary(path):

@@ -239,17 +239,24 @@ __global__ void k_new_pose(const double* __restrict__ old_pose, int oldkey, cons
   svs::se3_mul(A, B, AB);
   for (int q = 0; q < 7; ++q) out[q] = AB[q];
 }
-__global__ void k_grow_count(int Np_old, int Np_new, const int* __restrict__ old_ptr, const int* __restrict__ add_idx, int* __restrict__ cnt) {
+__device__ __forceinline__ bool observes(const MapDev& m, int p, int v) {
+  for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i)
+    if (m.vis_pose[i] == v) return true;
+  return false;
+}
+// a tracked point gains an observation by `vertex` unless it has one already (std::map::insert keeps the old one)
+__global__ void k_grow_count(MapDev m, int Np_new, int vertex, const int* __restrict__ add_idx, int* __restrict__ cnt) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= Np_new) return;
-  cnt[p] = p < Np_old ? old_ptr[p + 1] - old_ptr[p] + (add_idx[p] >= 0) : 2;
+  cnt[p] = p < m.Np ? m.vis_ptr[p + 1] - m.vis_ptr[p] + (add_idx[p] >= 0 && !observes(m, p, vertex)) : 2;
 }
 __global__ void k_mark_tracks(int n, const int* __restrict__ track_point, int* __restrict__ add_idx) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < n) add_idx[track_point[t]] = t;
 }
-// one thread per point moves its observations to their new place and appends the new keyframe's (its id is the
-// largest, so it is the last of the point's ascending list); a new point is seen by its anchor frame and the keyframe
+// one thread per point moves its observations to their new place and inserts the tracked vertex's before the first
+// observation by a larger vertex (a new keyframe's id is the largest: it goes last); a new point is seen by its anchor
+// frame and the keyframe
 __global__ void k_grow_move(MapDev m, int Np_new, int newkey, const int* __restrict__ add_idx, const int* __restrict__ new_ptr,
                             const double* __restrict__ track_center, const int* __restrict__ track_level,
                             const int* __restrict__ new_anchor, const double* __restrict__ new_anchor_center,
@@ -265,9 +272,13 @@ __global__ void k_grow_move(MapDev m, int Np_new, int newkey, const int* __restr
     ++at;
   };
   if (p < m.Np) {
-    for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i) put(m.vis_pose[i], m.center + 3 * (size_t)i, m.level[i]);
     const int t = add_idx[p];
-    if (t >= 0) put(newkey, track_center + 3 * (size_t)t, track_level[t]);
+    bool pending = t >= 0 && !observes(m, p, newkey);
+    for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i) {
+      if (pending && m.vis_pose[i] > newkey) { put(newkey, track_center + 3 * (size_t)t, track_level[t]); pending = false; }
+      put(m.vis_pose[i], m.center + 3 * (size_t)i, m.level[i]);
+    }
+    if (pending) put(newkey, track_center + 3 * (size_t)t, track_level[t]);
   } else {
     const int q = p - m.Np;
     put(new_anchor[q], new_anchor_center + 3 * (size_t)q, new_anchor_level[q]);
@@ -735,7 +746,7 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
   // observations
   if (Np2) {
     if (n_track) k_mark_tracks<<<(n_track + 255) / 256, 256, 0, h->stream>>>(n_track, Ii(s_tp), Ii(s_add));
-    k_grow_count<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(Np, Np2, h->m.vis_ptr, Ii(s_add), Ii(s_cnt));
+    k_grow_count<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, Ii(s_add), Ii(s_cnt));
     k_scan<<<1, 1024, 0, h->stream>>>(Ii(s_cnt), Np2, reinterpret_cast<int*>(B2 + lo.o_vptr));
     k_grow_move<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, Ii(s_add), reinterpret_cast<const int*>(B2 + lo.o_vptr), D(s_tc),
                                                         Ii(s_tl), Ii(s_na), D(s_nac), Ii(s_nal), D(s_nc), Ii(s_nl),
@@ -769,3 +780,58 @@ int svs_map_last_edges(svs_map* h, int E, int* e_point, int* e_pose, int* e_anch
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------ hooks of loop.cu (internal.cuh)
+
+void svs::map_view(svs_map* h, MapView* v) {
+  v->V = h->V; v->Np = h->Np; v->nnz = h->nnz; v->device = h->device; v->stream = h->stream;
+  v->pose = h->m.pose; v->anchor = h->m.anchor; v->xyz = h->m.xyz; v->vis_ptr = h->m.vis_ptr; v->vis_pose = h->m.vis_pose;
+  v->center = h->m.center; v->level = h->m.level;
+}
+
+void svs::map_set_error(svs_map* h, const char* msg) { h->err = msg; }
+
+void svs::launch_scan(const int* cnt, int n, int* ptr, cudaStream_t stream) { k_scan<<<1, 1024, 0, stream>>>(cnt, n, ptr); }
+
+int svs::map_add_observations(svs_map* h, int vertex, int n, const int* d_point, const double* d_center, const int* d_level) {
+  const int V = h->V, Np = h->Np, nnz = h->nnz;
+  if (n == 0 || Np == 0) return SVS_OK;
+  cudaSetDevice(h->device);
+  // the new tables are sized for n more observations; nnz becomes what the scan counted (a point the vertex already
+  // observes gains none)
+  const MapLayout lo = map_layout(V, Np, nnz + n);
+  const size_t s_add = 0, s_cnt = al256(sizeof(int) * (size_t)Np), need = 2 * s_cnt;
+  GCK(cudaStreamSynchronize(h->stream));
+  if (need > h->upd_cap) {
+    cudaFree(h->d_upd); h->d_upd = nullptr; h->upd_cap = 0;
+    GCK(cudaMalloc(&h->d_upd, 2 * need));
+    h->upd_cap = 2 * need;
+  }
+  char* B2 = nullptr;
+  GCK(cudaMalloc(&B2, lo.total + lo.total / 4));
+  int* add = reinterpret_cast<int*>(h->d_upd + s_add);
+  int* cnt = reinterpret_cast<int*>(h->d_upd + s_cnt);
+  int nnz2 = 0;
+  cudaError_t e = cudaMemsetAsync(add, 0xff, sizeof(int) * (size_t)Np, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_pose, h->m.pose, sizeof(double) * 7 * (size_t)V, cudaMemcpyDeviceToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_anch, h->m.anchor, sizeof(int) * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_xyz, h->m.xyz, sizeof(double) * 3 * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
+  int* vptr2 = reinterpret_cast<int*>(B2 + lo.o_vptr);
+  if (e == cudaSuccess) {
+    k_mark_tracks<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_point, add);
+    k_grow_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, Np, vertex, add, cnt);
+    k_scan<<<1, 1024, 0, h->stream>>>(cnt, Np, vptr2);
+    k_grow_move<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, Np, vertex, add, vptr2, d_center, d_level, nullptr, nullptr,
+                                                        nullptr, nullptr, nullptr, reinterpret_cast<int*>(B2 + lo.o_vpose),
+                                                        reinterpret_cast<double*>(B2 + lo.o_cen), reinterpret_cast<int*>(B2 + lo.o_lvl));
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&nnz2, vptr2 + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) { cudaFree(B2); h->err = std::string("map_add_observations: ") + cudaGetErrorString(e); return SVS_ERR_CUDA; }
+  cudaFree(h->d_map);
+  h->d_map = B2; h->map_cap = lo.total + lo.total / 4;
+  map_bind(h, B2, lo, V, Np, nnz2);
+  h->d_win_last = nullptr;   // the window's observations changed; the pose graph (V vertices) stays
+  return SVS_OK;
+}

@@ -1,5 +1,7 @@
 // internal.cuh -- cross-module hooks inside libsvsb200.so (not part of the C ABI)
 #pragma once
+#include <cuda_runtime.h>
+
 #include "../../include/svs_b200.h"
 
 namespace svs {
@@ -37,4 +39,42 @@ __attribute__((visibility("hidden"))) unsigned long long ba_problem_serial(const
 // keypoints of the last svs_fast_detect* call on this handle, on its device: xy [n][2] in cell order, cell_off [ncells + 1]
 __attribute__((visibility("hidden"))) void fast_device_results(svs_fast* f, const int** d_xy, const int** d_cell_off, int* ncells,
                                                                 int* n, int* device);
+
+// the matcher's shape and where its keyframe slots keep their poses: slot s's T_me_from_w[7] lies at
+// (char*)slot_T + s * slot_stride on the device
+struct MatcherView {
+  int device, nlevels, max_kf, max_pts;
+  svs_match_level lv[SVS_MATCH_MAX_LEVELS];
+  double* slot_T;
+  size_t slot_stride;
+};
+__attribute__((visibility("hidden"))) void matcher_view(svs_matcher* m, MatcherView* v);
+// svs_match on candidate points that already lie on the matcher's device (read once the call is made); the results stay
+// on the device for matcher_device_results / svs_calcFastMotionOnly_matched.  Returns after the kernel has finished.
+__attribute__((visibility("hidden"))) int match_device(svs_matcher* m, const double T_cur_from_actkey[7],
+                                                       const double T_actkey_from_w[7], const svs_match_point* d_pts, int n,
+                                                       int search_radius, int thr_mean, int thr_std);
+__attribute__((visibility("hidden"))) void pose_capacity(const svs_pose* h, int* device, int* max_obs);
+
+// the device map's tables as they lie now (valid until the map is next changed) and its stream
+struct MapView {
+  int V, Np, nnz, device;
+  cudaStream_t stream;
+  const double* pose;       // [V][7]
+  const int* anchor;        // [Np]
+  const double* xyz;        // [Np][3]
+  const int* vis_ptr;       // [Np+1]
+  const int* vis_pose;      // [nnz]
+  const double* center;     // [nnz][3]
+  const int* level;         // [nnz]
+};
+__attribute__((visibility("hidden"))) void map_view(svs_map* h, MapView* v);
+__attribute__((visibility("hidden"))) void map_set_error(svs_map* h, const char* msg);
+// exclusive scan of n counts into ptr[n + 1] by one CTA on `stream` (graph.cu's k_scan)
+__attribute__((visibility("hidden"))) void launch_scan(const int* cnt, int n, int* ptr, cudaStream_t stream);
+// addNewObsToOldPoints (slam_graph.cpp:400-420) for an existing vertex: n distinct points (device arrays on the map's
+// device, ready on its stream) gain an observation by `vertex` at its ascending-vertex position in their lists; a point
+// the vertex already observes keeps its observation.  Forgets the last assembled window, keeps the pose graph.
+__attribute__((visibility("hidden"))) int map_add_observations(svs_map* h, int vertex, int n, const int* d_point,
+                                                               const double* d_center, const int* d_level);
 }  // namespace svs

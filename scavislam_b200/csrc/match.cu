@@ -12,6 +12,7 @@
 // -fmad=false and written operation by operation like the CPU oracle so that the uint8
 // truncation of the warped patch is bit-identical.
 #include <algorithm>
+#include <cstddef>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -287,7 +288,51 @@ namespace svs {
 void matcher_device_results(svs_matcher* m, const svs_match_result** d_res, int* n, int* device) {
   *d_res = m->d_res; *n = m->last_n; *device = m->device;
 }
+void matcher_view(svs_matcher* m, MatcherView* v) {
+  v->device = m->device; v->nlevels = m->nlevels; v->max_kf = m->max_kf; v->max_pts = m->max_pts;
+  for (int l = 0; l < kMaxLv; ++l) v->lv[l] = l < m->nlevels ? m->lv[l] : svs_match_level{};
+  v->slot_T = reinterpret_cast<double*>(reinterpret_cast<char*>(m->d_kf) + offsetof(KfDev, T));
+  v->slot_stride = sizeof(KfDev);
+}
 }  // namespace svs
+
+// k_match on n candidate points at d_pts (device memory of the handle's device); the results stay in h->d_res
+static int match_launch(svs_matcher* h, const double T_cur_from_actkey[7], const double T_actkey_from_w[7],
+                        const svs_match_point* d_pts, int n, int search_radius, int thr_mean, int thr_std) {
+  MatchArgs a;
+  memset(&a, 0, sizeof a);
+  a.nlevels = h->nlevels;
+  for (int l = 0; l < h->nlevels; ++l) {
+    LvDev& L = a.lv[l];
+    L.w = h->lv[l].w; L.h = h->lv[l].h; L.f = h->lv[l].f; L.px = h->lv[l].px; L.py = h->lv[l].py;
+    L.cur = h->d_cur[l]; L.cur_pitch = h->pitch[l];
+    L.kp_xy = h->d_kp_xy[l]; L.kp_content = h->d_kp_content[l];
+    L.bucket_ptr = h->d_bucket_ptr[l]; L.bucket_item = h->d_bucket_item[l];
+    L.nkp = h->nkp[l]; L.bw = h->bw[l]; L.bh = h->bh[l];
+  }
+  a.kf = h->d_kf; a.nkf = h->max_kf;
+  a.disp = h->d_disp; a.disp_pitch = h->disp_pitch;
+  a.radius = search_radius; a.thr_mean = thr_mean; a.thr_std = thr_std;
+  memcpy(a.T_cur_from_actkey, T_cur_from_actkey, sizeof(double) * 7);
+  memcpy(a.T_actkey_from_w, T_actkey_from_w, sizeof(double) * 7);
+  k_match<<<(n + kWarps - 1) / kWarps, kWarps * 32, 0, h->stream>>>(a, d_pts, n, h->d_res);
+  MCK(cudaGetLastError());
+  return SVS_OK;
+}
+
+int svs::match_device(svs_matcher* h, const double T_cur_from_actkey[7], const double T_actkey_from_w[7],
+                      const svs_match_point* d_pts, int n, int search_radius, int thr_mean, int thr_std) {
+  svs::NvtxRange nvtx_("match");
+  h->last_n = 0;
+  if (n < 0 || n > h->max_pts || search_radius < 0) { h->err = "match_device: bad point count or radius"; return SVS_ERR_INVALID; }
+  if (n == 0) return SVS_OK;
+  cudaSetDevice(h->device);
+  const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, d_pts, n, search_radius, thr_mean, thr_std);
+  if (rc != SVS_OK) return rc;
+  MCK(cudaStreamSynchronize(h->stream));
+  h->last_n = n;
+  return SVS_OK;
+}
 
 extern "C" {
 
@@ -467,25 +512,9 @@ int svs_match(svs_matcher * h, const double T_cur_from_actkey[7], const double T
   h->last_n = 0;
   if (n == 0) return 0;
   cudaSetDevice(h->device);
-  MatchArgs a;
-  memset(&a, 0, sizeof a);
-  a.nlevels = h->nlevels;
-  for (int l = 0; l < h->nlevels; ++l) {
-    LvDev& L = a.lv[l];
-    L.w = h->lv[l].w; L.h = h->lv[l].h; L.f = h->lv[l].f; L.px = h->lv[l].px; L.py = h->lv[l].py;
-    L.cur = h->d_cur[l]; L.cur_pitch = h->pitch[l];
-    L.kp_xy = h->d_kp_xy[l]; L.kp_content = h->d_kp_content[l];
-    L.bucket_ptr = h->d_bucket_ptr[l]; L.bucket_item = h->d_bucket_item[l];
-    L.nkp = h->nkp[l]; L.bw = h->bw[l]; L.bh = h->bh[l];
-  }
-  a.kf = h->d_kf; a.nkf = h->max_kf;
-  a.disp = h->d_disp; a.disp_pitch = h->disp_pitch;
-  a.radius = search_radius; a.thr_mean = thr_mean; a.thr_std = thr_std;
-  memcpy(a.T_cur_from_actkey, T_cur_from_actkey, sizeof(double) * 7);
-  memcpy(a.T_actkey_from_w, T_actkey_from_w, sizeof(double) * 7);
   MCK(cudaMemcpyAsync(h->d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  k_match<<<(n + kWarps - 1) / kWarps, kWarps * 32, 0, h->stream>>>(a, h->d_pts, n, h->d_res);
-  MCK(cudaGetLastError());
+  const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, h->d_pts, n, search_radius, thr_mean, thr_std);
+  if (rc != SVS_OK) return rc;
   MCK(cudaMemcpyAsync(out, h->d_res, sizeof(svs_match_result) * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
   MCK(cudaStreamSynchronize(h->stream));
   h->last_n = n;

@@ -647,6 +647,8 @@ struct svs_pose {
     }                                                                   \
   } while (0)
 
+void svs::pose_capacity(const svs_pose* h, int* device, int* max_obs) { *device = h->device; *max_obs = h->max_obs; }
+
 // true when p is device (or managed) memory of the handle's device
 static bool on_handle_device(const svs_pose* h, const void* p) {
   cudaPointerAttributes a{};
