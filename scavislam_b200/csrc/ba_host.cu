@@ -1374,10 +1374,11 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     long long dbg[64];
     cudaMemcpy(dbg, d.dbg, sizeof dbg, cudaMemcpyDeviceToHost);
     fprintf(stderr, "k_solve cycles since setup (branch factored, cluster sync, separators factored, separators solved + sync, "
-            "branch solved, end):\n");
+            "branch solved with its pose update, end), then the setup from the wait for the build on:\n");
     for (int g = 0; g < 2; ++g) {
       fprintf(stderr, "  CTA %d:", g);
       for (int i = 0; i < 6; ++i) fprintf(stderr, " %lld", dbg[g * 6 + i]);
+      fprintf(stderr, " setup %lld", dbg[27 + 16 * g]);
       const long long* q = dbg + 12 + 16 * g;
       if (!roles) { fprintf(stderr, "\n"); continue; }
       fprintf(stderr, "\n     chain: hand-over %lld chol %lld wait-urgent+load %lld publish %lld | unit thread 8: loop-top+factor %lld wait-rows %lld "

@@ -73,6 +73,10 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
 }
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
+  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(s), "l"(gmem));
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 
@@ -635,48 +639,156 @@ __device__ void factor_range(const BaDev& d, const Team& T, const SolveShared& S
 // `buf` (2 x half blocks) in chunks of whole rows, double buffered: warp 0 walks the chain while the other warps
 // fetch the next chunk.  Per row the chain is one shared-memory round trip (x_i) and six FMAs; no reduction across
 // lanes, no shuffles.  Only blocks whose column lies in [c0, c1) are applied.
+//
+// A branch's pass walks two row ranges as one stream of chunks: the separator rows (x known, only scattered), then
+// its own rows.  Positions v in [0, n) count up through [b0, b1) and then [a0, a1); the walk runs from n down to 0 and
+// no chunk crosses from one range into the other.
 constexpr int kMaxChunks = 48;
-__device__ void scatter_rows(const BaDev& d, int lo, int hi, int c0, int c1, int buf_off, int half, const SolveShared& S,
-                             int* sChunk) {
+struct Walk {
+  int a0, a1, b0, b1;   // rows [a0, a1) first, then [b0, b1)
+  __device__ __forceinline__ int n() const { return (a1 - a0) + (b1 - b0); }
+  __device__ __forceinline__ int row(int v) const { return v < b1 - b0 ? b0 + v : a0 + v - (b1 - b0); }
+  __device__ __forceinline__ int floor(int v) const { return v > b1 - b0 ? b1 - b0 : 0; }   // lowest position of the
+                                                                                           // range of position v - 1
+};
+
+// Chunk boundaries of the positions [0, top): top = b[0] > b[1] > ... (positions [b[k+1], b[k]) form chunk k: the
+// longest run of whole rows of one range of at most `half` blocks, or one row if it is longer), at most kMaxChunks of
+// them, their count in sChunk[kMaxChunks + 1].  One warp: the lanes test 32 candidate lower ends of a chunk at once
+// (the block count of a run only grows as its lower end moves down, so the first lane that stops is the greedy end).
+__device__ void plan_chunks(const int* rptr, const Walk& W, int top, int half, int* sChunk) {
+  const int lane = threadIdx.x & 31;
+  int n = 0, a = top;
+  if (lane == 0) sChunk[0] = top;
+  while (a > 0 && n < kMaxChunks) {
+    const int lo = W.floor(a), end = rptr[W.row(a - 1) + 1];
+    int b = lo;
+    for (int base = a - 1;; base -= 32) {
+      const int c = base - lane;
+      const bool stop = c <= lo || end - rptr[W.row(c - 1)] > half;
+      const unsigned m = __ballot_sync(0xffffffffu, stop);
+      if (m) { b = base - (__ffs(m) - 1); break; }
+    }
+    ++n;
+    if (lane == 0) sChunk[n] = b;
+    a = b;
+  }
+  if (lane == 0) sChunk[kMaxChunks + 1] = n;
+}
+
+// Chunk k into its half of the buffer (cp.async, one commit group), by threads tid of nth.
+__device__ __forceinline__ void load_chunk(const BaDev& d, const int* rptr, const Walk& W, const int* sChunk, int k,
+                                           int buf_off, int half, int tid, int nth) {
+  const int b0 = rptr[W.row(sChunk[k + 1])], n16 = (rptr[W.row(sChunk[k] - 1) + 1] - b0) * 18;
+  double* dst = sm_solve + buf_off + (k & 1) * half * 36;
+  const double* src = d.Nrow + (size_t)b0 * 36;
+  for (int c = tid; c < n16; c += nth) cp_async16(dst + 2 * (size_t)c, src + 2 * (size_t)c);
+  cp_async_commit();
+}
+
+// The first round of a backward pass (its chunk plan, and the first chunk in flight), so that a CTA can do it while it
+// waits for the other one; scatter_rows(..., planned = true) then starts with the rows.
+__device__ void plan_rows(const BaDev& d, const Walk& W, int top, int buf_off, int half, const SolveShared& S, int* sChunk) {
+  if (threadIdx.x < 32) plan_chunks(S.upd_ptr, W, top, half, sChunk);
+  bar_sync(kBarBack, kSolveThreads);
+  if (top > 0) load_chunk(d, S.upd_ptr, W, sChunk, 0, buf_off, half, threadIdx.x, kSolveThreads);
+}
+
+// The pose update (G2oVertexSE3::oplusImpl) rides behind the backward pass: once a chunk of rows is done, x of its rows
+// is final, and during the next chunk the warps that do not share warp 0's scheduler apply exp(dx) T of those rows
+// into the trial buffer (pose and Rt of 1 - cur, and dx into d.x).  Row i is taken by pose thread i % kPoseThreads.
+// A thread adds its rows' terms of scale = sum dx (lambda dx + b) into its own sum in the order it takes them (chunks in
+// walking order, rows ascending inside a chunk); the threads' sums meet in the kernel's fixed reduction.  So the order
+// is fixed by the structure alone.
+constexpr int kPoseThreads = 9 * 32;
+__device__ __forceinline__ int pose_thread(int warp, int lane) { return (warp & 3) ? (warp - (warp >> 2) - 1) * 32 + lane : -1; }
+struct PoseTail {
+  bool on_a, on_b;  // update the poses of the rows [a0, a1) / [b0, b1) of the walk
+  double lambda;
+  int cur;
+};
+struct PoseIn {     // what the update of row j reads besides x_j: fetched one chunk ahead
+  int j, p;
+  double b[6], T[7];
+};
+__device__ __forceinline__ void pose_load(const BaDev& d, int cur, int j, PoseIn& q) {
+  q.j = j;
+  q.p = d.perm[j];
+#pragma unroll
+  for (int rr = 0; rr < 6; ++rr) q.b[rr] = d.bp[6 * q.p + rr];
+#pragma unroll
+  for (int rr = 0; rr < 7; ++rr) q.T[rr] = d.pose[cur][7 * (size_t)q.p + rr];
+}
+__device__ __forceinline__ void pose_apply(const BaDev& d, const PoseIn& q, const double* xj, bool fixed, double lambda,
+                                           int cur, double& sc) {
+  const int p = q.p;
+  double dx[6], Tn[7];
+#pragma unroll
+  for (int rr = 0; rr < 6; ++rr) {
+    dx[rr] = fixed ? 0. : xj[rr];
+    sc += dx[rr] * (lambda * dx[rr] + q.b[rr]);
+  }
+  if (fixed) {
+#pragma unroll
+    for (int rr = 0; rr < 7; ++rr) Tn[rr] = q.T[rr];
+  } else {
+    double dT[7];
+    se3_exp(dx, dT);
+    se3_mul(dT, q.T, Tn);
+  }
+  double R[9];
+  quat_to_R(Tn, R);
+#pragma unroll
+  for (int rr = 0; rr < 6; ++rr) d.x[6 * p + rr] = dx[rr];
+#pragma unroll
+  for (int rr = 0; rr < 7; ++rr) d.pose[1 - cur][7 * (size_t)p + rr] = Tn[rr];
+#pragma unroll
+  for (int rr = 0; rr < 9; ++rr) d.Rt[1 - cur][12 * (size_t)p + rr] = R[rr];
+  d.Rt[1 - cur][12 * (size_t)p + 9] = Tn[4];
+  d.Rt[1 - cur][12 * (size_t)p + 10] = Tn[5];
+  d.Rt[1 - cur][12 * (size_t)p + 11] = Tn[6];
+}
+
+__device__ void scatter_rows(const BaDev& d, const Walk& W, int c0, int c1, int buf_off, int half, const SolveShared& S,
+                             int* sChunk, bool planned, const PoseTail& pt, double& sc) {
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const int* rptr = S.upd_ptr;   // the forward pass's index arrays have been replaced by the row-major ones
   const int* rcol = S.row_idx;
   double* xv = sm_solve + S.yv_off;
   const int r = lane % 6, g = lane / 6;   // five lane groups take the blocks of a row; lanes 30, 31 idle
-  for (int top = hi; top > lo;) {
-    // chunk boundaries top = b[0] > b[1] > ... (rows [b[k+1], b[k]) form chunk k), worked out once by one thread
-    if (t == 0) {
-      int n = 0, a = top;
-      sChunk[0] = top;
-      while (a > lo && n < kMaxChunks) {
-        int b = a - 1;
-        while (b > lo && rptr[a] - rptr[b - 1] <= half) --b;
-        sChunk[++n] = b;
-        a = b;
-      }
-      sChunk[kMaxChunks + 1] = n;
+  const int pw = (pt.on_a || pt.on_b) ? pose_thread(warp, lane) : -1;
+  PoseIn pin;
+  pin.j = -1;
+  // the rows [lo, hi) of chunk k, whether their poses are updated, this pose thread's first row there (or one past the
+  // chunk), and the update of every one of its rows there
+  auto chunk_rows = [&](int k, int& lo, int& hi) { lo = W.row(sChunk[k + 1]); hi = W.row(sChunk[k] - 1) + 1; };
+  auto chunk_poses = [&](int k) { return sChunk[k + 1] >= W.b1 - W.b0 ? pt.on_a : pt.on_b; };
+  auto first_row = [&](int lo) { return lo + (pw - lo % kPoseThreads + kPoseThreads) % kPoseThreads; };
+  auto poses_of = [&](int k) {
+    if (!chunk_poses(k)) return;
+    int lo, hi;
+    chunk_rows(k, lo, hi);
+    for (int i = first_row(lo); i < hi; i += kPoseThreads) {
+      if (i != pin.j) pose_load(d, pt.cur, i, pin);
+      pose_apply(d, pin, xv + 6 * i, S.sfix[i], pt.lambda, pt.cur, sc);
     }
-    bar_sync(kBarBack, kSolveThreads);
-    const int nchunks = sChunk[kMaxChunks + 1];
-    auto load_chunk = [&](int k, int tid, int nth) {
-      const int b0 = rptr[sChunk[k + 1]], n16 = (rptr[sChunk[k]] - b0) * 18;
-      double* dst = sm_solve + buf_off + (k & 1) * half * 36;
-      const double* src = d.Nrow + (size_t)b0 * 36;
-      for (int c = tid; c < n16; c += nth) cp_async16(dst + 2 * (size_t)c, src + 2 * (size_t)c);
-      cp_async_commit();
-    };
-    load_chunk(0, t, kSolveThreads);
+  };
+  for (int top = W.n(); top > 0; planned = false) {
+    if (!planned) plan_rows(d, W, top, buf_off, half, S, sChunk);
     cp_async_wait_all();
     bar_sync(kBarBack, kSolveThreads);
+    const int nchunks = sChunk[kMaxChunks + 1];
     for (int k = 0; k < nchunks; ++k) {
-      if (k + 1 < nchunks && warp > 0) load_chunk(k + 1, t - 32, kSolveThreads - 32);
+      if (k + 1 < nchunks && warp > 0) load_chunk(d, rptr, W, sChunk, k + 1, buf_off, half, t - 32, kSolveThreads - 32);
       if (warp == 0) {
         const double* b = sm_solve + buf_off + (k & 1) * half * 36;
-        const int rlo = sChunk[k + 1], b0 = rptr[rlo];
+        int rlo, rhi;
+        chunk_rows(k, rlo, rhi);
+        const int b0 = rptr[rlo];
         // Software pipeline: everything of a row that does not depend on x -- its block range, this lane's first
         // block (column and the N row) -- is fetched while the previous row is being scattered; what is left on the
         // chain per row is the read of x_i, six FMAs and the read-modify-write of the target column.
-        int i = sChunk[k] - 1;
+        int i = rhi - 1;
         int p0 = 0, nb = 0, col = -1, colB = -1;
         double Nt[6] = {0, 0, 0, 0, 0, 0}, NtB[6] = {0, 0, 0, 0, 0, 0};
         auto prefetch = [&](int row) {   // two blocks per lane group (g and g + 5): a window row has 7-8 blocks
@@ -721,35 +833,29 @@ __device__ void scatter_rows(const BaDev& d, int lo, int hi, int c0, int c1, int
             }
           __syncwarp();
         }
+      } else if (pw >= 0) {
+        if (k > 0) poses_of(k - 1);   // chunk k - 1 is done: x of its rows is final
+        int lo, hi;                   // what the updates of chunk k read besides x, in flight during this chunk
+        chunk_rows(k, lo, hi);
+        const int i = first_row(lo);
+        if (chunk_poses(k) && i < hi) pose_load(d, pt.cur, i, pin);
       }
       cp_async_wait_all();
       bar_sync(kBarBack, kSolveThreads);
     }
+    if (pw >= 0 && nchunks > 0) poses_of(nchunks - 1);
     top = sChunk[nchunks];
     bar_sync(kBarBack, kSolveThreads);   // sChunk is rewritten by the next round
   }
 }
 
-//   rows [k0, k1): x already known (separator rows of a branch), only scattered;  rows [j0, j1): solved here.
-//   S.yv holds c (= z for the columns of the range, x elsewhere).
-__device__ void backsolve_rows(const BaDev& d, int j0, int j1, int k0, int k1, int buf_off, int half, const SolveShared& S,
-                               int* sChunk) {
-  if (j0 >= j1) return;
-  double* xv = sm_solve + S.yv_off;
-  for (int i = 6 * j0 + (int)threadIdx.x; i < 6 * j1; i += kSolveThreads) xv[i] = d.ywork[i];   // c <- z
-  __syncthreads();
-  scatter_rows(d, k0, k1, j0, j1, buf_off, half, S, sChunk);
-  scatter_rows(d, j0, j1, j0, j1, buf_off, half, S, sChunk);
-}
-
 // Between the forward and the backward pass the column-oriented index arrays in shared memory (upd_ptr, row_idx)
-// are replaced by the row-oriented ones (rptr, rcol).
-__device__ void load_row_index(const BaDev& d, const SolveShared& S) {
-  const int t = threadIdx.x;
-  __syncthreads();
-  for (int i = t; i <= d.P; i += kSolveThreads) S.upd_ptr[i] = d.rptr[i];
-  for (int i = t; i < d.nblk - d.P; i += kSolveThreads) S.row_idx[i] = d.rcol[i];
-  __syncthreads();
+// are replaced by the row-oriented ones (rptr, rcol): entries [r0, r1) of rptr and [e0, e1) of rcol, in flight as one
+// cp.async group.
+__device__ void load_row_index(const BaDev& d, const SolveShared& S, int r0, int r1, int e0, int e1) {
+  for (int i = r0 + (int)threadIdx.x; i < r1; i += kSolveThreads) cp_async4(S.upd_ptr + i, d.rptr + i);
+  for (int i = e0 + (int)threadIdx.x; i < e1; i += kSolveThreads) cp_async4(S.row_idx + i, d.rcol + i);
+  cp_async_commit();
 }
 
 // smem layout: [ring: cap*36 doubles][area: nsep*36 doubles][y: 6P doubles][meta ints: col_ptr (P+1),
@@ -766,25 +872,14 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   __shared__ __align__(16) double sCdiag[22];
   __shared__ int sXfail;   // written by the other CTA of the cluster
   __shared__ int sChunk[kMaxChunks + 2];
-  pdl_wait();
-  pdl_launch_dependents();
-  LmCtl* ctl = d.ctl;
-  if (ctl->max_iters > 0 && (ctl->stop || ctl->iter >= ctl->max_iters)) return;   // speculatively enqueued trial: nothing left to do
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank();
   const int t = threadIdx.x, nt = kSolveThreads, lane = t & 31, warp = t >> 5;
-  const unsigned long long t_start = global_ns();
-  if (rank == 0 && t == 0 && ctl->t_build_start) {   // the build before this launch has completed
-    ctl->ns_build += (long long)(t_start - ctl->t_build_start);
-    ctl->t_build_start = 0;
-  }
   const int P = d.P, nblk = d.nblk;
-  const double lambda = ctl->lambda;
-  const int cur = ctl->cur;
-  long long* const timeline = (kTimeline && d.dbg) ? d.dbg + 160 : nullptr;
-  if (timeline && rank == 0 && t == 0) timeline[2 * d.P + 1] = (long long)global_ns();
   const int G = d.nbranch;                 // 1: a single chain, 2: two ends + separator (cluster of 2 CTAs)
   const int sep0 = d.branch_ptr[G];        // first separator column (= P when G == 1)
+  const int my0 = d.branch_ptr[rank], my1 = d.branch_ptr[rank + 1];   // this CTA's branch
+  const int sep_blk0 = G > 1 ? d.col_ptr[sep0] : nblk;
   SolveShared S;
   const int ring_off = 0, area_off = cap * 36;
   double* area = sm_solve + area_off;
@@ -800,18 +895,43 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   for (int i = t; i <= P; i += nt) { S.col_ptr[i] = d.col_ptr[i]; S.upd_ptr[i] = d.upd_ptr[i]; }
   for (int i = t; i < nblk; i += nt) S.row_idx[i] = d.row_idx[i];
   for (int i = t; i < P; i += nt) S.sfix[i] = d.fixed[d.perm[i]];
-  const int my0 = d.branch_ptr[rank], my1 = d.branch_ptr[rank + 1];   // this CTA's branch
-  for (int i = t; i < 6 * P; i += nt) {   // right-hand side in elimination order: bs = bp - bc
-    const int j = i / 6, rr = i - 6 * j;
-    const bool mine = (j >= my0 && j < my1) || (rank == 0 && j >= sep0);
-    double v = 0.;
-    if (mine) { const int p = d.perm[j]; v = d.bp[6 * p + rr] - d.bc[6 * p + rr]; }
-    yv_k[i] = v;
+  const int p_first = t < P ? d.perm[t] : 0;   // the pose of this thread's first right-hand-side row
+  const int rsep = d.rptr[sep0];               // row-major blocks of the rows before the separator
+  // Everything above is the problem's structure, which no kernel of a trial writes, so it is staged before the wait.
+  // In a chained trial every kernel executes pdl_wait() before pdl_launch_dependents(): the CTAs of this launch exist
+  // only once k_build_wave is past its own wait, i.e. once everything enqueued before the build has completed (the
+  // problem's set-up included).  What the build writes (S, bp, bc) and the control block (lambda, cur, the early exit)
+  // are read below the wait.  Without programmatic serialisation (pdl == 0) the wait returns at once and the launch
+  // itself follows the previous kernel.
+  pdl_wait();
+  pdl_launch_dependents();
+  LmCtl* ctl = d.ctl;
+  if (ctl->max_iters > 0 && (ctl->stop || ctl->iter >= ctl->max_iters)) return;   // speculatively enqueued trial: nothing left to do
+  const unsigned long long t_start = global_ns();
+  const long long c_start = clock64();
+  if (rank == 0 && t == 0 && ctl->t_build_start) {   // the build before this launch has completed
+    ctl->ns_build += (long long)(t_start - ctl->t_build_start);
+    ctl->t_build_start = 0;
   }
-  const int sep_blk0 = G > 1 ? d.col_ptr[sep0] : nblk;
+  const double lambda = ctl->lambda;
+  const int cur = ctl->cur;
+  long long* const timeline = (kTimeline && d.dbg) ? d.dbg + 160 : nullptr;
+  if (timeline && rank == 0 && t == 0) timeline[2 * d.P + 1] = (long long)global_ns();
   if (G > 1) {   // separator blocks: CTA 0 starts from S, CTA 1 from zero; both accumulate their branch's updates
-    for (int i = t; i < nsep * 36; i += nt) area[i] = rank == 0 ? d.S[(size_t)sep_blk0 * 36 + i] : 0.;
+    if (rank == 0) {
+      for (int i = t; i < nsep * 18; i += nt) cp_async16(area + 2 * i, d.S + (size_t)sep_blk0 * 36 + 2 * i);
+      cp_async_commit();
+    } else {
+      for (int i = t; i < nsep * 36; i += nt) area[i] = 0.;
+    }
   }
+  for (int j = t; j < P; j += nt) {   // right-hand side in elimination order: bs = bp - bc
+    const bool mine = (j >= my0 && j < my1) || (rank == 0 && j >= sep0);
+    const int p = j == t ? p_first : d.perm[j];
+#pragma unroll
+    for (int rr = 0; rr < 6; ++rr) yv_k[6 * j + rr] = mine ? d.bp[6 * p + rr] - d.bc[6 * p + rr] : 0.;
+  }
+  cp_async_wait_all();
   __syncthreads();
   long long tk[8];
   tk[0] = clock64();
@@ -823,7 +943,18 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
   br.timeline = timeline;
   factor_range<kTimeline, kDiag>(d, br, S, lambda);
   tk[1] = clock64();
+  // In flight from here on: c = z on the branch rows, where the backward pass starts (the separator phase touches only
+  // the separator rows of y), and the row-major index.  CTA 0 of two keeps the separator's part of the column-major one
+  // until the separator is factored: rptr[0, sep0) and rcol[0, rptr[sep0]) lie below everything the separator's
+  // columns read (upd_ptr[sep0, P], row_idx from col_ptr[sep0] on).
+  for (int i = t; i < 3 * (my1 - my0); i += nt) cp_async16(yv_k + 6 * my0 + 2 * i, d.ywork + 6 * my0 + 2 * i);
+  cp_async_commit();
+  const bool split_index = G > 1 && rank == 0;
+  load_row_index(d, S, 0, split_index ? sep0 : P + 1, 0, split_index ? rsep : nblk - P);
   int failed = sFail[0][0] | sFail[0][1];
+  // The branch's backward pass walks the separator rows (x known, only scattered), then its own rows.  Its first round
+  // is planned and its first chunk fetched before cluster sync #2 (plan_rows), where CTA 1 would otherwise idle.
+  const Walk wb = G > 1 ? Walk{sep0, P, my0, my1} : Walk{my0, my1, 0, 0};
   if (G > 1) {
     if (rank == 1 && t == 0) sXfail = failed;   // read by CTA 0 below
     cluster.sync();   // #1: both branches factored, CTA 1's separator area and right-hand side complete
@@ -850,8 +981,17 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
         failed = sFail[1][0] | sFail[1][1];
       }
       tk[3] = clock64();
-      load_row_index(d, S);
-      if (!failed) backsolve_rows(d, sep0, P, 0, 0, ring_off, cap / 2, S, sChunk);
+      load_row_index(d, S, sep0, P + 1, rsep, nblk - P);
+      if (!failed) {   // the separator rows: c <- z, then solved
+        for (int i = t; i < 3 * (P - sep0); i += nt) cp_async16(yv_k + 6 * sep0 + 2 * i, d.ywork + 6 * sep0 + 2 * i);
+        cp_async_commit();
+        cp_async_wait_all();
+        __syncthreads();
+        const PoseTail none = {false, false, 0., 0};
+        double unused = 0.;
+        scatter_rows(d, Walk{sep0, P, 0, 0}, sep0, P, ring_off, cap / 2, S, sChunk, false, none, unused);
+        plan_rows(d, wb, wb.n(), ring_off, cap / 2, S, sChunk);
+      }
       __syncthreads();
       // push the separator solution and the verdict into CTA 1
       double* rx = cluster.map_shared_rank(yv_k, 1);
@@ -859,17 +999,22 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
       for (int i = 6 * sep0 + t; i < 6 * P; i += nt) rx[i] = yv_k[i];
       if (t == 0) *rf = failed;
     } else {
-      load_row_index(d, S);
+      cp_async_wait_all();
+      __syncthreads();
+      if (!failed) plan_rows(d, wb, wb.n(), ring_off, cap / 2, S, sChunk);
       tk[3] = tk[2];
     }
     cluster.sync();   // #2
     if (rank == 1) failed = sXfail;
   } else {
-    load_row_index(d, S);
+    cp_async_wait_all();
+    __syncthreads();
+    if (!failed) plan_rows(d, wb, wb.n(), ring_off, cap / 2, S, sChunk);
     tk[2] = tk[3] = tk[1];
   }
   tk[4] = clock64();
   if (failed) {
+    cp_async_wait_all();
     if (rank == 0) {
       if (t == 0) { ctl->chol_fail = 1; ctl->scale_pose = 0; }
       for (int i = t; i < 7 * P; i += nt) d.pose[1 - cur][i] = d.pose[cur][i];
@@ -880,60 +1025,33 @@ k_solve(BaDev d, int cap, int nsep, int refill_branch, int prof) {
     if (G > 1) cluster.sync();   // keeps the barrier count of the two CTAs equal (#3)
     return;
   }
-  backsolve_rows(d, my0, my1, G > 1 ? sep0 : P, P, ring_off, cap / 2, S, sChunk);
-  __syncthreads();
-  tk[5] = clock64();
-  double* xv = yv_k;
-  // --- pose update (G2oVertexSE3::oplusImpl) into the trial buffer; scale = sum x (lambda x + b)
+  // --- backward pass of the branch with the pose update of its rows behind it (CTA 0 also updates the separator's
+  //     poses): scale = sum x (lambda x + b)
   double sc = 0;
-  for (int p = t; p < P; p += nt) {
-    const int j = d.pos[p];
-    if (!((j >= my0 && j < my1) || (rank == 0 && j >= sep0))) continue;
-    double dx[6], T[7], Tn[7];
-#pragma unroll
-    for (int rr = 0; rr < 6; ++rr) {
-      dx[rr] = d.fixed[p] ? 0. : xv[6 * j + rr];
-      d.x[6 * p + rr] = dx[rr];
-      sc += dx[rr] * (lambda * dx[rr] + d.bp[6 * p + rr]);
-    }
-#pragma unroll
-    for (int rr = 0; rr < 7; ++rr) T[rr] = d.pose[cur][7 * (size_t)p + rr];
-    if (d.fixed[p]) {
-#pragma unroll
-      for (int rr = 0; rr < 7; ++rr) Tn[rr] = T[rr];
-    } else {
-      double dT[7];
-      se3_exp(dx, dT);
-      se3_mul(dT, T, Tn);
-    }
-    double R[9];
-    quat_to_R(Tn, R);
-#pragma unroll
-    for (int rr = 0; rr < 7; ++rr) d.pose[1 - cur][7 * (size_t)p + rr] = Tn[rr];
-#pragma unroll
-    for (int rr = 0; rr < 9; ++rr) d.Rt[1 - cur][12 * (size_t)p + rr] = R[rr];
-    d.Rt[1 - cur][12 * (size_t)p + 9] = Tn[4];
-    d.Rt[1 - cur][12 * (size_t)p + 10] = Tn[5];
-    d.Rt[1 - cur][12 * (size_t)p + 11] = Tn[6];
-  }
+  const PoseTail poses = {G == 1 || rank == 0, true, lambda, cur};
+  scatter_rows(d, wb, my0, my1, ring_off, cap / 2, S, sChunk, true, poses, sc);
+  tk[5] = clock64();
   sc = warp_sum(sc);
   if (lane == 0) sRed[warp] = sc;
   __syncthreads();
-  double mine = 0;
+  double total = 0;
   if (t == 0)
-    for (int w = 0; w < nt / 32; ++w) mine += sRed[w];
+    for (int w = 0; w < nt / 32; ++w) total += sRed[w];
   if (G > 1) {
-    if (rank == 1 && t == 0) *cluster.map_shared_rank(&sRed[kSolveThreads / 32], 0) = mine;   // push into CTA 0
+    if (rank == 1 && t == 0) *cluster.map_shared_rank(&sRed[kSolveThreads / 32], 0) = total;   // push into CTA 0
     cluster.sync();   // #3
   }
   if (rank == 0 && t == 0) {
-    ctl->scale_pose = mine + sRed[kSolveThreads / 32];
+    ctl->scale_pose = total + sRed[kSolveThreads / 32];
     ctl->chol_fail = 0;
     ctl->ns_solve += (long long)(global_ns() - t_start);
   }
   tk[6] = clock64();
-  if (d.dbg && t == 0)   // phase boundaries in cycles since the setup
+  if (d.dbg && t == 0) {   // phase boundaries in cycles since the setup, and the setup itself from the wait on (slot 15
+                           // of the CTA's role counters, which no role uses)
     for (int i = 1; i < 7; ++i) d.dbg[rank * 6 + i - 1] = tk[i] - tk[0];
+    d.dbg[12 + 16 * rank + 15] = tk[0] - c_start;
+  }
 }
 
 // ---------------------------------------------------------------------------------------- host side
