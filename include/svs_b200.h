@@ -786,6 +786,74 @@ int svs_globalLoopClosure(svs_map *map, svs_matcher *m, svs_pose *po, const svs_
                           const int *vertex_slot, svs_loop_result *res, int cap, int *track_point, double *track_uvu,
                           int *track_level);
 
+/* ------------------------------------------------------------------ local re-registration of a keyframe
+ * Backend::localRegisterFrame (backend.cpp:549-784): the root keyframe is matched against the frames of its
+ * neighbourhood that are not yet its neighbours, from the device map, its pose graph and the matcher's keyframe slots,
+ * and on success SlamGraph::registerKeyframes' addNewObsToOldPoints on the root vertex (slam_graph.cpp:189-205, 400-420).
+ *   Inputs.  The pose graph must be set (svs_map_set_graph), else SVS_ERR_STATE.  root: a map vertex index.
+ *     window_vertex[P]: the double window (svs_map_select_window).  vertex_slot[V]: the matcher slot holding each
+ *     vertex's keyframe pyramid, -1 = none.  The matcher's current frame must be the root keyframe: its pyramid, its
+ *     disparity and its FAST corners re-detected on the stored cells (recomputeFastCorners, backend.cpp:453-469).
+ *     po: the pose handle; cam: the level-0 stereo camera of the LM and the gate; covis_thr: graph_.covis_thr().
+ *   1 Neighbourhoods and candidates (:433-449, :472-546, slam_graph.cpp:105-140).  direct = root and every vertex of
+ *     root's neighbour list.  The neighbourhood framesInNeighborhood(root, |direct| + 40) is a BFS from root over the
+ *     neighbour lists in their stored order (strongest first): the queue may hold a vertex more than once, a vertex
+ *     outside the window is dropped when it is popped, and the BFS stops once the set has |direct| + 40 vertices.  Root
+ *     outside the window gives an empty neighbourhood.  A point is a candidate when a frame of neighbourhood \ direct
+ *     observes it, its anchor is in the window, and (int)(cam_vec[anchor_level].map(T_root_from_w T_anchor^-1
+ *     xyz_anchor)) lies in the level image (border 0; no depth test, as in the reference).  anchor_level and
+ *     anchor_obs_pyr = centre / 2^level come from the anchor's own observation of the point.  Candidates are in
+ *     ascending point index (the reference's unordered_set order is unspecified).  Fewer than covis_thr: stage 1.
+ *   2 matchAndAlign (:725-784).  Every slot receives its vertex's map pose (no vertex gets a predicted pose) and keeps
+ *     it after the call.  svs_match at radius 10 (thr_mean 22, thr_std 10) with T_cur_from_actkey = identity and
+ *     T_actkey_from_w = root's map pose; fewer than covis_thr matches: stage 2.  calcFastMotionOnly with
+ *     PoseOptimizerParams(true, 2, 25) -> T_align1; svs_match at radius 4 from T_align1; the LM with (true, 2, 15)
+ *     -> T_newroot_from_oldroot; fewer than covis_thr matches: stage 3.  A NaN residual gives SVS_ERR_NUMERIC.
+ *   3 keyframesToRegister (:615-722).  Each match reprojected with T_newroot_from_oldroot is kept as a track when
+ *     |du|, |dv| < 2 * 2^anchor_level and |du_right| < 6 (svs_globalLoopClosure's test).  Each track counts towards
+ *     every vertex that observes its point, anchors a candidate and is not in direct: strength, and with the
+ *     reference's names num_left when u > w/2 (else num_right), num_lower when v > h/2 (else num_upper), w and h of the
+ *     matcher's level 0.  A counted vertex qualifies when strength >= covis_thr and each of the four counts >=
+ *     covis_thr / 2 (integer division).  No vertex qualifies: stage 4.
+ *   4 Commit (registerKeyframes' addNewObsToOldPoints).  Every track whose point a qualifying vertex observes becomes an
+ *     observation of root (uvu at level 0, anchor_level) at its ascending-vertex position, once per point; where root
+ *     already observes the point its observation stays.  Root's map pose is not changed (the reference restores it);
+ *     T_newroot_from_w = T_newroot_from_oldroot * T_root_from_w is returned.  Like svs_map_add_keyframe this forgets
+ *     the last assembled window; the pose graph stays.  addNewEdges stays with the caller: the neighbour lists, the
+ *     METRIC edges and each constraint with root placed at T_newroot_from_w (INTEGRATION.md).
+ *   Output.  res: the counts of every stage reached.  stats[n_stats]: one row per counted vertex in ascending vertex
+ *     order (the reference's ImageStatsTable order is unspecified).  tracks: track_point / track_uvu [.][3] /
+ *     track_level / track_committed, in match order (the reference's trackpoint-list order is unspecified), whenever
+ *     the gate ran.  cap_stats >= V and cap_tracks >= n_candidates always suffice.  Returns SVS_OK whether or not the
+ *     frame was registered; a rejection (stages 1-4) leaves the map bit-identical.  The host reads counts, poses and
+ *     the small outputs only.
+ *   Refused with SVS_ERR_INVALID, the map and the slots as they were: a NULL argument, root outside [0, V),
+ *     covis_thr < 1, a window vertex listed twice, a slot outside the matcher or used twice, handles on different
+ *     devices, a candidate whose anchor has no slot, no observation of the point or a level the matcher lacks, more
+ *     candidates than the matcher's max_points or the pose handle's max_obs, and cap_stats < n_stats or
+ *     cap_tracks < n_tracks (the sizes needed are in res).  The message is in svs_map_last_error. */
+typedef struct {
+  int registered;                /* the map was updated */
+  int stage;                     /* 0 registered; 1 candidates < covis_thr; 2 first match < covis_thr; 3 second match <
+                                    covis_thr; 4 no vertex qualifies */
+  int n_direct, n_neighborhood, n_candidates, n_matched1, n_matched2;
+  int n_tracks;                  /* the gated matches */
+  int n_stats;                   /* the vertices keyframesToRegister counted */
+  int n_neighbors;               /* the qualifying vertices */
+  int n_committed;               /* the tracks committed to root */
+  double T_align1[7];            /* T_newroot_from_oldroot after the first LM */
+  double T_newroot_from_oldroot[7], T_newroot_from_w[7];   /* the latter defined when registered */
+  svs_pose_stats lm[2];
+} svs_register_result;
+typedef struct {
+  int vertex, strength, num_left, num_right, num_upper, num_lower;
+  int qualified;
+} svs_register_stats;
+int svs_localRegisterFrame(svs_map *map, svs_matcher *m, svs_pose *po, const svs_cam *cam, int covis_thr, int root, int P,
+                           const int *window_vertex, const int *vertex_slot, svs_register_result *res, int cap_stats,
+                           svs_register_stats *stats, int cap_tracks, int *track_point, double *track_uvu,
+                           int *track_level, int *track_committed);
+
 /* ------------------------------------------------------------------ place recognition
  * PlaceRecognizer::addLocation (placerecognizer.cpp:206-324) after the caller's SURF step: vocabulary words, TF-IDF
  * loop candidates (calcLoopStatistics, :131-172) and geometricCheck (:175-202) = BFMatcher(NORM_L2).match +

@@ -620,6 +620,40 @@ class DeviceMap {
     }
     return r.verified != 0;
   }
+
+  // Backend::localRegisterFrame (backend.cpp:549-784) on this map; semantics: svs_localRegisterFrame.  The pose graph
+  // must be set (setGraph); the matcher holds the root keyframe as its current frame and the keyframe pyramids in the
+  // slots vertex_slot names.  Returns true when the frame was registered and the map grew; *res (when given) holds the
+  // counts of every stage reached, *stats the stats table, *tracks the gated tracks.  Throws std::runtime_error on a
+  // refused call (the missing pose graph included) and where the reference throws (a NaN residual).
+  struct RegisterTracks { std::vector<int> point, level, committed; std::vector<double> uvu; };
+  bool localRegisterFrame(GuidedMatcher& matcher, BA_SE3_XYZ_STEREO& ba, const svs_cam& cam, int covis_thr, int root_id,
+                          const std::vector<int>& window_vertex, const std::vector<int>& vertex_slot,
+                          svs_register_result* res = nullptr, std::vector<svs_register_stats>* stats = nullptr,
+                          RegisterTracks* tracks = nullptr) {
+    if (!ok_) throw std::runtime_error("no CUDA device");
+    if ((int)vertex_slot.size() != V_) throw std::runtime_error("vertex_slot must name a slot (or -1) for every vertex");
+    const int cs = V_ > 0 ? V_ : 1, ct = Np_ > 0 ? Np_ : 1;   // stats <= vertices, tracks <= candidates <= points
+    std::vector<svs_register_stats> st(cs);
+    std::vector<int> tp(ct), tl(ct), tc(ct);
+    std::vector<double> tu(3 * (size_t)ct);
+    svs_register_result r{};
+    const int rc = svs_localRegisterFrame(h_, matcher.handle(), ba.handle(), &cam, covis_thr, root_id, (int)window_vertex.size(),
+                                          window_vertex.data(), vertex_slot.data(), &r, cs, st.data(), ct, tp.data(), tu.data(),
+                                          tl.data(), tc.data());
+    if (res) *res = r;
+    if (rc != SVS_OK) throw std::runtime_error(svs_map_last_error(h_));
+    const bool gated = r.stage == 0 || r.stage == 4;
+    if (stats) stats->assign(st.begin(), st.begin() + (gated ? r.n_stats : 0));
+    if (tracks) {
+      const int n = gated ? r.n_tracks : 0;
+      tracks->point.assign(tp.begin(), tp.begin() + n);
+      tracks->level.assign(tl.begin(), tl.begin() + n);
+      tracks->committed.assign(tc.begin(), tc.begin() + n);
+      tracks->uvu.assign(tu.begin(), tu.begin() + 3 * (size_t)n);
+    }
+    return r.registered != 0;
+  }
   bool get(std::vector<double>* T_me_from_world, std::vector<double>* xyz_anchor) {
     T_me_from_world->resize(7 * (size_t)V_); xyz_anchor->resize(3 * (size_t)(Np_ > 0 ? Np_ : 1));
     const bool r = ok_ && svs_map_get(h_, T_me_from_world->data(), xyz_anchor->data()) == SVS_OK;

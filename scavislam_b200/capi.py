@@ -165,6 +165,22 @@ class SvsLoopResult(C.Structure):
                 ("lm", SvsPoseStats * 2)]
 
 
+REGISTER_COUNTS = ("registered", "stage", "n_direct", "n_neighborhood", "n_candidates", "n_matched1", "n_matched2", "n_tracks",
+                   "n_stats", "n_neighbors", "n_committed")
+
+
+class SvsRegisterResult(C.Structure):
+    _fields_ = [(f, C.c_int) for f in REGISTER_COUNTS] + [
+        ("T_align1", C.c_double * 7), ("T_newroot_from_oldroot", C.c_double * 7), ("T_newroot_from_w", C.c_double * 7),
+        ("lm", SvsPoseStats * 2)]
+
+
+# svs_register_stats
+REGISTER_STATS_DTYPE = np.dtype([("vertex", np.int32), ("strength", np.int32), ("num_left", np.int32),
+                                 ("num_right", np.int32), ("num_upper", np.int32), ("num_lower", np.int32),
+                                 ("qualified", np.int32)])
+
+
 EXPORTS = [
     "svs_ba_create", "svs_ba_destroy", "svs_last_error", "svs_ba_set_problem", "svs_ba_optimize",
     "svs_ba_get_poses", "svs_ba_get_points", "svs_ba_reset_state", "svs_optimiseInnerAndOuterWindow",
@@ -197,7 +213,7 @@ EXPORTS = [
     "svs_ba_covariance", "svs_ba_set_problem_device", "svs_ba_observation_grad", "svs_ba_window_grad",
     "svs_place_create", "svs_place_destroy", "svs_place_last_error", "svs_place_add_location", "svs_place_num_places",
     "svs_place_last_words", "svs_place_last_scores", "svs_place_last_matches", "svs_place_last_hypotheses",
-    "svs_globalLoopClosure",
+    "svs_globalLoopClosure", "svs_localRegisterFrame",
 ]
 
 
@@ -329,6 +345,8 @@ def lib():
     L.svs_map_last_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp]
     L.svs_globalLoopClosure.argtypes = [vp, vp, vp, C.POINTER(SvsCam), C.c_int, C.c_int, C.c_int, c_dp, C.c_int, c_ip, c_ip,
                                         C.POINTER(SvsLoopResult), C.c_int, c_ip, c_dp, c_ip]
+    L.svs_localRegisterFrame.argtypes = [vp, vp, vp, C.POINTER(SvsCam), C.c_int, C.c_int, C.c_int, c_ip, c_ip,
+                                         C.POINTER(SvsRegisterResult), C.c_int, vp, C.c_int, c_ip, c_dp, c_ip, c_ip]
     L.svs_constraints_create.argtypes = [C.c_int, C.POINTER(vp)]
     L.svs_constraints_destroy.argtypes = [vp]
     L.svs_constraints_destroy.restype = None
@@ -1467,6 +1485,36 @@ class DeviceMap:
             raise err
         n = out["n_tracks"] if out["stage"] in (0, 3, 4) else 0
         return out, dict(point=tp[:n].copy(), uvu=tu[:n].copy(), level=tl[:n].copy())
+
+    def local_register_frame(self, matcher, pose, cam, covis_thr, root, window_vertex, vertex_slot, cap_stats=None,
+                             cap_tracks=None):
+        """Backend::localRegisterFrame on the device (svs_localRegisterFrame): `matcher` (a GuidedMatcher) holds the root
+        keyframe as its current frame and the keyframe pyramids in the slots vertex_slot names, `pose` is a
+        PoseOptimizer; the pose graph must be set (set_graph).  Returns (result dict, stats [REGISTER_STATS_DTYPE] in
+        ascending vertex order, tracks dict(point, uvu, level, committed) in match order); a registered frame has grown
+        the map.  A refused call raises SvsError with the result dict as .result."""
+        win = np.ascontiguousarray(window_vertex, np.int32)
+        slot = np.ascontiguousarray(vertex_slot, np.int32)
+        cs = max(self.V, 1) if cap_stats is None else int(cap_stats)
+        ct = max(self.Np, 1) if cap_tracks is None else int(cap_tracks)
+        st = np.zeros(max(cs, 1), REGISTER_STATS_DTYPE)
+        tp, tu = np.zeros(max(ct, 1), np.int32), np.zeros((max(ct, 1), 3))
+        tl, tc = np.zeros(max(ct, 1), np.int32), np.zeros(max(ct, 1), np.int32)
+        r = SvsRegisterResult()
+        cm = SvsCam(*[float(x) for x in cam])
+        rc = lib().svs_localRegisterFrame(self._h, matcher._h, pose._h, C.byref(cm), int(covis_thr), int(root), len(win), _ip(win),
+                                          _ip(slot), C.byref(r), cs, st.ctypes.data, ct, _ip(tp), _dp(tu), _ip(tl), _ip(tc))
+        out = {f: getattr(r, f) for f in REGISTER_COUNTS}
+        for f in ("T_align1", "T_newroot_from_oldroot", "T_newroot_from_w"):
+            out[f] = np.array(getattr(r, f)[:])
+        out["lm"] = [PoseOptimizer._stats(r.lm[k]) for k in range(2)]
+        if rc != 0:
+            err = SvsError(rc, lib().svs_map_last_error(self._h).decode())
+            err.result = out
+            raise err
+        gated = out["stage"] in (0, 4)
+        nt, ns = (out["n_tracks"], out["n_stats"]) if gated else (0, 0)
+        return out, st[:ns].copy(), dict(point=tp[:nt].copy(), uvu=tu[:nt].copy(), level=tl[:nt].copy(), committed=tc[:nt].copy())
 
 
 def load_surf_vocabulary(path):

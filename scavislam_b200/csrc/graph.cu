@@ -791,6 +791,11 @@ void svs::map_view(svs_map* h, MapView* v) {
 
 void svs::map_set_error(svs_map* h, const char* msg) { h->err = msg; }
 
+bool svs::map_graph(svs_map* h, const int** nbr_ptr, const int** nbr_id, int* nnzN) {
+  *nbr_ptr = h->g.nbr_ptr; *nbr_id = h->g.nbr_id; *nnzN = h->nnzN;
+  return h->g.nbr_ptr != nullptr;
+}
+
 void svs::launch_scan(const int* cnt, int n, int* ptr, cudaStream_t stream) { k_scan<<<1, 1024, 0, stream>>>(cnt, n, ptr); }
 
 int svs::map_add_observations(svs_map* h, int vertex, int n, const int* d_point, const double* d_center, const int* d_level) {

@@ -70,6 +70,9 @@ struct MapView {
 };
 __attribute__((visibility("hidden"))) void map_view(svs_map* h, MapView* v);
 __attribute__((visibility("hidden"))) void map_set_error(svs_map* h, const char* msg);
+// the pose graph of svs_map_set_graph on the map's device (nbr_ptr [V+1], nbr_id [nnzN], strongest first); false when
+// none is set
+__attribute__((visibility("hidden"))) bool map_graph(svs_map* h, const int** nbr_ptr, const int** nbr_id, int* nnzN);
 // exclusive scan of n counts into ptr[n + 1] by one CTA on `stream` (graph.cu's k_scan)
 __attribute__((visibility("hidden"))) void launch_scan(const int* cnt, int n, int* ptr, cudaStream_t stream);
 // addNewObsToOldPoints (slam_graph.cpp:400-420) for an existing vertex: n distinct points (device arrays on the map's

@@ -150,3 +150,73 @@ def make_scene(oracle, n_kf=8, radius=0.4, reach=2, per_level=(160, 60), drift=(
                 query=query, loop=loop, window=np.arange(max(0, n_kf - 2 * reach), n_kf + 1, dtype=np.int32),
                 T_true_query_from_loop=T_true_ql, T_query_from_loop=perturb(T_true_ql, prop_err[0], prop_err[1], rng),
                 loop_features=fast_features(oracle, frames[loop]["pyr"]))
+
+
+def path_graph(m, V, reach):
+    """The pose graph of the path: keyframes within `reach` steps are neighbours, with strength = the number of points
+    both observe, listed strongest first (ties: the larger id first).  Returns svs_map_set_graph's (nbr_ptr, nbr_id)."""
+    sees = [set() for _ in range(V)]
+    for p in range(len(m["point_anchor"])):
+        for v in m["vis_pose"][m["vis_ptr"][p]:m["vis_ptr"][p + 1]]:
+            sees[int(v)].add(p)
+    ptr, ids = [0], []
+    for v in range(V):
+        nb = [(len(sees[v] & sees[j]), j) for j in range(max(0, v - reach), min(V, v + reach + 1)) if j != v]
+        ids += [j for _, j in sorted(nb, reverse=True)]
+        ptr.append(len(ids))
+    return np.array(ptr, np.int32), np.array(ids, np.int32)
+
+
+def make_register_scene(oracle, n_kf=8, reach=2, **kw):
+    """A revisit inside the double window for Backend::localRegisterFrame: the path of make_scene with every keyframe
+    0..n_kf in the window and the pose graph of path_graph.  Root is the last keyframe; its direct neighbours are the
+    `reach` keyframes before it, and it sees the points of keyframes 0 and 1, which are in its window but not its
+    neighbours.  Root's stored pose has drifted by make_scene's `drift`; every other stored pose is true, so the points
+    the registration matches against all place root where it truly is."""
+    sc = make_scene(oracle, n_kf=n_kf, reach=reach, **kw)
+    T, st = sc["true_T"], sc["map"]["poses"]
+    Dw = mul(inv(T[n_kf]), st[n_kf])
+    poses = np.array([mul(T[k], Dw) if k == n_kf else T[k] for k in range(n_kf + 1)])
+    m = dict(sc["map"], poses=poses)
+    nbr_ptr, nbr_id = path_graph(m, n_kf + 1, reach)
+    return dict(sc, map=m, root=n_kf, window=np.arange(n_kf + 1, dtype=np.int32), nbr_ptr=nbr_ptr, nbr_id=nbr_id,
+                root_features=fast_features(oracle, sc["frames"][n_kf]["pyr"]))
+
+
+def make_flat_register_scene(oracle, n, n_direct_anchored=0, seed=11):
+    """A flat map for Backend::localRegisterFrame: vertices 0 (root), 1 (its only neighbour), 2 and 3 all at the
+    identity and all seeing the same rendered image, with the pose graph 0-1-2-3.  n points at FAST corners (in the
+    order `seed` shuffles them) are anchored in 2 and seen by 2 and 3 (3 observes them but anchors none); the next
+    n_direct_anchored corners are anchored in the direct neighbour 1 and seen by 1 and 2.  Every candidate is predicted
+    on the corner it was made from, so the number of tracks follows n."""
+    from .synth_images import render_frame as _render
+    img, disp = _render(np.zeros(3), 0.0, seed=77)
+    pyr = fi.uint8_pyramid(img, NLV)
+    xy = oracle.fast_detect_roi(img, 8, 632, 8, 472, 12)
+    xy = xy[disp[xy[:, 1], xy[:, 0]] > 1]
+    xy = xy[np.random.default_rng(seed).permutation(len(xy))]
+    feats = []
+    for l in range(NLV):
+        k = oracle.fast_detect_roi(pyr[l], 0, CAM_W >> l, 0, CAM_H >> l, 12)
+        feats.append((k, np.arange(len(k), dtype=np.int32)))
+    N = n + n_direct_anchored
+    assert N <= len(xy)
+    u, v = xy[:N, 0].astype(np.float64), xy[:N, 1].astype(np.float64)
+    d = disp[xy[:N, 1], xy[:N, 0]].astype(np.float64)
+    z = CAM_F * CAM_B / d
+    X = np.stack([(u - CAM_PX) / CAM_F * z, (v - CAM_PY) / CAM_F * z, z], 1)
+    vp, vs, cen, anchor = [0], [], [], []
+    for p in range(N):
+        a, seen = (2, (2, 3)) if p < n else (1, (1, 2))
+        anchor.append(a)
+        for vert in seen:
+            vs.append(vert); cen.append([u[p], v[p], u[p] - d[p]])
+        vp.append(len(vs))
+    I7 = np.array([0, 0, 0, 1, 0, 0, 0.0])
+    m = dict(poses=np.tile(I7, (4, 1)), point_anchor=np.array(anchor, np.int32), xyz_anchor=X.reshape(-1, 3),
+             vis_ptr=np.array(vp, np.int32), vis_pose=np.array(vs, np.int32), feat_center=np.array(cen).reshape(-1, 3),
+             feat_level=np.zeros(len(vs), np.int32))
+    fr = dict(pyr=pyr, disp=disp)
+    return dict(levels=levels(), cam=(CAM_F, CAM_PX, CAM_PY, CAM_B), frames=[fr] * 4, map=m, root=0,
+                window=np.arange(4, dtype=np.int32), nbr_ptr=np.array([0, 1, 3, 5, 6], np.int32),
+                nbr_id=np.array([1, 0, 2, 1, 3, 2], np.int32), root_features=feats)
