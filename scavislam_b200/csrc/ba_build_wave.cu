@@ -6,10 +6,12 @@
 //     of them scatter into the same K(K+1)/2 blocks of the reduced camera system;
 //   * edges are linearised 32 at a time (one lane per edge, several landmarks per wave), which
 //     keeps every lane busy where one-warp-per-landmark leaves 3/4 of them idle;
-//   * the Schur products Y_m B_n^T (and the direct J^T W J terms) are accumulated over all
-//     landmarks of the task in registers -- each lane owns up to 7 (pair, row) units of 6 doubles --
-//     and flushed with ONE set of RED.F64 per task instead of one per landmark (the FP64
-//     reduction rate, scripts/ubench/lat.cu, would make a per-landmark scatter a large share of a launch).
+//   * the task's whole contribution to the reduced system, S_task = sum_e G_e^T G_e - sum_l Y_l B_l^T (G_e the
+//     3 x 6K scaled Jacobian of edge e over the task's slots, Y_l = B_l (Hll + lambda I)^-1, B_l the 6K x 3 Hpl stack),
+//     is one FP64 tensor-core product (mma.m8n8k4.f64, DMMA) on 8 x 8 tiles of the 6K x 6K block, accumulated over
+//     all landmarks of the task in the tile fragments and flushed with ONE set of RED.F64 per task instead of one
+//     per landmark (the FP64 reduction rate, scripts/ubench/lat.cu, would make a per-landmark scatter a large share
+//     of a launch).
 //
 // Reference semantics: G2oEdgeProjectPSI2UVU::linearizeOplus (anchored_points.cpp:168-189), g2o
 // BaseMultiEdge::constructQuadraticForm, BlockSolver<6,3>::buildSystem / solve (Schur part).
@@ -25,11 +27,23 @@ constexpr int kWvWarps = 4;
 constexpr int kWvLm = 8;       // landmarks per wave
 constexpr int kWvSlots = 40;   // slots per wave
 constexpr int kWvJ = 19;       // row stride of the per-edge Jacobian rows (odd: conflict-free 64-bit stores)
-constexpr int kWvLmD = 56;     // per-landmark scratch: D(6) bl(3) Dinv(9) A_aa(36) + pad
+constexpr int kWvLmD = 18;     // per-landmark scratch: D(6) bl(3) Dinv(9)
 constexpr int kWvDoubles = 2 * 32 * kWvJ + 32 * 9 + 32 * 3 + 2 * kWvSlots * 18 + kWvLm * kWvLmD + 32;
-constexpr int kWvInts = 8 + 40;   // slot poses, pair table (36) padded
+constexpr int kWvInts = 8 + 40;   // slot poses, block table (36) padded
+constexpr int kWvTiles = 6;       // 8-wide tiles over the 6K <= 48 rows / columns of a task's block
+constexpr int kWvM = 56;          // row stride of the task's block staged for the flush
+static_assert((8 * kWvTiles - 1) * kWvM + 8 * kWvTiles <= kWvDoubles && kWvDoubles % 2 == 0,
+              "the staged block fits a warp's 16-byte aligned shared memory");
 
 size_t build_wave_smem_bytes() { return (size_t)kWvWarps * (kWvDoubles * 8 + kWvInts * 4); }
+
+// D += A B on one 8 x 8 tile, k = 4: lane holds A[lane >> 2][lane & 3], B[lane & 3][lane >> 2] and
+// D[lane >> 2][2 (lane & 3) + {0, 1}]
+__device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double b) {
+  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
+}
+// upper tile pair (t1 <= t2) -> accumulator index
+__host__ __device__ constexpr int tile_pair(int t1, int t2) { return t2 * (t2 + 1) / 2 + t1; }
 
 // kTimeline: the overlap timeline's instance (SVS_SOLVE_TIMING=3, `timeline` = d.dbg + 160); the other one is the plain
 // kernel, whose code the instrumentation must not touch
@@ -119,34 +133,24 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
   double Ra[9], ta[3];
   load12(Rt, ia, Ra, ta);
 
-  // slot poses and the pair table, ordered by kind so that the 32 units of a round mostly share a
-  // code path: anchor-row pairs (0,n), diagonal pairs (m,m), (0,0), then the plain pairs
+  // slot poses and the block table: sPair[tile_pair(m, n)] = (d.tbl entry (block << 1 | transpose) << 6) | m << 3 | n
+  // for the slots m <= n
   if (lane == 0) sPose[0] = ia;
   if (lane < k && !(has_self && lane == 0)) sPose[lane + off] = d.e_pose[e_base + lane];
   __syncwarp();
-  const int npairs = K * (K + 1) / 2;
-  for (int p = lane; p < npairs; p += 32) {
-    int m, n;
-    if (p < K - 1) { m = 0; n = 1 + p; }
-    else if (p < 2 * K - 2) { m = n = 1 + p - (K - 1); }
-    else if (p == 2 * K - 2) { m = n = 0; }
-    else {
-      int rem = p - (2 * K - 1);
-      m = 1;
-      while (rem >= K - 1 - m) { rem -= K - 1 - m; ++m; }
-      n = m + 1 + rem;
-    }
-    const int t = d.tbl[(size_t)sPose[m] * d.P + sPose[n]];
-    sPair[p] = ((t >> 1) << 11) | ((t & 1) << 10) | (m << 5) | n;
+  for (int p = lane; p < K * (K + 1) / 2; p += 32) {
+    int n = 0;
+    while (tile_pair(0, n + 1) <= p) ++n;
+    const int m = p - tile_pair(0, n);
+    sPair[p] = d.tbl[(size_t)sPose[m] * d.P + sPose[n]] << 6 | m << 3 | n;
   }
   __syncwarp();
 
-  const int nunits = npairs * 6;
-  double acc[7][6];
+  // the upper 8 x 8 tiles of the task's 6K x 6K block, as DMMA accumulator fragments
+  const int ntiles = (6 * K + 7) / 8;
+  double acc[tile_pair(0, kWvTiles)][2];
 #pragma unroll
-  for (int q = 0; q < 7; ++q)
-#pragma unroll
-    for (int c = 0; c < 6; ++c) acc[q][c] = 0.;
+  for (int p = 0; p < tile_pair(0, kWvTiles); ++p) acc[p][0] = acc[p][1] = 0.;
   double accg[2] = {0., 0.}, accc[2] = {0., 0.};
 
   int nw_max = 32 / k;
@@ -188,7 +192,7 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
       for (int i = 0; i < k; ++i) s += sChi[lane * k + i];
       d.chi_l[lm0 + w0 + lane] = s;
     }
-    // ---- phase 2: per-landmark sums over its edges: anchor Hpl block (18), Hll (6), b_l (3), A_aa (21);
+    // ---- phase 2: per-landmark sums over its edges: anchor Hpl block (18), Hll (6), b_l (3);
     //      one loop per kind so that the lanes of a round share a code path
     for (int it = lane; it < nw * 18; it += 32) {
       const int j = it / 18, t = it - j * 18, r = t / 3, c = t - r * 3;
@@ -213,17 +217,6 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
       double s = 0.;
       for (int i = 0; i < k; ++i, Js += 9, Ee += 3) s -= Js[c] * Ee[0] + Js[3 + c] * Ee[1] + Js[6 + c] * Ee[2];
       sLm[j * kWvLmD + 6 + c] = s;
-    }
-    for (int it = lane; it < nw * 21; it += 32) {
-      // anchor diagonal: all edges' J~a^T J~a; the self edge keeps g2o's J1^T W J1 (SURVEY 8c(4))
-      const int j = it / 21, u = it - j * 21;
-      const int r = (u >= 1) + (u >= 3) + (u >= 6) + (u >= 10) + (u >= 15), c = u - r * (r + 1) / 2;
-      const int i0 = skip_self ? i_first : 0;
-      const double* Ja = sJa + kWvJ * (j * k + i0);
-      double s = 0.;
-      for (int i = i0; i < k; ++i, Ja += kWvJ) s += Ja[r] * Ja[c] + Ja[6 + r] * Ja[6 + c] + Ja[12 + r] * Ja[12 + c];
-      sLm[j * kWvLmD + 18 + r * 6 + c] = s;
-      sLm[j * kWvLmD + 18 + c * 6 + r] = s;
     }
     __syncwarp();
     PBW(2);
@@ -279,59 +272,65 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
     }
     __syncwarp();
     PBW(3);
-    // ---- phase 5: accumulate the task's contribution to the reduced system in registers.
-    //      The Schur product common to every unit runs branch-free (9 16-byte loads of B_n, FMAs straight
-    //      into the accumulators); the direct J^T W J terms of the few special pairs follow in their own loops.
+    // ---- phase 5: the wave's S_task terms on the tensor cores.  A lane's k-row is kb + (lane & 3), its column in tile t
+    //      is 8 t + (lane >> 2): the A and B fragments of a tile load the same element of the k-row, so one value per
+    //      lane and tile serves both operands.  k-rows past the wave's end, and columns past 6K, load zero.
+    {
+      const int kq = lane & 3, cl = lane >> 2;
+      // G_e^T G_e, one slot at a time: the k-rows are (landmark, residual row) of the slot's edge; its row of G is
+      // J~a in slot 0's columns (tile 0) and J~p in slot s's, so only the tiles of {0} and slot s take part.  The
+      // self edge (slot 0) brings J~a alone -- g2o's J1^T W J1, SURVEY 8c(4) -- and nothing under the B5 skip.
 #pragma unroll
-    for (int q = 0; q < 7; ++q) {
-      const int u = lane + 32 * q;
-      if (u < nunits) {
-        const int p = u / 6, r = u - p * 6;
-        const int pk = sPair[p];
-        const int m = (pk >> 5) & 31, n = pk & 31;
-        {
-          const double* Ym = sY + 18 * m + r * 3;
-          const double2* Bn = reinterpret_cast<const double2*>(sB + 18 * n);
-#pragma unroll 1
-          for (int j = 0; j < nw; ++j, Ym += 18 * K, Bn += 9 * K) {
-            const double y0 = -Ym[0], y1 = -Ym[1], y2 = -Ym[2];
-            double bb[18];
+      for (int s = 0; s < 8; ++s) {
+        if (s >= K) break;
+        if (s == 0 && (!has_self || skip_self)) continue;
+        const int i = s == 0 ? 0 : s - off;
+        for (int kb = 0; kb < 3 * nw; kb += 4) {
+          const int kr = kb + kq, j = kr / 3, q = kr - 3 * j;
+          const bool valid = kr < 3 * nw;
+          const double* Ja = sJa + kWvJ * (j * k + i) + 6 * q;
+          const double* Jp = sJp + kWvJ * (j * k + i) + 6 * q;
+          double g[kWvTiles];
 #pragma unroll
-            for (int i = 0; i < 9; ++i) { const double2 t2 = Bn[i]; bb[2 * i] = t2.x; bb[2 * i + 1] = t2.y; }
-#pragma unroll
-            for (int c = 0; c < 6; ++c)
-              acc[q][c] = fma(y2, bb[c * 3 + 2], fma(y1, bb[c * 3 + 1], fma(y0, bb[c * 3], acc[q][c])));
+          for (int t = 0; t < kWvTiles; ++t) {
+            const int col = 8 * t + cl;
+            double v = 0.;
+            if (t == 0 && col < 6) { if (valid) v = Ja[col]; }
+            else if (s > 0 && col >= 6 * s && col < 6 * s + 6) { if (valid) v = Jp[col - 6 * s]; }
+            g[t] = v;
           }
-        }
-        if (m == n) {
-          if (m > 0) {   // own J~p^T J~p of the observer
-            const double* Jp = sJp + kWvJ * (m - off);
-#pragma unroll 1
-            for (int j = 0; j < nw; ++j, Jp += kWvJ * k) {
-              const double a0 = Jp[r], a1 = Jp[6 + r], a2 = Jp[12 + r];
 #pragma unroll
-              for (int c = 0; c < 6; ++c)
-                acc[q][c] = fma(a2, Jp[12 + c], fma(a1, Jp[6 + c], fma(a0, Jp[c], acc[q][c])));
-            }
-          } else {       // anchor diagonal, summed over the edges in phase 2
-            const double* A = sLm + 18 + r * 6;
-#pragma unroll 1
-            for (int j = 0; j < nw; ++j, A += kWvLmD) {
+          for (int t2 = 0; t2 < kWvTiles; ++t2) {
+            const bool in2 = t2 == 0 || t2 == 6 * s / 8 || t2 == (6 * s + 5) / 8;
 #pragma unroll
-              for (int c = 0; c < 6; ++c) acc[q][c] += A[c];
+            for (int t1 = 0; t1 <= t2; ++t1) {
+              const bool in1 = t1 == 0 || t1 == 6 * s / 8 || t1 == (6 * s + 5) / 8;
+              if (s > 0 && in1 && in2) dmma884(acc[tile_pair(t1, t2)][0], acc[tile_pair(t1, t2)][1], g[t1], g[t2]);
+              if (s == 0 && t1 == 0 && t2 == 0) dmma884(acc[0][0], acc[0][1], g[0], g[0]);
             }
           }
-        } else if (m == 0) {   // anchor x observer: J~a^T J~p
-          const double* Ja = sJa + kWvJ * (n - off);
-          const double* Jp = sJp + kWvJ * (n - off);
-#pragma unroll 1
-          for (int j = 0; j < nw; ++j, Ja += kWvJ * k, Jp += kWvJ * k) {
-            const double a0 = Ja[r], a1 = Ja[6 + r], a2 = Ja[12 + r];
-#pragma unroll
-            for (int c = 0; c < 6; ++c)
-              acc[q][c] = fma(a2, Jp[12 + c], fma(a1, Jp[6 + c], fma(a0, Jp[c], acc[q][c])));
-          }
         }
+      }
+      // - Y B^T: the k-rows are (landmark, column of Hpl); slot n's block of landmark j holds B[r][q] at
+      // sB + 18 (j K + n) + 3 r + q, i.e. column 6 n + r at sB + 18 j K + 3 (6 n + r) + q
+      for (int kb = 0; kb < 3 * nw; kb += 4) {
+        const int kr = kb + kq, j = kr / 3, q = kr - 3 * j;
+        const bool valid = kr < 3 * nw;
+        const int o = 18 * j * K + q;
+        double fy[kWvTiles], fb[kWvTiles];
+#pragma unroll
+        for (int t = 0; t < kWvTiles; ++t) {
+          const int col = 8 * t + cl;
+          const bool ok = valid && col < 6 * K;
+          fy[t] = ok ? -sY[o + 3 * col] : 0.;
+          fb[t] = ok ? sB[o + 3 * col] : 0.;
+        }
+#pragma unroll
+        for (int t2 = 0; t2 < kWvTiles; ++t2)
+          if (t2 < ntiles) {
+#pragma unroll
+            for (int t1 = 0; t1 <= t2; ++t1) dmma884(acc[tile_pair(t1, t2)][0], acc[tile_pair(t1, t2)][1], fy[t1], fb[t2]);
+          }
       }
     }
     PBW(4);
@@ -362,17 +361,26 @@ k_build_wave(BaDev d, int robust, double delta, int n_task_blocks, int prof, int
     __syncwarp();
     PBW(5);
   }
-  // ---- flush: one RED.F64 per accumulated element for the whole task
+  // ---- flush: one RED.F64 per element of the upper block triangle for the whole task.  The tiles go through the
+  //      warp's shared memory (free once the last wave is done; row stride kWvM, 16-byte stores without bank conflicts),
+  //      so that consecutive lanes add into consecutive elements of a block.  An element of a diagonal block below the
+  //      diagonal whose tile lies below the tile diagonal is read from its mirror image.
+  {
+    double* sM = sm;
 #pragma unroll
-  for (int q = 0; q < 7; ++q) {
-    const int u = lane + 32 * q;
-    if (u < nunits) {
-      const int p = u / 6, r = u - p * 6;
-      const int pk = sPair[p];
-      double* blk = d.S + 36 * (size_t)(pk >> 11);
-      const int tr = (pk >> 10) & 1;
+    for (int t2 = 0; t2 < kWvTiles; ++t2)
 #pragma unroll
-      for (int c = 0; c < 6; ++c) atomicAdd(blk + (tr ? c * 6 + r : r * 6 + c), acc[q][c]);
+      for (int t1 = 0; t1 <= t2; ++t1)
+        if (t2 < ntiles)
+          *reinterpret_cast<double2*>(sM + (8 * t1 + (lane >> 2)) * kWvM + 8 * t2 + 2 * (lane & 3)) =
+              make_double2(acc[tile_pair(t1, t2)][0], acc[tile_pair(t1, t2)][1]);
+    __syncwarp();
+    for (int e = lane; e < 36 * (K * (K + 1) / 2); e += 32) {
+      const int p = e / 36, w = e - 36 * p;
+      const int pk = sPair[p], m = (pk >> 3) & 7, n = pk & 7, t = pk >> 6;
+      const int tr = t & 1, r = tr ? w % 6 : w / 6, c = tr ? w / 6 : w % 6;
+      const int row = 6 * m + r, col = 6 * n + c;
+      atomicAdd(d.S + 36 * (size_t)(t >> 1) + w, (row >> 3) > (col >> 3) ? sM[col * kWvM + row] : sM[row * kWvM + col]);
     }
   }
 #pragma unroll
@@ -425,7 +433,7 @@ void launch_build_wave(const BaDev& d, int robust, double delta, cudaStream_t st
   int task_blocks = (d.ntasks + kWvWarps - 1) / kWvWarps;
   const int c_blocks = (d.C + kWvWarps * 32 - 1) / (kWvWarps * 32);
   // persistent grid when the tasks outnumber the warp slots: as many task CTAs as are resident at once (255 registers
-  // and 111 KB of shared memory per CTA: two per SM), tasks drawn from a counter; otherwise one task per warp
+  // and 101 KB of shared memory per CTA: two per SM), tasks drawn from a counter; otherwise one task per warp
   const int resident = build_wave_resident_ctas();
   const int persist = task_blocks > resident ? 1 : 0;
   if (persist) task_blocks = resident;
