@@ -540,6 +540,128 @@ int svs_match(svs_matcher *h, const double T_cur_from_actkey[7], const double T_
               const svs_match_point *pts, int n, int search_radius, int thr_mean, int thr_std,
               svs_match_result *out);
 
+/* ------------------------------------------------------------------ the tracked frame's bookkeeping
+ * StereoFrontend::processFrame after the LM (stereo_frontend.cpp:184-306): matchAndTrack's candidate groups and budget
+ * (:977-1065), processMatchedPoints (:834-974), shallWeDropNewKeyframe (:512-528) and addMorePointsToOtherFrame
+ * (:724-823, the seeding of addNewPoints and addNewKeyframe).  Everything is read from the matcher handle: the results
+ * and candidates of its last match, the current frame's FAST corners per level and its level-0 disparity. */
+
+/* the reference's ui / params_ values; SVS_FRONTEND_PARAMS_DEFAULT mirrors them */
+typedef struct {
+  unsigned long long seed;     /* emission order of the seeding (see svs_addMorePoints) */
+  float max_reproj_error;      /* ui.max_reproj_error */
+  int newpoint_clearance;      /* params_.newpoint_clearance, R in [0, 64] */
+  int num_max_points;          /* ui.num_max_points: the seeding keeps at most (num_max_points >> l) + 1 points at
+                                  level l (matchAndTrack's budget is an argument of svs_match_track) */
+  int min_num_points;          /* ui.min_num_points: add flag (i, j) = grid3x3[i][j] <= min_num_points */
+  int featureless_corners_thr; /* params_.new_keyframe_featuerless_corners_thr */
+  float parallax_thr;          /* ui.parallax_thr */
+} svs_frontend_params;
+#define SVS_FRONTEND_PARAMS_DEFAULT {0ull, 2.f, 2, 300, 25, 2, 0.75f}
+
+/* PointStatistics (stereo_frontend.h:160-177) and av_track_length_.  Grid index i comes from u, j from v:
+ * grid2x2[i][j] with i = 0 when u < (int)(w * 0.5); grid3x3[i][j] with the thirds (int)(w * third) and
+ * (int)(w * 2 * third), float third = 1./3. (w, h of matcher level 0). */
+typedef struct {
+  int num_matched_points[SVS_MATCH_MAX_LEVELS];
+  int grid2x2[2][2];
+  int grid3x3[3][3];
+  double av_track_length;   /* sum of ||uv_pyr - curkey_uv_pyr|| in match order (double) / num_tracked: NaN at 0 */
+  int num_tracked;          /* entries that passed the gate */
+  int num_new;              /* of which new two-view points */
+} svs_point_stats;
+
+/* one gated match, in match order: candidate index, class (1 = NewTwoViewPoint, index < n_new; 0 = TrackPoint),
+ * anchor level and the observation uvu at level 0 */
+typedef struct {
+  int index;
+  int is_new;
+  int anchor_level;
+  int reserved;
+  double uvu[3];
+} svs_tracked_point;
+
+/* one seeded CandidatePoint<3>: level, uv_pyr, uvu_pyr = (u, v, u - disp), xyz = T_newkey_from_cur * xyz_cur and
+ * normal = -xyz_cur / |xyz_cur| (xyz_cur = unmap_uvu(uvu_pyr * 2^level), the normal is not transformed) */
+typedef struct {
+  int level;
+  int reserved;
+  double uv_pyr[2];
+  double uvu_pyr[3];
+  double xyz[3];
+  double normal[3];
+} svs_new_point;
+
+/* matchAndTrack's matching (stereo_frontend.cpp:977-1065) in one call.  The n candidates come as n_groups >= 2
+ * consecutive groups ending at group_end[g] (non-decreasing, group_end[n_groups-1] = n): group 0 is
+ * newpoint_map[actkey], groups 1 .. n_groups-2 the neighbours' newpoint_map lists in the order the caller walks
+ * strength_to_neighbors (weakest first), the last group the neighbourhood's point_list.  One k_match launch covers all
+ * candidates (an entry does not depend on the others, so matching groups that are then discarded is exact); a device
+ * kernel then applies the stop rule: neighbour group g is kept iff 2 * (matched entries of groups 0 .. g-1) <
+ * num_max_points and every earlier neighbour group was kept.  Entries of a group that is not kept get matched = 0; their
+ * other fields mean nothing.  The device results are then the reference's TrackData in order, and
+ * svs_calcFastMotionOnly_matched / svs_processMatchedPoints work on them as after svs_match.  *num_new_feat_matched =
+ * matched entries of groups 0 .. n_groups-2 (the new-point boundary in candidate order is group_end[n_groups-2]),
+ * *num_obs = all matched entries.  out (n entries) may be NULL.  Returns SVS_OK or a negative SVS_ERR_*; a refused
+ * call leaves the results of the previous match in place. */
+int svs_match_track(svs_matcher *h, const double T_cur_from_actkey[7], const double T_actkey_from_w[7],
+                    const svs_match_point *pts, int n, int n_groups, const int *group_end, int num_max_points,
+                    int search_radius, int thr_mean, int thr_std, svs_match_result *out, int *num_new_feat_matched,
+                    int *num_obs);
+
+/* processMatchedPoints (stereo_frontend.cpp:834-974) on the results of the last svs_match or svs_match_track:
+ * entry i (matched) passes when, with uvu_pred = SE3XYZ_STEREO::map(T_cur_from_actkey, xyz_actkey) on `cam`
+ * (level 0), |du|, |dv| < max_reproj_error * 2^anchor_level (a float product) and |du_right| < 3. * max_reproj_error;
+ * `abs` is read as the floating-point overload, as in svs_globalLoopClosure.  n_new is the candidate-index boundary
+ * between new points and tracks (num_new_feat_matched's group_end).  Writes the gated entries in match order to out
+ * (room for the n candidates of the last match; may be NULL), the statistics, the 3x3 add flags of addNewKeyframe
+ * (add_flags[3 * i + j] = grid3x3[i][j] <= min_num_points; may be NULL) and *drop_keyframe =
+ * svs_shallWeDropNewKeyframe(stats, T_cur_from_actkey, params) (may be NULL).  The gated points stay on the device as
+ * the per-level point tree at uv_pyr = uvu.xy / 2^anchor_level, with the flags and num_matched_points, for
+ * svs_addMorePoints(fresh = 0) until the next match.  Returns the number of gated entries, SVS_ERR_STATE when the last
+ * match was not svs_match / svs_match_track on this handle, or another negative SVS_ERR_*; a refused call changes
+ * nothing. */
+int svs_processMatchedPoints(svs_matcher *h, const double T_cur_from_actkey[7], const svs_cam *cam, int n_new,
+                             const svs_frontend_params *params, svs_tracked_point *out, svs_point_stats *stats,
+                             int add_flags[9], int *drop_keyframe);
+
+/* shallWeDropNewKeyframe (stereo_frontend.cpp:512-528): more than featureless_corners_thr quadrants with fewer than 15
+ * points, or |t(T_cur_from_actkey)| > parallax_thr, or av_track_length > 75.  Plain host code.  Returns 1 (drop) or 0,
+ * and SVS_ERR_INVALID (negative, so not usable as a boolean) when an argument is NULL. */
+int svs_shallWeDropNewKeyframe(const svs_point_stats *stats, const double T_cur_from_actkey[7],
+                               const svs_frontend_params *params);
+
+/* addMorePointsToOtherFrame (stereo_frontend.cpp:724-823) on the current frame of the matcher, for each level l:
+ *   a corner (u, v) of the level's FAST corners is taken when disp = disp0[v<<l][u<<l] * 2^-l > 0, (u<<l, v<<l) is in
+ *   the level-0 frame with border 1, the add flag of its 3x3 cell (thirds as in svs_point_stats, on u<<l, v<<l) is set
+ *   and the window Rect_<double>(u-R, v-R, 2R+1, 2R+1) holds no point of the level's tree (so a point at x-R is inside,
+ *   one at x+R+1 is not).  A taken corner joins the tree.  Level l keeps its taken corners until one makes
+ *   num_points_in[l] + kept exceed cap = num_max_points >> l (pyrFromZero_i of VisionTools, which is not vendored, is
+ *   assumed to be that shift), so it keeps min(taken, max(1, cap + 1 - num_points_in[l])).
+ *   fresh = 1: addNewPoints (the first frame): empty trees, every flag set, num_points_in = 0.  fresh = 0:
+ *   addMorePoints: the trees, flags and num_matched_points of the last svs_processMatchedPoints, which the call reads
+ *   and does not change; SVS_ERR_STATE when there was none since the last match.
+ * Order (a DEVIATION): the reference walks QuadTree::EquiIter (quadtree.h:163-336), which draws from Sample::uniform.
+ * The stand-in keeps its structure with a seeded hash.  With sm(x) = SplitMix64 (x += 0x9E3779B97F4A7C15;
+ * z = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)) and
+ * H(a, b, c, d, e) = sm(sm(sm(sm(sm(a) ^ b) ^ c) ^ d) ^ e) on uint64:
+ *   the tree is the regular midpoint quadtree over [0, w_l) x [0, h_l) (children split at x + width * 0.5 in double;
+ *   the reference's adaptive tree has the same non-empty nodes); a node's path holds two bits per depth from the root,
+ *   (u >= x_mid) << 1 | (v >= y_mid), the first step highest.  Of corners at one position only the first (lowest
+ *   index) exists, as in the reference's tree (delta 1).  At depth d = 0, 1, ... every node that holds a corner not
+ *   yet emitted emits the one with the smallest key H(seed, 0, l, u, v) (ties: lower corner index); the nodes of one
+ *   depth emit in the order of H(seed, 1, l, d, path), ties by path.  The corners are processed in emission order.
+ * Outputs are in seeding order, level by level: points (may be NULL), the same as svs_match_point rows with
+ * keyframe = keyframe_slot, anchor_level = l, xyz_anchor = xyz, anchor_obs_pyr = uv_pyr (may be NULL), and counts[l]
+ * (SVS_MATCH_MAX_LEVELS entries, may be NULL).  The reference's push_front keeps them in reverse in newpoint_map: a
+ * caller who wants its later match order reverses each call's rows.  cap (the room of points / rows) must be at least
+ * the sum over levels of (num_max_points >> l) + 1.  Levels wider or taller than 65535 are SVS_ERR_UNSUPPORTED.
+ * Returns the number of points or a negative SVS_ERR_*; a refused call changes nothing. */
+int svs_addMorePoints(svs_matcher *h, int fresh, const double T_newkey_from_cur[7], const svs_cam *cam, int keyframe_slot,
+                      const svs_frontend_params *params, svs_new_point *points, svs_match_point *rows, int cap,
+                      int *counts);
+
+
 /* ------------------------------------------------------------------ frame preprocessing ("next" row, SURVEY 8f) */
 
 typedef struct svs_prep svs_prep;

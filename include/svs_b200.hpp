@@ -331,7 +331,8 @@ class DenseTrackerCpuVariant {
 class GuidedMatcher {
  public:
   GuidedMatcher(const std::vector<svs_match_level>& cam_vec, int max_keyframes = 8, int max_points = 8192,
-                int max_keypoints = 65536) {
+                int max_keypoints = 65536)
+      : nlevels_((int)cam_vec.size()), max_points_(max_points) {
     ok_ = svs_matcher_create(-1, (int)cam_vec.size(), cam_vec.data(), max_keyframes, max_points, max_keypoints, &h_) == SVS_OK;
   }
   ~GuidedMatcher() { if (h_) svs_matcher_destroy(h_); }
@@ -350,11 +351,78 @@ class GuidedMatcher {
     return svs_match(h_, T_cur_from_actkey, T_actkey_from_w, ap_map.data(), (int)ap_map.size(), SEARCHRADIUS, thr_mean,
                      thr_std, track_data->data());
   }
+  // matchAndTrack's matching (stereo_frontend.cpp:977-1050): groups = newpoint_map[actkey_id], the neighbours'
+  // newpoint_map lists in strength_to_neighbors order, neighborhood_->point_list.  Returns num_obs or a negative SVS_ERR_*.
+  int matchAndTrack(const double T_cur_from_actkey[7], const double T_actkey_from_w[7],
+                    const std::vector<std::vector<svs_match_point>>& groups, int num_max_points,
+                    std::vector<svs_match_result>* track_data, int* num_new_feat_matched, int SEARCHRADIUS = 4,
+                    int thr_mean = 22, int thr_std = 10) {
+    std::vector<svs_match_point> pts;
+    std::vector<int> ends;
+    for (const auto& g : groups) { pts.insert(pts.end(), g.begin(), g.end()); ends.push_back((int)pts.size()); }
+    track_data->resize(pts.size());
+    if (!ok_) return -1;
+    int num_obs = 0;
+    const int rc = svs_match_track(h_, T_cur_from_actkey, T_actkey_from_w, pts.data(), (int)pts.size(), (int)ends.size(),
+                                   ends.data(), num_max_points, SEARCHRADIUS, thr_mean, thr_std, track_data->data(),
+                                   num_new_feat_matched, &num_obs);
+    return rc < 0 ? rc : num_obs;
+  }
+  // processMatchedPoints (stereo_frontend.cpp:834-974) on the last match, with the add flags of addNewKeyframe and the
+  // result of shallWeDropNewKeyframe.  Returns the number of gated entries or a negative SVS_ERR_*.
+  int processMatchedPoints(const double T_cur_from_actkey[7], const svs_cam& cam, int num_new_feat_boundary,
+                           std::vector<svs_tracked_point>* tracked, svs_point_stats* stats, int add_flags[9],
+                           bool* drop_keyframe, const svs_frontend_params& params = frontendDefaults()) {
+    tracked->resize(max_points_);
+    int drop = 0;
+    const int rc = ok_ ? svs_processMatchedPoints(h_, T_cur_from_actkey, &cam, num_new_feat_boundary, &params,
+                                                   tracked->data(), stats, add_flags, &drop)
+                       : -1;
+    tracked->resize(rc > 0 ? rc : 0);
+    if (drop_keyframe) *drop_keyframe = drop == 1;
+    return rc;
+  }
+  // addNewPoints (stereo_frontend.cpp:682-704): seeding of the first frame.  Returns the number of points or < 0.
+  int addNewPoints(const svs_cam& cam, int keyframe_slot, std::vector<svs_new_point>* points,
+                   std::vector<svs_match_point>* rows, const svs_frontend_params& params = frontendDefaults()) {
+    return seed(1, cam, keyframe_slot, points, rows, params);
+  }
+  // addMorePoints (stereo_frontend.cpp:706-720) after processMatchedPoints: its tree, flags and point counts.
+  int addMorePoints(const svs_cam& cam, int keyframe_slot, std::vector<svs_new_point>* points,
+                    std::vector<svs_match_point>* rows, const svs_frontend_params& params = frontendDefaults()) {
+    return seed(0, cam, keyframe_slot, points, rows, params);
+  }
+  static svs_frontend_params frontendDefaults() {
+    svs_frontend_params p = SVS_FRONTEND_PARAMS_DEFAULT;
+    return p;
+  }
 
  private:
+  int seed(int fresh, const svs_cam& cam, int slot, std::vector<svs_new_point>* points, std::vector<svs_match_point>* rows,
+           const svs_frontend_params& params) {
+    int cap = 0;
+    for (int l = 0; l < nlevels_; ++l) cap += (params.num_max_points >> l) + 1;
+    points->resize(cap);
+    rows->resize(cap);
+    const double I[7] = {0, 0, 0, 1, 0, 0, 0};
+    const int rc = ok_ ? svs_addMorePoints(h_, fresh, I, &cam, slot, &params, points->data(), rows->data(), cap, nullptr) : -1;
+    points->resize(rc > 0 ? rc : 0);
+    rows->resize(rc > 0 ? rc : 0);
+    return rc;
+  }
+  int nlevels_ = 0, max_points_ = 0;
   svs_matcher* h_ = nullptr;
   bool ok_ = false;
 };
+
+// StereoFrontend::PointStatistics (stereo_frontend.h:160-177)
+using PointStatistics = svs_point_stats;
+
+// StereoFrontend::shallWeDropNewKeyframe (stereo_frontend.cpp:512-528)
+inline bool shallWeDropNewKeyframe(const PointStatistics& stats, const double T_cur_from_actkey[7],
+                                   const svs_frontend_params& params = GuidedMatcher::frontendDefaults()) {
+  return svs_shallWeDropNewKeyframe(&stats, T_cur_from_actkey, &params) == 1;
+}
 
 // ScaViSLAM::PoseOptimizerParams (pose_optimizer.h:38-58)
 struct PoseOptimizerParams : svs_pose_params {

@@ -147,6 +147,36 @@ MATCH_POINT_DTYPE = np.dtype([("keyframe", "i4"), ("anchor_level", "i4"), ("xyz_
                               ("anchor_obs_pyr", "f8", 2)])
 
 
+class SvsFrontendParams(C.Structure):
+    _fields_ = [("seed", C.c_ulonglong), ("max_reproj_error", C.c_float), ("newpoint_clearance", C.c_int),
+                ("num_max_points", C.c_int), ("min_num_points", C.c_int), ("featureless_corners_thr", C.c_int),
+                ("parallax_thr", C.c_float)]
+
+
+def frontend_params(seed=0, max_reproj_error=2.0, newpoint_clearance=2, num_max_points=300, min_num_points=25,
+                    featureless_corners_thr=2, parallax_thr=0.75):
+    """svs_frontend_params; the defaults are SVS_FRONTEND_PARAMS_DEFAULT."""
+    return SvsFrontendParams(int(seed), float(max_reproj_error), int(newpoint_clearance), int(num_max_points),
+                             int(min_num_points), int(featureless_corners_thr), float(parallax_thr))
+
+
+class SvsPointStats(C.Structure):
+    _fields_ = [("num_matched_points", C.c_int * 4), ("grid2x2", C.c_int * 4), ("grid3x3", C.c_int * 9),
+                ("av_track_length", C.c_double), ("num_tracked", C.c_int), ("num_new", C.c_int)]
+
+    def as_dict(self):
+        return dict(num_matched_points=list(self.num_matched_points), grid2x2=np.array(self.grid2x2[:]).reshape(2, 2),
+                    grid3x3=np.array(self.grid3x3[:]).reshape(3, 3), av_track_length=self.av_track_length,
+                    num_tracked=self.num_tracked, num_new=self.num_new)
+
+
+# svs_tracked_point / svs_new_point
+TRACKED_POINT_DTYPE = np.dtype([("index", "i4"), ("is_new", "i4"), ("anchor_level", "i4"), ("reserved", "i4"),
+                                ("uvu", "f8", 3)])
+NEW_POINT_DTYPE = np.dtype([("level", "i4"), ("reserved", "i4"), ("uv_pyr", "f8", 2), ("uvu_pyr", "f8", 3),
+                            ("xyz", "f8", 3), ("normal", "f8", 3)])
+
+
 class SvsPlaceParams(C.Structure):
     _fields_ = [("num_ransac", C.c_int), ("pixel_thr", C.c_double), ("seed", C.c_ulonglong)]
 
@@ -214,6 +244,7 @@ EXPORTS = [
     "svs_place_create", "svs_place_destroy", "svs_place_last_error", "svs_place_add_location", "svs_place_num_places",
     "svs_place_last_words", "svs_place_last_scores", "svs_place_last_matches", "svs_place_last_hypotheses",
     "svs_globalLoopClosure", "svs_localRegisterFrame",
+    "svs_match_track", "svs_processMatchedPoints", "svs_shallWeDropNewKeyframe", "svs_addMorePoints",
 ]
 
 
@@ -390,6 +421,13 @@ def lib():
     L.svs_matcher_set_features_from_fast.argtypes = [vp, C.c_int, vp]
     L.svs_match.argtypes = [vp, c_dp, c_dp, C.POINTER(SvsMatchPoint), C.c_int, C.c_int, C.c_int, C.c_int,
                             C.POINTER(SvsMatchResult)]
+    L.svs_match_track.argtypes = [vp, c_dp, c_dp, C.POINTER(SvsMatchPoint), C.c_int, C.c_int, c_ip, C.c_int, C.c_int,
+                                  C.c_int, C.c_int, C.POINTER(SvsMatchResult), c_ip, c_ip]
+    L.svs_processMatchedPoints.argtypes = [vp, c_dp, C.POINTER(SvsCam), C.c_int, C.POINTER(SvsFrontendParams), vp,
+                                           C.POINTER(SvsPointStats), c_ip, c_ip]
+    L.svs_shallWeDropNewKeyframe.argtypes = [C.POINTER(SvsPointStats), c_dp, C.POINTER(SvsFrontendParams)]
+    L.svs_addMorePoints.argtypes = [vp, C.c_int, c_dp, C.POINTER(SvsCam), C.c_int, C.POINTER(SvsFrontendParams), vp, vp,
+                                    C.c_int, c_ip]
     L.svs_place_create.argtypes = [C.c_int, C.c_int, c_fp, C.POINTER(SvsCam), C.POINTER(vp)]
     L.svs_place_destroy.argtypes = [vp]
     L.svs_place_destroy.restype = None
@@ -1003,6 +1041,7 @@ class GuidedMatcher:
         if rc != 0:
             raise SvsError(rc, "svs_matcher_create failed (no CUDA device? there is no CPU fallback)")
         self.nlevels = len(levels)
+        self.max_points = max_points
 
     def close(self):
         if self._h:
@@ -1069,6 +1108,67 @@ class GuidedMatcher:
         if rc < 0:
             self._ck(rc)
         return out
+
+    def match_track(self, T_cur_from_actkey, T_actkey_from_w, groups, num_max_points, search_radius, thr_mean, thr_std):
+        """matchAndTrack's matching: groups = [newpoint_map[actkey], neighbours' newpoint_map lists ..., point_list],
+        each a MATCH_POINT_DTYPE array.  Returns (MATCH_RESULT_DTYPE over all candidates, num_new_feat_matched,
+        num_obs); entries of a neighbour group past the budget have matched = 0."""
+        if len(groups) < 2:
+            raise ValueError("groups: at least the active keyframe's new points and the neighbourhood's points")
+        pts = np.ascontiguousarray(np.concatenate([np.asarray(g, MATCH_POINT_DTYPE) for g in groups]), MATCH_POINT_DTYPE)
+        ends = np.cumsum([len(g) for g in groups]).astype(np.int32)
+        out = np.zeros(len(pts), MATCH_RESULT_DTYPE)
+        a, b = C.c_int(), C.c_int()
+        self._ck(lib().svs_match_track(self._h, _dp(np.ascontiguousarray(T_cur_from_actkey, np.float64)),
+                                       _dp(np.ascontiguousarray(T_actkey_from_w, np.float64)),
+                                       pts.ctypes.data_as(C.POINTER(SvsMatchPoint)), len(pts), len(groups), _ip(ends),
+                                       int(num_max_points), int(search_radius), int(thr_mean), int(thr_std),
+                                       out.ctypes.data_as(C.POINTER(SvsMatchResult)), C.byref(a), C.byref(b)))
+        return out, a.value, b.value
+
+    def process_matched_points(self, T_cur_from_actkey, cam, n_new, params=None):
+        """processMatchedPoints on the last match: returns (TRACKED_POINT_DTYPE gated entries, stats dict,
+        add_flags [3, 3], drop_keyframe)."""
+        p = params or frontend_params()
+        out = np.zeros(self.max_points, TRACKED_POINT_DTYPE)   # room for every candidate of the last match
+        st = SvsPointStats()
+        flags = np.zeros(9, np.int32)
+        drop = C.c_int()
+        rc = lib().svs_processMatchedPoints(self._h, _dp(np.ascontiguousarray(T_cur_from_actkey, np.float64)),
+                                            C.byref(SvsCam(*[float(x) for x in cam])), int(n_new), C.byref(p),
+                                            out.ctypes.data, C.byref(st), _ip(flags), C.byref(drop))
+        if rc < 0:
+            self._ck(rc)
+        return out[:rc], st.as_dict(), flags.reshape(3, 3), bool(drop.value)
+
+    def add_more_points(self, fresh, cam, keyframe_slot, T_newkey_from_cur=None, params=None):
+        """addNewPoints (fresh = 1) / addMorePoints (fresh = 0, after process_matched_points) on the current frame:
+        returns (NEW_POINT_DTYPE points, MATCH_POINT_DTYPE rows, counts per level), in seeding order."""
+        p = params or frontend_params()
+        T = np.array([0, 0, 0, 1, 0, 0, 0], np.float64) if T_newkey_from_cur is None else \
+            np.ascontiguousarray(T_newkey_from_cur, np.float64)
+        cap = sum((p.num_max_points >> l) + 1 for l in range(self.nlevels))
+        pts = np.zeros(cap, NEW_POINT_DTYPE)
+        rows = np.zeros(cap, MATCH_POINT_DTYPE)
+        counts = np.zeros(4, np.int32)
+        rc = lib().svs_addMorePoints(self._h, int(fresh), _dp(T), C.byref(SvsCam(*[float(x) for x in cam])),
+                                     int(keyframe_slot), C.byref(p), pts.ctypes.data, rows.ctypes.data, cap, _ip(counts))
+        if rc < 0:
+            self._ck(rc)
+        return pts[:rc], rows[:rc], counts[:self.nlevels]
+
+
+def shall_we_drop_new_keyframe(stats, T_cur_from_actkey, params=None):
+    """svs_shallWeDropNewKeyframe on a stats dict of process_matched_points."""
+    st = SvsPointStats()
+    st.num_matched_points[:] = list(stats["num_matched_points"])
+    st.grid2x2[:] = [int(x) for x in np.asarray(stats["grid2x2"]).reshape(-1)]
+    st.grid3x3[:] = [int(x) for x in np.asarray(stats["grid3x3"]).reshape(-1)]
+    st.av_track_length = float(stats["av_track_length"])
+    st.num_tracked, st.num_new = int(stats["num_tracked"]), int(stats["num_new"])
+    p = params or frontend_params()
+    return bool(lib().svs_shallWeDropNewKeyframe(C.byref(st), _dp(np.ascontiguousarray(T_cur_from_actkey, np.float64)),
+                                                 C.byref(p)))
 
 
 class FramePreprocessor:

@@ -5,6 +5,48 @@
 #include "../../include/svs_b200.h"
 
 namespace svs {
+#ifdef __CUDACC__
+// the reprojection gate of processMatchedPoints and of the loop / registration checks: the match predicted with T
+// (SE3XYZ_STEREO::map as k_pose_lm computes it, R = T's rotation, camera f, px, py, b) lies within thr_uv pixels in u
+// and v and within thr_r in u_right.  Compile with -fmad=false: the oracles restate it without contraction.
+__device__ __forceinline__ bool reproj_gate(const svs_match_result& r, const double R[9], const double T[7], double f, double px,
+                                            double py, double b, double thr_uv, double thr_r) {
+  const double X0 = r.xyz_actkey[0], X1 = r.xyz_actkey[1], X2 = r.xyz_actkey[2];
+  const double x = R[0] * X0 + R[1] * X1 + R[2] * X2 + T[4];
+  const double y = R[3] * X0 + R[4] * X1 + R[5] * X2 + T[5];
+  const double z = R[6] * X0 + R[7] * X1 + R[8] * X2 + T[6];
+  const double d0 = r.obs[0] - (f * (x / z) + px);
+  const double d1 = r.obs[1] - (f * (y / z) + py);
+  const double d2 = r.obs[2] - ((x - b) / z * f + px);
+  return fabs(d0) < thr_uv && fabs(d1) < thr_uv && fabs(d2) < thr_r;
+}
+#endif
+
+// the matcher's internals that frontend_points.cu works on (match.cu owns them)
+struct FrontState;   // frontend_points.cu: the gated points (the point tree), flags and seeding scratch, allocated on first use
+struct MatcherCore {
+  int device, nlevels, max_pts, max_kp;
+  svs_match_level lv[SVS_MATCH_MAX_LEVELS];
+  cudaStream_t stream;
+  svs_match_point* d_pts;          // the handle's candidate buffer
+  svs_match_result* d_res;
+  const int* d_kp_xy[SVS_MATCH_MAX_LEVELS];
+  int nkp[SVS_MATCH_MAX_LEVELS];
+  const float* d_disp;
+  int disp_pitch;
+  int last_n;
+  int last_pts_own;                // the last match read its candidates from d_pts (svs_match / svs_match_track)
+  unsigned long long match_serial; // counts every match on the handle
+  FrontState** front;
+};
+__attribute__((visibility("hidden"))) void matcher_core(svs_matcher* m, MatcherCore* c);
+__attribute__((visibility("hidden"))) void matcher_set_error(svs_matcher* m, const char* msg);
+// k_match on n candidates already in the handle's d_pts, enqueued on its stream (no wait); the results become the
+// handle's last match (last_n = n) once the caller has synchronised
+__attribute__((visibility("hidden"))) int match_enqueue_own(svs_matcher* m, const double T_cur_from_actkey[7],
+                                                            const double T_actkey_from_w[7], int n, int search_radius,
+                                                            int thr_mean, int thr_std);
+__attribute__((visibility("hidden"))) void front_state_free(FrontState* s);
 // device-resident results of the last svs_match on this handle (n = number of candidate points)
 __attribute__((visibility("hidden"))) void matcher_device_results(svs_matcher* m, const svs_match_result** d_res, int* n,
                                                                    int* device);

@@ -273,6 +273,9 @@ struct svs_matcher {
   svs_match_point* d_pts = nullptr;
   svs_match_result* d_res = nullptr;
   int last_n = 0;   // candidate points of the last svs_match (results stay in d_res)
+  int last_pts_own = 0;                 // the last match read its candidates from d_pts
+  unsigned long long match_serial = 0;  // counts every match on the handle
+  svs::FrontState* front = nullptr;     // frontend_points.cu's state, allocated on first use
 };
 
 #define MCK(call)                                                       \
@@ -288,6 +291,18 @@ namespace svs {
 void matcher_device_results(svs_matcher* m, const svs_match_result** d_res, int* n, int* device) {
   *d_res = m->d_res; *n = m->last_n; *device = m->device;
 }
+void matcher_core(svs_matcher* m, MatcherCore* c) {
+  c->device = m->device; c->nlevels = m->nlevels; c->max_pts = m->max_pts; c->max_kp = m->max_kp;
+  for (int l = 0; l < kMaxLv; ++l) {
+    c->lv[l] = l < m->nlevels ? m->lv[l] : svs_match_level{};
+    c->d_kp_xy[l] = m->d_kp_xy[l]; c->nkp[l] = m->nkp[l];
+  }
+  c->stream = m->stream; c->d_pts = m->d_pts; c->d_res = m->d_res;
+  c->d_disp = m->d_disp; c->disp_pitch = m->disp_pitch;
+  c->last_n = m->last_n; c->last_pts_own = m->last_pts_own; c->match_serial = m->match_serial;
+  c->front = &m->front;
+}
+void matcher_set_error(svs_matcher* m, const char* msg) { m->err = msg; }
 void matcher_view(svs_matcher* m, MatcherView* v) {
   v->device = m->device; v->nlevels = m->nlevels; v->max_kf = m->max_kf; v->max_pts = m->max_pts;
   for (int l = 0; l < kMaxLv; ++l) v->lv[l] = l < m->nlevels ? m->lv[l] : svs_match_level{};
@@ -324,12 +339,26 @@ int svs::match_device(svs_matcher* h, const double T_cur_from_actkey[7], const d
                       const svs_match_point* d_pts, int n, int search_radius, int thr_mean, int thr_std) {
   svs::NvtxRange nvtx_("match");
   h->last_n = 0;
+  h->last_pts_own = 0;
+  ++h->match_serial;
   if (n < 0 || n > h->max_pts || search_radius < 0) { h->err = "match_device: bad point count or radius"; return SVS_ERR_INVALID; }
   if (n == 0) return SVS_OK;
   cudaSetDevice(h->device);
   const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, d_pts, n, search_radius, thr_mean, thr_std);
   if (rc != SVS_OK) return rc;
   MCK(cudaStreamSynchronize(h->stream));
+  h->last_n = n;
+  return SVS_OK;
+}
+
+int svs::match_enqueue_own(svs_matcher* h, const double T_cur_from_actkey[7], const double T_actkey_from_w[7], int n,
+                           int search_radius, int thr_mean, int thr_std) {
+  h->last_n = 0;
+  h->last_pts_own = 1;
+  ++h->match_serial;
+  if (n == 0) return SVS_OK;
+  const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, h->d_pts, n, search_radius, thr_mean, thr_std);
+  if (rc != SVS_OK) return rc;
   h->last_n = n;
   return SVS_OK;
 }
@@ -393,6 +422,7 @@ void svs_matcher_destroy(svs_matcher * h) {
   }
   for (unsigned char* p : h->d_kfimg) cudaFree(p);
   cudaFree(h->d_kf); cudaFree(h->d_disp); cudaFree(h->d_pts); cudaFree(h->d_res);
+  svs::front_state_free(h->front);
   if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
@@ -510,6 +540,8 @@ int svs_match(svs_matcher * h, const double T_cur_from_actkey[7], const double T
   if (!h || !T_cur_from_actkey || !T_actkey_from_w || n < 0 || n > h->max_pts || (n && (!pts || !out)) || search_radius < 0)
     return SVS_ERR_INVALID;
   h->last_n = 0;
+  h->last_pts_own = 1;
+  ++h->match_serial;
   if (n == 0) return 0;
   cudaSetDevice(h->device);
   MCK(cudaMemcpyAsync(h->d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
