@@ -266,11 +266,12 @@ def lib():
         raise RuntimeError(f"{LIB_PATH} missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
     L = C.CDLL(LIB_PATH)
     vp = C.c_void_p
+    for prefix in ("ba", "chol6", "fast", "dt", "dtc", "prep", "matcher", "pose", "place", "map", "constraints"):
+        destroy = getattr(L, f"svs_{prefix}_destroy")
+        destroy.argtypes, destroy.restype = [vp], None
+        last_error = getattr(L, "svs_last_error" if prefix == "ba" else f"svs_{prefix}_last_error")
+        last_error.argtypes, last_error.restype = [vp], C.c_char_p
     L.svs_ba_create.argtypes = [C.POINTER(SvsBaOpts), C.POINTER(vp)]
-    L.svs_ba_destroy.argtypes = [vp]
-    L.svs_ba_destroy.restype = None
-    L.svs_last_error.argtypes = [vp]
-    L.svs_last_error.restype = C.c_char_p
     prob = [C.c_int, c_dp, c_up, C.c_int, c_dp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp,
             C.c_int, c_ip, c_ip, c_dp, c_dp, C.POINTER(SvsCam)]
     L.svs_ba_set_problem.argtypes = [vp] + prob
@@ -305,10 +306,6 @@ def lib():
     L.svs_ba_set_problem_sharded.argtypes = [vp] + prob
     L.svs_ba_get_points_all.argtypes = [vp, c_dp]
     L.svs_chol6_create.argtypes = [C.c_int, C.POINTER(vp)]
-    L.svs_chol6_destroy.argtypes = [vp]
-    L.svs_chol6_destroy.restype = None
-    L.svs_chol6_last_error.argtypes = [vp]
-    L.svs_chol6_last_error.restype = C.c_char_p
     L.svs_chol6_init.argtypes = [vp]
     L.svs_chol6_solve.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                   C.POINTER(SvsChol6Stats)]
@@ -317,10 +314,6 @@ def lib():
     L.svs_chol6_solve_pattern.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_void_p, C.c_int, c_ip, c_ip, C.c_void_p, C.c_int,
                                           C.POINTER(SvsChol6InvStats)]
     L.svs_fast_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
-    L.svs_fast_destroy.argtypes = [vp]
-    L.svs_fast_destroy.restype = None
-    L.svs_fast_last_error.argtypes = [vp]
-    L.svs_fast_last_error.restype = C.c_char_p
     L.svs_fast_grid_init.argtypes = [C.c_int] * 9 + [C.POINTER(SvsFastGridParams), C.POINTER(SvsFastCell)]
     L.svs_fast_set_image.argtypes = [vp, c_up, C.c_int, C.c_int, C.c_int]
     L.svs_fast_set_image_device.argtypes = [vp, C.c_void_p, C.c_int, C.c_int, C.c_int]
@@ -329,10 +322,6 @@ def lib():
                                              c_ip, C.c_int, c_ip]
     c_fp = C.POINTER(C.c_float)
     L.svs_dt_create.argtypes = [C.c_int] * 5 + [C.POINTER(vp)]
-    L.svs_dt_destroy.argtypes = [vp]
-    L.svs_dt_destroy.restype = None
-    L.svs_dt_last_error.argtypes = [vp]
-    L.svs_dt_last_error.restype = C.c_char_p
     L.svs_dt_set_intrinsics.argtypes = [vp, C.c_int, C.c_float, C.c_float, C.c_float]
     L.svs_dt_set_images.argtypes = [vp, C.c_int, c_fp, c_fp, c_fp, c_fp, C.c_int]
     L.svs_dt_set_disparity.argtypes = [vp, c_fp, C.c_int, C.c_int, C.c_int]
@@ -344,10 +333,6 @@ def lib():
     L.svs_dt_track.argtypes = [vp, c_dp, C.POINTER(SvsDtStats)]
     L.svs_dt_residual_image.argtypes = [vp, C.c_int, c_dp, c_fp]
     L.svs_prep_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
-    L.svs_prep_destroy.argtypes = [vp]
-    L.svs_prep_destroy.restype = None
-    L.svs_prep_last_error.argtypes = [vp]
-    L.svs_prep_last_error.restype = C.c_char_p
     L.svs_prep_process.argtypes = [vp, c_up, C.c_int]
     pvp = C.POINTER(C.c_void_p)
     L.svs_prep_level.argtypes = [vp, C.c_int, c_ip, c_ip, pvp, c_ip, pvp, pvp, pvp, c_ip]
@@ -357,10 +342,6 @@ def lib():
     L.svs_dt_swap_prev_cur.argtypes = [vp]
     L.svs_matcher_set_pyramid_device.argtypes = [vp, C.c_int, c_dp, C.POINTER(C.c_void_p), c_ip]
     L.svs_map_create.argtypes = [C.c_int, C.POINTER(vp)]
-    L.svs_map_destroy.argtypes = [vp]
-    L.svs_map_destroy.restype = None
-    L.svs_map_last_error.argtypes = [vp]
-    L.svs_map_last_error.restype = C.c_char_p
     L.svs_map_set.argtypes = [vp, C.c_int, c_dp, C.c_int, c_ip, c_dp, c_ip, c_ip, c_dp, c_ip]
     L.svs_map_update_poses.argtypes = [vp, C.c_int, c_ip, c_dp]
     L.svs_map_update_points.argtypes = [vp, C.c_int, c_ip, c_dp]
@@ -379,17 +360,9 @@ def lib():
     L.svs_localRegisterFrame.argtypes = [vp, vp, vp, C.POINTER(SvsCam), C.c_int, C.c_int, C.c_int, c_ip, c_ip,
                                          C.POINTER(SvsRegisterResult), C.c_int, vp, C.c_int, c_ip, c_dp, c_ip, c_ip]
     L.svs_constraints_create.argtypes = [C.c_int, C.POINTER(vp)]
-    L.svs_constraints_destroy.argtypes = [vp]
-    L.svs_constraints_destroy.restype = None
-    L.svs_constraints_last_error.argtypes = [vp]
-    L.svs_constraints_last_error.restype = C.c_char_p
     L.svs_computeConstraint_batch.argtypes = [vp, C.c_int, c_dp, c_ip, c_ip, C.c_int, c_ip, c_dp, C.c_int, c_ip, c_ip,
                                               c_dp, c_dp, c_ip]
     L.svs_dtc_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
-    L.svs_dtc_destroy.argtypes = [vp]
-    L.svs_dtc_destroy.restype = None
-    L.svs_dtc_last_error.argtypes = [vp]
-    L.svs_dtc_last_error.restype = C.c_char_p
     L.svs_dtc_set_prev_u8.argtypes = [vp, C.c_int, C.c_void_p, C.c_int, C.c_int]
     L.svs_dtc_set_cur.argtypes = [vp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.svs_dtc_set_disparity.argtypes = [vp, c_fp, C.c_int]
@@ -398,10 +371,6 @@ def lib():
     L.svs_dtc_set_point_cloud.argtypes = [vp, C.c_int, c_fp]
     L.svs_denseTrackingCpu.argtypes = [vp, C.POINTER(SvsCam), c_dp, C.POINTER(SvsDtStats)]
     L.svs_pose_create.argtypes = [C.c_int, C.c_int, C.POINTER(vp)]
-    L.svs_pose_destroy.argtypes = [vp]
-    L.svs_pose_destroy.restype = None
-    L.svs_pose_last_error.argtypes = [vp]
-    L.svs_pose_last_error.restype = C.c_char_p
     L.svs_calcFastMotionOnly.argtypes = [vp, C.c_int, c_ip, c_dp, C.c_int, c_dp, C.POINTER(SvsCam),
                                          C.POINTER(SvsPoseParams), c_dp, C.POINTER(SvsPoseStats)]
     L.svs_calcFastMotionOnly_matched.argtypes = [vp, vp, C.POINTER(SvsCam), C.POINTER(SvsPoseParams), c_dp,
@@ -411,10 +380,6 @@ def lib():
     L.svs_pose_grad.argtypes = [vp, C.c_double, vp, vp, vp, vp, C.c_int, C.POINTER(SvsPoseGradStats)]
     ucpp = C.POINTER(C.POINTER(C.c_ubyte))
     L.svs_matcher_create.argtypes = [C.c_int, C.c_int, C.POINTER(SvsMatchLevel), C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
-    L.svs_matcher_destroy.argtypes = [vp]
-    L.svs_matcher_destroy.restype = None
-    L.svs_matcher_last_error.argtypes = [vp]
-    L.svs_matcher_last_error.restype = C.c_char_p
     L.svs_matcher_set_keyframe.argtypes = [vp, C.c_int, c_dp, ucpp, c_ip]
     L.svs_matcher_set_current.argtypes = [vp, ucpp, c_ip, c_fp, C.c_int]
     L.svs_matcher_set_features.argtypes = [vp, C.c_int, c_ip, c_ip, C.c_int]
@@ -429,10 +394,6 @@ def lib():
     L.svs_addMorePoints.argtypes = [vp, C.c_int, c_dp, C.POINTER(SvsCam), C.c_int, C.POINTER(SvsFrontendParams), vp, vp,
                                     C.c_int, c_ip]
     L.svs_place_create.argtypes = [C.c_int, C.c_int, c_fp, C.POINTER(SvsCam), C.POINTER(vp)]
-    L.svs_place_destroy.argtypes = [vp]
-    L.svs_place_destroy.restype = None
-    L.svs_place_last_error.argtypes = [vp]
-    L.svs_place_last_error.restype = C.c_char_p
     L.svs_place_add_location.argtypes = [vp, C.c_int, C.c_int, c_fp, c_dp, C.c_int, C.c_int, c_ip,
                                          C.POINTER(SvsPlaceParams), C.POINTER(SvsPlaceResult), c_ip, c_ip]
     L.svs_place_num_places.argtypes = [vp]
@@ -471,21 +432,21 @@ class SvsError(RuntimeError):
         self.rc = rc
 
 
-class BundleAdjuster:
-    """Thin host-side mirror of SlamGraph::optimize (reference slam_graph.cpp:319-355)."""
+class _Handle:
+    """One opaque handle of the C ABI.  A subclass names its destroy and last-error functions; close() (or the
+    garbage collector) destroys the handle."""
+    _destroy = _last_error = None
+    _h = None
 
-    def __init__(self, device: int = -1, flags: int = 0):
+    def _open(self, create, *args, why="no CUDA device? there is no CPU fallback"):
         self._h = C.c_void_p()
-        o = SvsBaOpts(device, flags)
-        rc = lib().svs_ba_create(C.byref(o), C.byref(self._h))
+        rc = getattr(lib(), create)(*args, C.byref(self._h))
         if rc != 0:
-            raise SvsError(rc, "svs_ba_create failed (no CUDA device? there is no CPU fallback)")
-        self._keep = None
-        self.P = self.L = self.E = self.C = 0
+            raise SvsError(rc, f"{create} failed ({why})")
 
     def close(self):
         if self._h:
-            lib().svs_ba_destroy(self._h)
+            getattr(lib(), self._destroy)(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -494,9 +455,24 @@ class BundleAdjuster:
         except Exception:
             pass
 
-    def _check(self, rc):
+    def _error(self, rc):
+        return SvsError(rc, getattr(lib(), self._last_error)(self._h).decode())
+
+    def _ck(self, rc):
         if rc != 0:
-            raise SvsError(rc, lib().svs_last_error(self._h).decode())
+            raise self._error(rc)
+
+
+class BundleAdjuster(_Handle):
+    """Thin host-side mirror of SlamGraph::optimize (reference slam_graph.cpp:319-355)."""
+
+    _destroy, _last_error = "svs_ba_destroy", "svs_last_error"
+
+    def __init__(self, device: int = -1, flags: int = 0):
+        o = SvsBaOpts(device, flags)
+        self._open("svs_ba_create", C.byref(o))
+        self._keep = None
+        self.P = self.L = self.E = self.C = 0
 
     @staticmethod
     def _arrays(pb):
@@ -529,7 +505,7 @@ class BundleAdjuster:
         else:
             k = self._arrays(pb)
             args, cam = self._prob_args(pb, k)
-            self._check(lib().svs_ba_set_problem(self._h, *args))
+            self._ck(lib().svs_ba_set_problem(self._h, *args))
         self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
 
     def _set_problem_device(self, pb):
@@ -551,7 +527,7 @@ class BundleAdjuster:
         cam = SvsCam(float(pb.cam[0]), float(pb.cam[1]), float(pb.cam[2]), float(pb.cam[3]))
         torch.cuda.current_stream(dev).synchronize()   # the handle reads the arrays on its own stream
         p = ptr
-        self._check(lib().svs_ba_set_problem_device(
+        self._ck(lib().svs_ba_set_problem_device(
             self._h, int(pb.P), p["pose_qt"], p["fixed"], int(pb.L), p["psi"], int(pb.E), p["e_point"], p["e_pose"],
             p["e_anchor"], p["e_obs"], p["e_info"], int(pb.C), p["c_i"], p["c_j"], p["c_T"], p["c_Lambda"],
             C.byref(cam)))
@@ -561,40 +537,40 @@ class BundleAdjuster:
         it = lib().svs_ba_optimize(self._h, int(num_iters), int(robust), float(huber_delta), float(lambda_init),
                                    int(max_trials), C.byref(st))
         if it <= -100:
-            raise SvsError(it + 100, lib().svs_last_error(self._h).decode())
+            self._ck(it + 100)
         return it, st.as_dict()
 
     def poses(self):
         out = np.zeros((self.P, 7))
-        self._check(lib().svs_ba_get_poses(self._h, _dp(out)))
+        self._ck(lib().svs_ba_get_poses(self._h, _dp(out)))
         return out
 
     def points(self):
         out = np.zeros((self.L, 3))
-        self._check(lib().svs_ba_get_points(self._h, _dp(out)))
+        self._ck(lib().svs_ba_get_points(self._h, _dp(out)))
         return out
 
     def reset_state(self):
-        self._check(lib().svs_ba_reset_state(self._h))
+        self._ck(lib().svs_ba_reset_state(self._h))
 
     def chi2(self, robust=True, huber_delta=1.0):
         v = C.c_double()
-        self._check(lib().svs_ba_chi2(self._h, int(robust), float(huber_delta), C.byref(v)))
+        self._ck(lib().svs_ba_chi2(self._h, int(robust), float(huber_delta), C.byref(v)))
         return v.value
 
     def reduced_system(self, robust=True, huber_delta=1.0, lam=50.0):
         n = 6 * self.P
         S, bs = np.zeros((n, n)), np.zeros(n)
         chi = C.c_double()
-        self._check(lib().svs_ba_reduced_system(self._h, int(robust), float(huber_delta), float(lam), _dp(S), _dp(bs),
-                                                C.byref(chi)))
+        self._ck(lib().svs_ba_reduced_system(self._h, int(robust), float(huber_delta), float(lam), _dp(S), _dp(bs),
+                                             C.byref(chi)))
         return S, bs, chi.value
 
     def solve_reduced(self, robust=True, huber_delta=1.0, lam=50.0):
         x = np.zeros(6 * self.P)
         rc = lib().svs_ba_solve_reduced(self._h, int(robust), float(huber_delta), float(lam), _dp(x))
         if rc < 0:
-            self._check(rc)
+            self._ck(rc)
         return x, rc
 
     def covariance(self, robust=True, huber_delta=1.0, lam=0.0, pairs=()):
@@ -611,7 +587,7 @@ class BundleAdjuster:
                                      _ip(pi) if n else None, _ip(pj) if n else None, _dp(pair) if n else None,
                                      _dp(point), C.byref(st))
         if rc < 0:
-            self._check(rc)
+            self._ck(rc)
         return pose, pair, point, rc, st.as_dict()
 
     def observation_grad(self, dL_dpose=None, dL_dpsi=None, robust=True, huber_delta=1.0, lam=0.0):
@@ -643,7 +619,7 @@ class BundleAdjuster:
             rc = lib().svs_ba_observation_grad(self._h, int(robust), float(huber_delta), float(lam), ptr(gp), ptr(gl),
                                                ptr(dobs), ptr(dinfo), 0, C.byref(st))
         if rc < 0:
-            self._check(rc)
+            self._ck(rc)
         return dobs, dinfo, rc, st.as_dict()
 
     # outputs of window_grad: name -> (svs_ba_grad_out member, trailing shape)
@@ -688,57 +664,57 @@ class BundleAdjuster:
         rc = lib().svs_ba_window_grad(self._h, int(robust), float(huber_delta), float(lam), ptr(gp), ptr(gl),
                                       C.byref(out), on_device, C.byref(st))
         if rc < 0:
-            self._check(rc)
+            self._ck(rc)
         return res, rc, st.as_dict()
 
     # ---- stepwise trial API (window split by landmarks across ranks, SURVEY.md 8e)
     def set_structure(self, pairs):
         pairs = np.ascontiguousarray(pairs, np.int32).reshape(-1, 2)
         pi, pj = np.ascontiguousarray(pairs[:, 0]), np.ascontiguousarray(pairs[:, 1])
-        self._check(lib().svs_ba_set_structure(self._h, len(pairs), _ip(pi), _ip(pj)))
+        self._ck(lib().svs_ba_set_structure(self._h, len(pairs), _ip(pi), _ip(pj)))
 
     def lm_begin(self, lambda_init=50.0, max_trials=5):
-        self._check(lib().svs_ba_lm_begin(self._h, float(lambda_init), int(max_trials)))
+        self._ck(lib().svs_ba_lm_begin(self._h, float(lambda_init), int(max_trials)))
 
     def trial_build(self, robust=True, huber_delta=1.0):
-        self._check(lib().svs_ba_trial_build(self._h, int(robust), float(huber_delta)))
+        self._ck(lib().svs_ba_trial_build(self._h, int(robust), float(huber_delta)))
 
     def system_buffers(self):
         """(ptr_S, nS, ptr_bp, ptr_bc, nb, ptr_totals): raw device pointers for the caller's collective."""
         S, bp, bc, tot = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         nS, nb = C.c_longlong(), C.c_longlong()
-        self._check(lib().svs_ba_system_buffers(self._h, C.byref(S), C.byref(nS), C.byref(bp), C.byref(bc), C.byref(nb),
-                                                C.byref(tot)))
+        self._ck(lib().svs_ba_system_buffers(self._h, C.byref(S), C.byref(nS), C.byref(bp), C.byref(bc), C.byref(nb),
+                                             C.byref(tot)))
         return S.value, nS.value, bp.value, bc.value, nb.value, tot.value
 
     def trial_solve(self, robust=True, huber_delta=1.0):
-        self._check(lib().svs_ba_trial_solve(self._h, int(robust), float(huber_delta)))
+        self._ck(lib().svs_ba_trial_solve(self._h, int(robust), float(huber_delta)))
 
     def trial_decide(self):
         a, s, i = C.c_int(), C.c_int(), C.c_int()
-        self._check(lib().svs_ba_trial_decide(self._h, C.byref(a), C.byref(s), C.byref(i)))
+        self._ck(lib().svs_ba_trial_decide(self._h, C.byref(a), C.byref(s), C.byref(i)))
         return a.value, s.value, i.value
 
     # ---- one window sharded by landmarks across GPUs, driven inside the library (NCCL on the handle's stream)
     def comm_init(self, nranks, rank, unique_id):
         """unique_id: the 128 bytes rank 0 got from `comm_unique_id()`, broadcast by the caller."""
-        self._check(lib().svs_ba_comm_init(self._h, int(nranks), int(rank), bytes(unique_id)))
+        self._ck(lib().svs_ba_comm_init(self._h, int(nranks), int(rank), bytes(unique_id)))
 
     def set_problem_sharded(self, pb):
         """Every rank passes the WHOLE window; the library keeps landmarks l % nranks == rank."""
         k = self._arrays(pb)
         args, cam = self._prob_args(pb, k)
-        self._check(lib().svs_ba_set_problem_sharded(self._h, *args))
+        self._ck(lib().svs_ba_set_problem_sharded(self._h, *args))
         self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
 
     def points_all(self):
         out = np.zeros((self.L, 3))
-        self._check(lib().svs_ba_get_points_all(self._h, _dp(out)))
+        self._ck(lib().svs_ba_get_points_all(self._h, _dp(out)))
         return out
 
     def lm_stats(self):
         st = SvsBaStats()
-        self._check(lib().svs_ba_lm_stats(self._h, C.byref(st)))
+        self._ck(lib().svs_ba_lm_stats(self._h, C.byref(st)))
         return st.as_dict()
 
     def optimise_inner_and_outer_window(self, pb, num_iters, robust=True, huber_delta=1.0):
@@ -751,39 +727,25 @@ class BundleAdjuster:
         it = lib().svs_optimiseInnerAndOuterWindow(self._h, *args, int(num_iters), int(robust), float(huber_delta),
                                                    C.byref(st))
         if it <= -100:
-            raise SvsError(it + 100, lib().svs_last_error(self._h).decode())
+            self._ck(it + 100)
         self.P, self.L, self.E, self.C = pb.P, pb.L, pb.E, pb.C
         return it, k["pose_qt"], k["psi"], st.as_dict()
 
 
-class BlockCholesky6:
+class BlockCholesky6(_Handle):
     """g2o's LinearSolver<Matrix6d>::solve(A, x, b) on the device (svs_chol6_*): A is the upper triangle of a
     symmetric positive-definite matrix in block CCS -- col_ptr [P+1], row_idx [nnzb] (ascending, row <= column,
     every column ends in its diagonal block), blocks [nnzb][36] with each block column-major (Eigen's
     Matrix6d::data(); from numpy, B.ravel(order="F")) -- and b has 6P entries.  No damping is added."""
 
+    _destroy, _last_error = "svs_chol6_destroy", "svs_chol6_last_error"
+
     def __init__(self, device: int = -1):
-        self._h = C.c_void_p()
-        rc = lib().svs_chol6_create(int(device), C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_chol6_create failed (no CUDA device? there is no CPU fallback)")
-
-    def close(self):
-        if self._h:
-            lib().svs_chol6_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open("svs_chol6_create", int(device))
 
     def init(self):
         """LinearSolver::init(): forget the cached symbolic analysis."""
-        rc = lib().svs_chol6_init(self._h)
-        if rc != 0:
-            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+        self._ck(lib().svs_chol6_init(self._h))
 
     def solve(self, col_ptr, row_idx, blocks, b):
         """Returns (x, status, stats): status 0 = solved, 1 = not positive definite (x is zero).  blocks and b are
@@ -810,7 +772,7 @@ class BlockCholesky6:
         rc = lib().svs_chol6_solve(self._h, P, _ip(col_ptr), _ip(row_idx), C.c_void_p(args[0]), C.c_void_p(args[1]),
                                    C.c_void_p(args[2]), args[3], C.byref(st))
         if rc < 0:
-            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+            self._ck(rc)
         return x, rc, st.as_dict()
 
     def _inverse(self, col_ptr, row_idx, blocks, n, call):
@@ -834,7 +796,7 @@ class BlockCholesky6:
             args = (blocks.data_ptr(), out.data_ptr(), 1)
         rc = call(P, _ip(col_ptr), _ip(row_idx), C.c_void_p(args[0]), C.c_void_p(args[1]), args[2], C.byref(st))
         if rc < 0:
-            raise SvsError(rc, lib().svs_chol6_last_error(self._h).decode())
+            self._ck(rc)
         # column-major blocks -> ordinary 6x6 matrices
         return out.reshape(n, 6, 6).swapaxes(1, 2), rc, st.as_dict()
 
@@ -856,18 +818,17 @@ class BlockCholesky6:
                                  self._h, P, cp, ri, bl, n, _ip(r), _ip(c), out, dev, st))
 
 
-class FastGrid:
+class FastGrid(_Handle):
     """Host-side mirror of ScaViSLAM's FastGrid (reference fast_grid.h:30-64): same constructor
     arguments, detect / detectAdaptively on the GPU through the C ABI.  Keypoints come back as
     (xy[n,2] int32, cell_off[ncells+1]); the quadtree content of keypoint i in cell c is
     i - cell_off[c]."""
 
+    _destroy, _last_error = "svs_fast_destroy", "svs_fast_last_error"
+
     def __init__(self, img_w, img_h, num_features_per_cell, boundary_per_cell, fast_thr, grid_w, grid_h,
                  fast_min=10, fast_max=40, device=-1, max_keypoints=200000):
-        self._h = C.c_void_p()
-        rc = lib().svs_fast_create(device, img_w, img_h, max_keypoints, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_fast_create failed (no CUDA device? there is no CPU fallback)")
+        self._open("svs_fast_create", device, img_w, img_h, max_keypoints)
         self.params = SvsFastGridParams()
         self.cells = (SvsFastCell * (grid_w * grid_h))()
         rc = lib().svs_fast_grid_init(img_w, img_h, num_features_per_cell, boundary_per_cell, fast_thr, grid_w,
@@ -877,30 +838,12 @@ class FastGrid:
         self.max_kp = max_keypoints
         self.ncells = grid_w * grid_h
 
-    def close(self):
-        if self._h:
-            lib().svs_fast_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _err(self, rc):
-        raise SvsError(rc, lib().svs_fast_last_error(self._h).decode())
-
     def set_image(self, img):
         img = np.ascontiguousarray(img, np.uint8)
-        rc = lib().svs_fast_set_image(self._h, img.ctypes.data_as(c_up), img.strides[0], img.shape[1], img.shape[0])
-        if rc != 0:
-            self._err(rc)
+        self._ck(lib().svs_fast_set_image(self._h, img.ctypes.data_as(c_up), img.strides[0], img.shape[1], img.shape[0]))
 
     def set_image_device(self, ptr, pitch, w, h):
-        rc = lib().svs_fast_set_image_device(self._h, C.c_void_p(ptr), pitch, w, h)
-        if rc != 0:
-            self._err(rc)
+        self._ck(lib().svs_fast_set_image_device(self._h, C.c_void_p(ptr), pitch, w, h))
 
     def cell_list(self):
         return [(c.u0, c.u1, c.v0, c.v1, c.thr) for c in self.cells]
@@ -916,7 +859,7 @@ class FastGrid:
         off = np.zeros(n + 1, np.int32)
         tot = lib().svs_fast_detect(self._h, arr, n, _ip(out), self.max_kp, _ip(off))
         if tot < 0:
-            self._err(tot)
+            self._ck(tot)
         return out[:min(tot, self.max_kp)].copy(), off
 
     def detect_adaptively(self, trials):
@@ -926,35 +869,19 @@ class FastGrid:
         tot = lib().svs_fast_detect_adaptively(self._h, C.byref(self.params), self.cells, int(trials), _ip(out),
                                                self.max_kp, _ip(off))
         if tot < 0:
-            self._err(tot)
+            self._ck(tot)
         return out[:min(tot, self.max_kp)].copy(), off
 
 
-class DenseTracker:
+class DenseTracker(_Handle):
     """Host-side mirror of DenseTracker / GpuTracker (reference dense_tracking.h:40-96,
     gpu/dense_tracking.cuh:276-342) on top of the C ABI."""
 
+    _destroy, _last_error = "svs_dt_destroy", "svs_dt_last_error"
+
     def __init__(self, w0, h0, nlevels=3, flags=0, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_dt_create(device, w0, h0, nlevels, flags, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_dt_create failed (no CUDA device? there is no CPU fallback)")
+        self._open("svs_dt_create", device, w0, h0, nlevels, flags)
         self.w0, self.h0, self.nlevels = w0, h0, nlevels
-
-    def close(self):
-        if self._h:
-            lib().svs_dt_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_dt_last_error(self._h).decode())
 
     @staticmethod
     def _fp(a):
@@ -1028,35 +955,18 @@ class DenseTracker:
                        launches=st.launches, ms_total=st.ms_total)
 
 
-class GuidedMatcher:
+class GuidedMatcher(_Handle):
     """Host-side mirror of GuidedMatcher<StereoCamera> (reference matcher.hpp:62-186)."""
+
+    _destroy, _last_error = "svs_matcher_destroy", "svs_matcher_last_error"
 
     def __init__(self, levels, max_keyframes=8, max_points=8192, max_keypoints=65536, device=-1):
         """levels: list of (w, h, f, px, py) per pyramid level (cam_vec)."""
-        self._h = C.c_void_p()
         arr = (SvsMatchLevel * len(levels))(*[SvsMatchLevel(int(w), int(h), float(f), float(px), float(py))
                                               for (w, h, f, px, py) in levels])
-        rc = lib().svs_matcher_create(device, len(levels), arr, max_keyframes, max_points, max_keypoints,
-                                      C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_matcher_create failed (no CUDA device? there is no CPU fallback)")
+        self._open("svs_matcher_create", device, len(levels), arr, max_keyframes, max_points, max_keypoints)
         self.nlevels = len(levels)
         self.max_points = max_points
-
-    def close(self):
-        if self._h:
-            lib().svs_matcher_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_matcher_last_error(self._h).decode())
 
     def _pyr_args(self, pyr):
         ims = [np.ascontiguousarray(p, np.uint8) for p in pyr]
@@ -1171,31 +1081,15 @@ def shall_we_drop_new_keyframe(stats, T_cur_from_actkey, params=None):
                                                  C.byref(p)))
 
 
-class FramePreprocessor:
+class FramePreprocessor(_Handle):
     """FrameGrabber::preprocessing (reference frame_grabber.cpp:287-336) on the device: uint8 and
     float pyramids and the x/y derivatives of one frame; outputs stay on the GPU."""
 
+    _destroy, _last_error = "svs_prep_destroy", "svs_prep_last_error"
+
     def __init__(self, w, h, nlevels=3, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_prep_create(device, w, h, nlevels, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_prep_create failed (no CUDA device? there is no CPU fallback)")
+        self._open("svs_prep_create", device, w, h, nlevels)
         self.nlevels = nlevels
-
-    def close(self):
-        if self._h:
-            lib().svs_prep_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_prep_last_error(self._h).decode())
 
     def process(self, img):
         img = np.ascontiguousarray(img, np.uint8)
@@ -1223,29 +1117,13 @@ class FramePreprocessor:
         return out
 
 
-class PoseOptimizer:
+class PoseOptimizer(_Handle):
     """BA_SE3_XYZ_STEREO (reference pose_optimizer.h:495): motion-only LM, whole loop in one kernel."""
 
+    _destroy, _last_error = "svs_pose_destroy", "svs_pose_last_error"
+
     def __init__(self, max_obs=16384, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_pose_create(device, max_obs, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_pose_create failed (no CUDA device? there is no CPU fallback)")
-
-    def close(self):
-        if self._h:
-            lib().svs_pose_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_pose_last_error(self._h).decode())
+        self._open("svs_pose_create", device, max_obs)
 
     @staticmethod
     def _params(robust_kernel, kernel_param, num_iter, initial_mu):
@@ -1334,31 +1212,15 @@ class PoseOptimizer:
         return T, self._stats(st)
 
 
-class DenseTrackerCpuVariant:
+class DenseTrackerCpuVariant(_Handle):
     """DenseTracker as the reference builds it without SCAVISLAM_CUDA_SUPPORT (dense_tracking.cpp:222-423):
     denseTrackingCpu / computeDensePointCloudCpu semantics, executed on the GPU."""
 
+    _destroy, _last_error = "svs_dtc_destroy", "svs_dtc_last_error"
+
     def __init__(self, w, h, nlevels=3, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_dtc_create(device, w, h, nlevels, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_dtc_create failed (no CUDA device, or a level size is not a multiple of 4)")
+        self._open("svs_dtc_create", device, w, h, nlevels, why="no CUDA device, or a level size is not a multiple of 4")
         self.w, self.h, self.nlevels = w, h, nlevels
-
-    def close(self):
-        if self._h:
-            lib().svs_dtc_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_dtc_last_error(self._h).decode())
 
     @staticmethod
     def _cams(cams):
@@ -1406,25 +1268,13 @@ class DenseTrackerCpuVariant:
         return T, dict(chi2=list(st.chi2[:self.nlevels]), passes=list(st.passes[:self.nlevels]), ms_total=st.ms_total)
 
 
-class ConstraintBuilder:
+class ConstraintBuilder(_Handle):
     """SlamGraph::computeConstraint (reference slam_graph.cpp:785-846) for a batch of pose pairs."""
 
+    _destroy, _last_error = "svs_constraints_destroy", "svs_constraints_last_error"
+
     def __init__(self, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_constraints_create(device, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_constraints_create failed (no CUDA device? there is no CPU fallback)")
-
-    def close(self):
-        if self._h:
-            lib().svs_constraints_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._open("svs_constraints_create", device)
 
     def compute(self, poses, feat_ptr, feat_point, point_anchor, xyz_anchor, v1, v2):
         """Returns (T_1_from_2[n,7], Lambda[n,6,6], visibility_strength[n])."""
@@ -1437,35 +1287,18 @@ class ConstraintBuilder:
         T, Lam, ns = np.zeros((n, 7)), np.zeros((n, 36)), np.zeros(n, np.int32)
         rc = lib().svs_computeConstraint_batch(self._h, len(poses), _dp(poses), _ip(fp), _ip(fpt), len(pa), _ip(pa), _dp(xyz),
                                                n, _ip(v1), _ip(v2), _dp(T), _dp(Lam), _ip(ns))
-        if rc != 0:
-            raise SvsError(rc, lib().svs_constraints_last_error(self._h).decode())
+        self._ck(rc)
         return T, Lam.reshape(n, 6, 6), ns
 
 
-class DeviceMap:
+class DeviceMap(_Handle):
     """The part of SlamGraph the optimiser reads, kept on the device (reference slam_graph.hpp:65-137), and
     copyDataToG2o (slam_graph.cpp:985-1032) as kernels feeding a BundleAdjuster."""
 
+    _destroy, _last_error = "svs_map_destroy", "svs_map_last_error"
+
     def __init__(self, device=-1):
-        self._h = C.c_void_p()
-        rc = lib().svs_map_create(device, C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_map_create failed (no CUDA device? there is no CPU fallback)")
-
-    def close(self):
-        if self._h:
-            lib().svs_map_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _ck(self, rc):
-        if rc != 0:
-            raise SvsError(rc, lib().svs_map_last_error(self._h).decode())
+        self._open("svs_map_create", device)
 
     def set(self, poses, point_anchor, xyz_anchor, vis_ptr, vis_pose, feat_center, feat_level):
         poses = np.ascontiguousarray(poses, np.float64).reshape(-1, 7)
@@ -1580,7 +1413,7 @@ class DeviceMap:
             out[f] = np.array(getattr(r, f)[:])
         out["lm"] = [PoseOptimizer._stats(r.lm[k]) for k in range(2)]
         if rc != 0:
-            err = SvsError(rc, lib().svs_map_last_error(self._h).decode())
+            err = self._error(rc)
             err.result = out
             raise err
         n = out["n_tracks"] if out["stage"] in (0, 3, 4) else 0
@@ -1609,7 +1442,7 @@ class DeviceMap:
             out[f] = np.array(getattr(r, f)[:])
         out["lm"] = [PoseOptimizer._stats(r.lm[k]) for k in range(2)]
         if rc != 0:
-            err = SvsError(rc, lib().svs_map_last_error(self._h).decode())
+            err = self._error(rc)
             err.result = out
             raise err
         gated = out["stage"] in (0, 4)
@@ -1627,33 +1460,22 @@ def load_surf_vocabulary(path):
     return np.ascontiguousarray(img).view(np.float32).copy()
 
 
-class PlaceRecognizer:
+class PlaceRecognizer(_Handle):
     """PlaceRecognizer::addLocation (reference placerecognizer.cpp:206-324) on the device: words, TF-IDF loop
     candidates, brute-force match and the RANSAC check.  Semantics: include/svs_b200.h (svs_place)."""
 
+    _destroy, _last_error = "svs_place_destroy", "svs_place_last_error"
+
     def __init__(self, words, cam, device=-1):
         words = np.ascontiguousarray(words, np.float32).reshape(-1, 64)
-        self._h = C.c_void_p()
-        rc = lib().svs_place_create(device, len(words), words.ctypes.data_as(C.POINTER(C.c_float)),
-                                    C.byref(SvsCam(*[float(x) for x in cam])), C.byref(self._h))
-        if rc != 0:
-            raise SvsError(rc, "svs_place_create failed (no CUDA device? there is no CPU fallback)")
+        self._open("svs_place_create", device, len(words), words.ctypes.data_as(C.POINTER(C.c_float)),
+                   C.byref(SvsCam(*[float(x) for x in cam])))
         self._last_n = 0
 
-    def close(self):
-        if self._h:
-            lib().svs_place_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def _ck(self, rc):
+        """Counts are results here: only a negative value is an error."""
         if rc < 0:
-            raise SvsError(rc, lib().svs_place_last_error(self._h).decode())
+            raise self._error(rc)
         return rc
 
     @property

@@ -26,7 +26,7 @@
 #include "ba_kernels.cuh"
 #include "ba_rules.cuh"
 #include "ba_structure.cuh"
-#include "grow.cuh"
+#include "handle.cuh"
 #include "nccl_dyn.cuh"
 #include "host_pool.hpp"
 #include "marginals.cuh"
@@ -87,11 +87,8 @@ struct Symbolic {
   int nblk = 0;
 };
 
-struct svs_ba {
-  int device = 0;
+struct svs_ba : svs::Handle {
   int flags = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
   bool has_problem = false;
   unsigned long long serial = 0;   // problem serial (svs::ba_problem_serial): a new value at the start of every set-up
   double* d_raw = nullptr; double* h_raw = nullptr; size_t raw_cap = 0;   // user-order observations + weights (6 doubles per edge)
@@ -165,15 +162,6 @@ struct CudaErr {
   cudaError_t e;
   const char* what;
 };
-
-#define CK(call)                                                        \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
 
 constexpr size_t kAlign = 256;
 
@@ -388,11 +376,6 @@ int choose_branches(int P, const std::vector<std::vector<int>>& adj, std::vector
   return 2;
 }
 
-int fail(svs_ba* h, int code, const std::string& msg) {
-  h->err = msg;
-  return code;
-}
-
 // Entry points that work on the problem on the device: SVS_ERR_INVALID for a null handle, SVS_ERR_STATE before
 // a successful set_problem.
 int need_problem(svs_ba* h) {
@@ -402,8 +385,8 @@ int need_problem(svs_ba* h) {
 
 // Reads the device's control block into h->h_ctl (waits for the stream).
 int read_ctl(svs_ba* h) {
-  CK(cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_ctl, h->d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -447,9 +430,12 @@ int svs_device_info(char* buf, int buflen) {
 int svs_ba_create(const svs_ba_opts* opts, svs_ba** out) {
   if (!out) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_ba* h = new svs_ba();
+  int dev = opts ? opts->device : -1;
+  if (int rc = open_handle(h, dev)) {
+    delete h;
+    return rc;
+  }
   h->flags = opts ? opts->flags : 0;
   {   // threads of the per-landmark host loops of set_problem: a few, never more than half the machine
     const int hw = (int)std::thread::hardware_concurrency();
@@ -457,11 +443,7 @@ int svs_ba_create(const svs_ba_opts* opts, svs_ba** out) {
   }
   if (const char* ht = getenv("SVS_HOST_THREADS")) h->host_threads = std::max(1, atoi(ht));
   h->pool.set_threads(h->host_threads);
-  int dev = opts ? opts->device : -1;
-  if (dev < 0) cudaGetDevice(&dev);
-  h->device = dev;
-  if (cudaSetDevice(dev) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaMallocHost(&h->h_ctl, sizeof(LmCtl)) != cudaSuccess) {
+  if (cudaMallocHost(&h->h_ctl, sizeof(LmCtl)) != cudaSuccess) {
     delete h;
     return SVS_ERR_CUDA;
   }
@@ -472,8 +454,7 @@ int svs_ba_create(const svs_ba_opts* opts, svs_ba** out) {
 
 void svs_ba_destroy(svs_ba* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  cudaStreamSynchronize(h->stream);
+  begin_close(h);
   free_problem(h);
   free_arena(h);
   if (h->comm) { if (const NcclApi* nc = nccl_api()) nc->CommDestroy(h->comm); }
@@ -486,23 +467,22 @@ void svs_ba_destroy(svs_ba* h) {
   for (auto& e : h->ev) cudaEventDestroy(e);
   for (auto& e : h->tev) cudaEventDestroy(e);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_last_error(const svs_ba* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_last_error(const svs_ba* h) { return last_error(h); }
 
 // The end of both set_problem paths: upload the staged bytes from `from` on, gather the observations into the
 // internal order, clear the counters (and, on a new structure, the debug block) and the constraint chi2, and reset
 // the state to the initial values.
 static int finish_problem(svs_ba* h, size_t from, const double* d_obs_info, bool clear_dbg) {
   BaDev& d = h->d;
-  CK(cudaMemcpyAsync(h->arena + from, h->stage + from, h->upload_bytes - from, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->arena + from, h->stage + from, h->upload_bytes - from, cudaMemcpyHostToDevice, h->stream));
   launch_regroup(d, d_obs_info ? d_obs_info : h->d_raw, h->stream);   // [3][E] internal order <- [E][3] user order
-  CK(cudaMemsetAsync(d.ticket, 0, 4 * sizeof(unsigned), h->stream));   // k_update's ticket, k_build_wave's task counter pair
-  if (clear_dbg) CK(cudaMemsetAsync(d.dbg, 0, 160 * sizeof(long long), h->stream));
-  CK(cudaMemsetAsync(d.chi_c, 0, std::max(d.C, 1) * sizeof(double), h->stream));
-  CK(cudaMemsetAsync(d.chi_c_new, 0, std::max(d.C, 1) * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.ticket, 0, 4 * sizeof(unsigned), h->stream));   // k_update's ticket, k_build_wave's task counter pair
+  if (clear_dbg) SVS_CK(h, cudaMemsetAsync(d.dbg, 0, 160 * sizeof(long long), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.chi_c, 0, std::max(d.C, 1) * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.chi_c_new, 0, std::max(d.C, 1) * sizeof(double), h->stream));
   return svs_ba_reset_state(h);
 }
 
@@ -626,8 +606,8 @@ static int lay_arena(svs_ba* h, const Symbolic& sy, const LaySrc& s) {
   h->measuring = true;
   lay(h, sy, s, &d_pose0c, &d_psi0c);
   h->measuring = false;
-  CK(grow(h->arena_off, &h->arena_cap, &h->arena));
-  CK(grow<char>(h->upload_bytes, &h->stage_cap, nullptr, &h->stage));
+  SVS_CK(h, grow(h->arena_off, &h->arena_cap, &h->arena));
+  SVS_CK(h, grow<char>(h->upload_bytes, &h->stage_cap, nullptr, &h->stage));
   lay(h, sy, s, &d_pose0c, &d_psi0c);
   h->d_pose0 = const_cast<double*>(d_pose0c);
   h->d_psi0 = const_cast<double*>(d_psi0c);
@@ -666,7 +646,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   cudaSetDevice(h->device);
   h->pool.begin();   // the host loops below run on a few spinning threads until this call returns
   struct PoolEnd { SpinPool* p; ~PoolEnd() { p->end(); } } pool_end{&h->pool};
-  CK(cudaStreamSynchronize(h->stream));   // the arena and the staging buffer are about to be reused
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the arena and the staging buffer are about to be reused
   const bool host_timing = getenv("SVS_HOST_TIMING") != nullptr;
   // ---- same structure as the problem on the device: only the numbers travel
   if (h->has_problem && !h->k_on_device && P == h->k_P && L == h->k_L && E == h->k_E && C == h->k_C &&
@@ -690,7 +670,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
             const size_t b0 = bytes * q / parts, b1 = bytes * (q + 1) / parts;
             memcpy(dst + b0, src + b0, b1 - b0);
           });
-          CK(cudaMemcpyAsync(reinterpret_cast<char*>(h->d_raw) + (half ? bytes : 0), dst, bytes, cudaMemcpyHostToDevice, h->stream));
+          SVS_CK(h, cudaMemcpyAsync(reinterpret_cast<char*>(h->d_raw) + (half ? bytes : 0), dst, bytes, cudaMemcpyHostToDevice, h->stream));
         }
       }
       if (C) {
@@ -722,7 +702,7 @@ static int set_problem_impl(svs_ba* h, int P, const double* T_qt, const unsigned
   //      pinned memory and enqueues the DMA (observations, then weights) while this thread analyses the structure; a
   //      gather kernel brings them into the internal order afterwards.  The helper also keeps the copy of the index
   //      arrays that the same-structure test of the next call compares against.
-  if (E > 0 && !d_obs_info) CK(grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
+  if (E > 0 && !d_obs_info) SVS_CK(h, grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
   struct Side {   // (every return below waits for the helper: it reads the caller's arrays)
     Worker* w;
     cudaError_t err = cudaSuccess;
@@ -1072,10 +1052,10 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
                            const double* c_Lambda, const svs_cam* cam, const double* d_obs_info) {
   h->serial = next_serial();
   cudaSetDevice(h->device);
-  CK(cudaStreamSynchronize(h->stream));   // the scratch and the staging buffer are about to be reused
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the scratch and the staging buffer are about to be reused
   const cudaStream_t st = h->stream;
   const bool host_timing = getenv("SVS_HOST_TIMING") != nullptr;
-  if (E > 0 && !d_obs_info) CK(grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
+  if (E > 0 && !d_obs_info) SVS_CK(h, grow(6 * (size_t)E, &h->raw_cap, &h->d_raw, &h->h_raw));
   int sms = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
   StructIn in{};
@@ -1090,12 +1070,12 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   in.k_epoint = keep; in.k_epose = keep + E; in.k_eanchor = keep + 2 * (size_t)E; in.k_ci = keep + 3 * (size_t)E;
   in.k_cj = keep + 3 * (size_t)E + C; in.k_fixed = reinterpret_cast<const unsigned char*>(keep + 3 * (size_t)E + 2 * (size_t)C);
   StructOut so{};
-  CK(grow(launch_structure(in, nullptr, &so, st), &h->scr_cap, &h->d_scr));
+  SVS_CK(h, grow(launch_structure(in, nullptr, &so, st), &h->scr_cap, &h->d_scr));
   launch_structure(in, h->d_scr, &so, st);
-  CK(grow<char>(so.readback_bytes, &h->rb_cap, nullptr, &h->h_rb));
-  CK(cudaMemcpyAsync(h->h_rb, so.hdr, so.readback_bytes, cudaMemcpyDeviceToHost, st));
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(st));
+  SVS_CK(h, grow<char>(so.readback_bytes, &h->rb_cap, nullptr, &h->h_rb));
+  SVS_CK(h, cudaMemcpyAsync(h->h_rb, so.hdr, so.readback_bytes, cudaMemcpyDeviceToHost, st));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(st));
   const StructHdr hd = *reinterpret_cast<const StructHdr*>(h->h_rb);
   BaDev& d = h->d;
   if (hd.err & kStructPairRange) return fail(h, SVS_ERR_INVALID, "pose-pose edge index out of range");
@@ -1137,10 +1117,10 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   d.f = cam->f; d.px = cam->px; d.py = cam->py; d.b = cam->b;
   d.ntasks = hd.ntasks; d.ngen = hd.ngen; d.nlong = hd.nlong;
   if (int rc = lay_arena(h, sy, LaySrc{})) return rc;   // every array but the symbolic ones comes from the device
-  CK(cudaMemcpyAsync(h->arena + h->off_sym, h->stage + h->off_sym, h->off_sym_end - h->off_sym, cudaMemcpyHostToDevice, st));
+  SVS_CK(h, cudaMemcpyAsync(h->arena + h->off_sym, h->stage + h->off_sym, h->off_sym_end - h->off_sym, cudaMemcpyHostToDevice, st));
   // the device's results into the arena, and this structure's index arrays into the copy the next call compares with
   const size_t keep_bytes = 4 * (3 * (size_t)E + 2 * (size_t)C) + P;
-  CK(grow(keep_bytes, &h->keep_cap, &h->d_keep));
+  SVS_CK(h, grow(keep_bytes, &h->keep_cap, &h->d_keep));
   int* kp = reinterpret_cast<int*>(h->d_keep);
   CopyList cl;
   auto I = [](const int* p) { return const_cast<int*>(p); };
@@ -1159,7 +1139,7 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   cl.add(so.fixed, kp + 3 * (size_t)E + 2 * (size_t)C, P);
   if (!d_obs_info) { cl.add(e_obs, h->d_raw, 24 * (size_t)E); cl.add(e_info, h->d_raw + 3 * (size_t)E, 24 * (size_t)E); }
   launch_copies(cl, st);
-  CK(cudaMemsetAsync(I(d.col_need), 0, sizeof(int) * (size_t)std::max(P, 1), st));
+  SVS_CK(h, cudaMemsetAsync(I(d.col_need), 0, sizeof(int) * (size_t)std::max(P, 1), st));
   launch_col_need(so, L, C, c_i, c_j, d.pos, I(d.col_need), st);
   adopt_structure(h, sy, hd.Kmax, hd.Kmax_gen, P, L, E, C);
   h->k_on_device = true;
@@ -1168,13 +1148,6 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   h->lm_to_user.clear();
   h->lm_user_stale = true;
   return finish_problem(h, h->upload_bytes, d_obs_info, true);
-}
-
-// true when p is device (or managed) memory of the handle's device
-static bool on_handle_device(const svs_ba* h, const void* p) {
-  cudaPointerAttributes a{};
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
 }
 
 int svs_ba_set_problem_device(svs_ba* h, int P, const double* T_qt, const unsigned char* fixed, int L, const double* psi,
@@ -1192,11 +1165,11 @@ int svs_ba_set_problem_device(svs_ba* h, int P, const double* T_qt, const unsign
                           C ? c_i : nullptr, C ? c_j : nullptr, C ? c_T : nullptr, C ? c_Lambda : nullptr};
   cudaSetDevice(h->device);
   for (const void* p : arrays)
-    if (p && !on_handle_device(h, p)) return fail(h, SVS_ERR_INVALID, "an array is not device memory of the handle's device");
+    if (p && !on_device(h->device, p)) return fail(h, SVS_ERR_INVALID, "an array is not device memory of the handle's device");
   h->L_full = 0;
   const int rc = set_problem_dev(h, P, T_qt, P ? fixed : nullptr, L, psi, E, e_point, e_pose, e_anchor, e_obs, e_info, C,
                                  c_i, c_j, c_T, c_Lambda, cam, nullptr);
-  if (rc == SVS_OK) CK(cudaStreamSynchronize(h->stream));   // the caller's arrays may be reused now
+  if (rc == SVS_OK) SVS_CK(h, cudaStreamSynchronize(h->stream));   // the caller's arrays may be reused now
   return rc;
 }
 
@@ -1204,23 +1177,23 @@ int svs_ba_reset_state(svs_ba* h) {
   if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   BaDev& d = h->d;
-  CK(cudaMemcpyAsync(d.pose[0], h->d_pose0, 7 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaMemcpyAsync(d.psi[0], h->d_psi0, 3 * (size_t)d.L * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.pose[0], h->d_pose0, 7 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.psi[0], h->d_psi0, 3 * (size_t)d.L * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
   LmCtl z{};
   *h->h_ctl = z;
   h->cur_known = 0;
-  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   launch_prep(d, 0, h->stream);
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 
 static int clear_system(svs_ba* h) {
   BaDev& d = h->d;
-  CK(cudaMemsetAsync(d.S, 0, 36 * (size_t)d.nblk * sizeof(double), h->stream));
-  CK(cudaMemsetAsync(d.bp, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
-  CK(cudaMemsetAsync(d.bc, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
-  CK(cudaMemsetAsync(d.col_done, 0, std::max(d.P, 1) * sizeof(int), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.S, 0, 36 * (size_t)d.nblk * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.bp, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.bc, 0, 6 * (size_t)std::max(d.P, 1) * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.col_done, 0, std::max(d.P, 1) * sizeof(int), h->stream));
   return SVS_OK;
 }
 
@@ -1243,12 +1216,12 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     LmCtl z{};
     z.cur = cur; z.lambda = lambda_init; z.ni = 2; z.max_trials = max_trials; z.max_iters = num_iters;
     *h->h_ctl = z;
-    CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   }
   if ((rc = clear_system(h))) return rc;
   float ms[4] = {0, 0, 0, 0};  // build, solve, update(+decision), collectives
   int launches = 0;
-  CK(cudaEventRecord(h->ev[0], h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev[0], h->stream));
   int it = 0;
   const NcclApi* nc = h->comm ? nccl_api() : nullptr;   // sharded window: sums across ranks on this stream
   if (h->comm && !nc) return fail(h, SVS_ERR_STATE, "NCCL library not loadable");
@@ -1281,30 +1254,30 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
       launch_update(d, robust, huber_delta, 0, h->stream, 1);
     }
     for (int k = 0; k < ntr && !chained; ++k) {
-      CK(cudaEventRecord(h->tev[kEv * k + 0], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 0], h->stream));
       launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
-      CK(cudaEventRecord(h->tev[kEv * k + 1], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 1], h->stream));
       // every rank holds the partial reduced system of its landmarks: ONE all-reduce of S | bp | bc
       if (nc) CKN(nc->AllReduce(d.S, d.S, h->sys_count, kNcclFloat64, kNcclSum, h->comm, h->stream));
-      CK(cudaEventRecord(h->tev[kEv * k + 2], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 2], h->stream));
       solve(h);
-      CK(cudaEventRecord(h->tev[kEv * k + 3], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 3], h->stream));
       launch_update(d, robust, huber_delta, nc ? 1 : 0, h->stream);
-      CK(cudaEventRecord(h->tev[kEv * k + 4], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 4], h->stream));
       if (nc) {   // chi2 (accepted, trial) and the gain-ratio denominator of this rank's landmarks -> the same decision everywhere
         CKN(nc->AllReduce(d.totals, d.totals, 3, kNcclFloat64, kNcclSum, h->comm, h->stream));
         launch_decide_deferred(d, h->stream);
       }
-      CK(cudaEventRecord(h->tev[kEv * k + 5], h->stream));
+      SVS_CK(h, cudaEventRecord(h->tev[kEv * k + 5], h->stream));
     }
-    CK(cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->h_ctl, d.ctl, sizeof(LmCtl), cudaMemcpyDeviceToHost, h->stream));
     if (h->export_next) {   // one-call API: the accepted state rides back with the control block, in the caller's order
       const size_t n = 7 * (size_t)d.P + 3 * (size_t)d.L;
       launch_export(d, h->d_out, h->stream);
-      CK(cudaMemcpyAsync(h->h_out, h->d_out, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(h->h_out, h->d_out, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     }
-    CK(cudaStreamSynchronize(h->stream));
-    CK(cudaGetLastError());
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaGetLastError());
     const int done_trials = h->h_ctl->trials_total - trials_seen;
     trials_seen = h->h_ctl->trials_total;
     launches += per_trial * done_trials;
@@ -1319,8 +1292,8 @@ static int optimize(svs_ba* h, int num_iters, int robust, double huber_delta, do
     it = h->h_ctl->iter;
     if (it >= num_iters || (h->h_ctl->stop && !h->h_ctl->again)) break;
   }
-  CK(cudaEventRecord(h->ev[1], h->stream));
-  CK(cudaEventSynchronize(h->ev[1]));
+  SVS_CK(h, cudaEventRecord(h->ev[1], h->stream));
+  SVS_CK(h, cudaEventSynchronize(h->ev[1]));
   h->cur_known = h->h_ctl->cur;   // read back after the last trial of this call
   if (st) {
     fill_stats(h, st);
@@ -1405,8 +1378,8 @@ int svs_ba_get_poses(svs_ba* h, double* T_qt) {
   cudaSetDevice(h->device);
   if (int rc = read_ctl(h)) return rc;
   if (h->d.P)
-    CK(cudaMemcpyAsync(T_qt, h->d.pose[h->h_ctl->cur], 7 * (size_t)h->d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpyAsync(T_qt, h->d.pose[h->h_ctl->cur], 7 * (size_t)h->d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -1416,12 +1389,12 @@ int svs_ba_get_points(svs_ba* h, double* psi) {
   if (int rc = read_ctl(h)) return rc;
   const int L = h->d.L;
   std::vector<double> tmp(3 * (size_t)L);
-  if (L) CK(cudaMemcpyAsync(tmp.data(), h->d.psi[h->h_ctl->cur],3 * (size_t)L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(tmp.data(), h->d.psi[h->h_ctl->cur],3 * (size_t)L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (h->lm_user_stale) {   // a device set-up left the landmark order on the device only
     h->lm_to_user.resize(L);
-    if (L) CK(cudaMemcpyAsync(h->lm_to_user.data(), h->d.lm_user, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    if (L) SVS_CK(h, cudaMemcpyAsync(h->lm_to_user.data(), h->d.lm_user, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   }
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->lm_user_stale = false;
   // a sharded window (svs_ba_set_problem_sharded) addresses the caller's full-size array: only this rank's entries are written
   const size_t mul = h->L_full ? (size_t)h->comm_size : 1, add = h->L_full ? (size_t)h->comm_rank : 0;
@@ -1464,10 +1437,10 @@ int svs_ba_chi2(svs_ba* h, int robust, double huber_delta, double* chi2) {
   BaDev& d = h->d;
   launch_chi2(d, robust, huber_delta, h->stream);
   std::vector<double> a(d.L), c(d.C);
-  if (d.L) CK(cudaMemcpyAsync(a.data(), d.chi_l, d.L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  if (d.C) CK(cudaMemcpyAsync(c.data(), d.chi_c, d.C * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaGetLastError());
+  if (d.L) SVS_CK(h, cudaMemcpyAsync(a.data(), d.chi_l, d.L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (d.C) SVS_CK(h, cudaMemcpyAsync(c.data(), d.chi_c, d.C * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
   double s = 0;
   for (double v : a) s += v;
   for (double v : c) s += v;
@@ -1479,7 +1452,7 @@ static int set_lambda(svs_ba* h, double lambda) {
   if (int rc = read_ctl(h)) return rc;
   h->h_ctl->lambda = lambda;
   h->h_ctl->max_iters = 0;   // inspection hooks run the kernels unconditionally
-  CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   return SVS_OK;
 }
 
@@ -1496,19 +1469,19 @@ int svs_ba_reduced_system(svs_ba* h, int robust, double huber_delta, double lamb
   std::vector<double> S(36 * (size_t)d.nblk), bp(n), bc(n), chl(d.L), chc(d.C);
   std::vector<int> colp(P + 1), rowi(d.nblk), perm(P);
   std::vector<unsigned char> fx(P);
-  CK(cudaMemcpyAsync(S.data(), d.S, S.size() * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(S.data(), d.S, S.size() * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if (P) {
-    CK(cudaMemcpyAsync(bp.data(), d.bp, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(bc.data(), d.bc, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(perm.data(), d.perm, P * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(fx.data(), d.fixed, P, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(bp.data(), d.bp, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(bc.data(), d.bc, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(perm.data(), d.perm, P * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(fx.data(), d.fixed, P, cudaMemcpyDeviceToHost, h->stream));
   }
-  CK(cudaMemcpyAsync(colp.data(), d.col_ptr, (P + 1) * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaMemcpyAsync(rowi.data(), d.row_idx, d.nblk * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (d.L) CK(cudaMemcpyAsync(chl.data(), d.chi_l, d.L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  if (d.C) CK(cudaMemcpyAsync(chc.data(), d.chi_c, d.C * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(colp.data(), d.col_ptr, (P + 1) * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(rowi.data(), d.row_idx, d.nblk * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (d.L) SVS_CK(h, cudaMemcpyAsync(chl.data(), d.chi_l, d.L * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (d.C) SVS_CK(h, cudaMemcpyAsync(chc.data(), d.chi_c, d.C * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
   if ((rc = clear_system(h))) return rc;
   std::fill(Sd, Sd + (size_t)n * n, 0.);
   for (int j = 0; j < P; ++j)
@@ -1541,9 +1514,9 @@ int svs_ba_solve_reduced(svs_ba* h, int robust, double huber_delta, double lambd
   if ((rc = clear_system(h))) return rc;
   launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
   solve(h);
-  if (d.P) CK(cudaMemcpyAsync(x, d.x, 6 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  if (d.P) SVS_CK(h, cudaMemcpyAsync(x, d.x, 6 * (size_t)d.P * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = read_ctl(h))) return rc;
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   const int failed = h->h_ctl->chol_fail;
   if ((rc = clear_system(h))) return rc;
   return failed ? 1 : 0;
@@ -1578,9 +1551,9 @@ int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, 
   if (!h->cov_tables) {
     h->cov_tbl.resize((size_t)P * P);
     h->cov_pos.resize(P);
-    CK(cudaMemcpyAsync(h->cov_tbl.data(), d.tbl, h->cov_tbl.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(h->cov_pos.data(), d.pos, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->cov_tbl.data(), d.tbl, h->cov_tbl.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->cov_pos.data(), d.pos, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
     h->cov_tables = true;
   }
   // the kernels run unconditionally at this lambda; the control block is put back as it was found at the end
@@ -1588,9 +1561,9 @@ int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, 
   const LmCtl saved = *h->h_ctl;
   h->h_ctl->lambda = lambda;
   h->h_ctl->max_iters = 0;
-  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   if ((rc = clear_system(h))) return rc;
-  CK(cudaEventRecord(h->ev[0], h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev[0], h->stream));
   launch_build(d, h->Kmax_gen, robust, huber_delta, h->stream);
   const int general = solve(h, 1) ? 1 : 0;
   // requests: the diagonal blocks, then (j, i) for pair k -- its column-major gather is Cov(x_i, x_j) row-major
@@ -1599,21 +1572,21 @@ int svs_ba_covariance(svs_ba* h, int robust, double huber_delta, double lambda, 
   for (int p = 0; p < ndiag; ++p) rq_r[p] = rq_c[p] = p;
   for (int k = 0; k < npairs; ++k) { rq_r[ndiag + k] = pair_j[k]; rq_c[ndiag + k] = pair_i[k]; }
   int in_pattern = 0, ncols = 0;
-  CK(invert(d, general, h->cov_tbl.data(), h->cov_pos.data(), n, rq_r.data(), rq_c.data(), &h->inv, h->stream, &in_pattern,
-            &ncols));
+  SVS_CK(h, invert(d, general, h->cov_tbl.data(), h->cov_pos.data(), n, rq_r.data(), rq_c.data(), &h->inv, h->stream, &in_pattern,
+                   &ncols));
   const size_t nb = 36 * (size_t)n, npt = point_cov ? 9 * (size_t)L : 0;
-  CK(grow(nb + npt, &h->cov_cap, &h->d_cov, &h->h_cov));
+  SVS_CK(h, grow(nb + npt, &h->cov_cap, &h->d_cov, &h->h_cov));
   if (npt) launch_point_cov(d, h->inv.zx, lambda, h->d_cov + nb, h->stream);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(h->ev[1], h->stream));
-  CK(gather(d, h->inv, h->d_cov, h->stream));
-  if (nb + npt) CK(cudaMemcpyAsync(h->h_cov, h->d_cov, (nb + npt) * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev[1], h->stream));
+  SVS_CK(h, gather(d, h->inv, h->d_cov, h->stream));
+  if (nb + npt) SVS_CK(h, cudaMemcpyAsync(h->h_cov, h->d_cov, (nb + npt) * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = read_ctl(h))) return rc;
   const int failed = h->h_ctl->chol_fail;
   if ((rc = clear_system(h))) return rc;
   *h->h_ctl = saved;
-  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   // fixed poses are not variables: every block that involves one is zero
   const double* hc = h->h_cov;
   auto put = [&](double* dst, const double* src, bool zero) {
@@ -1647,11 +1620,11 @@ static int window_grad(svs_ba* h, const char* name, int robust, double huber_del
   if (on_device)
     for (const void* p : {(const void*)dL_dpose, (const void*)dL_dpsi, (const void*)out.dL_dobs, (const void*)out.dL_dinfo,
                           (const void*)out.dL_dcT, (const void*)out.dL_dcLambda, (const void*)out.dL_dcam})
-      if (p && !on_handle_device(h, p)) return fail(h, SVS_ERR_INVALID, fn + "an array is not device memory of the handle's device");
+      if (p && !svs::on_device(h->device, p)) return fail(h, SVS_ERR_INVALID, fn + "an array is not device memory of the handle's device");
   if (P == 0) {   // no poses, hence no edges and no constraints: only the camera's zero gradient to write
     if (out.dL_dcam && on_device) {
-      CK(cudaMemsetAsync(out.dL_dcam, 0, 4 * sizeof(double), h->stream));
-      CK(cudaStreamSynchronize(h->stream));
+      SVS_CK(h, cudaMemsetAsync(out.dL_dcam, 0, 4 * sizeof(double), h->stream));
+      SVS_CK(h, cudaStreamSynchronize(h->stream));
     } else if (out.dL_dcam) {
       std::fill(out.dL_dcam, out.dL_dcam + 4, 0.);
     }
@@ -1672,10 +1645,10 @@ static int window_grad(svs_ba* h, const char* name, int robust, double huber_del
   double* go = out.dL_dobs; double* gw = out.dL_dinfo;
   double* gcT = out.dL_dcT; double* gcL = out.dL_dcLambda; double* gcam = out.dL_dcam;
   if (!on_device) {
-    CK(grow(o_part + n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
+    SVS_CK(h, grow(o_part + n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
     if (dL_dpose) memcpy(h->h_cov, dL_dpose, o_psi * sizeof(double));
     if (dL_dpsi) memcpy(h->h_cov + o_psi, dL_dpsi, 3 * (size_t)L * sizeof(double));
-    if (dL_dpose || dL_dpsi) CK(cudaMemcpyAsync(h->d_cov, h->h_cov, o_obs * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    if (dL_dpose || dL_dpsi) SVS_CK(h, cudaMemcpyAsync(h->d_cov, h->h_cov, o_obs * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     gp = dL_dpose ? h->d_cov : nullptr;
     gl = dL_dpsi ? h->d_cov + o_psi : nullptr;
     go = go ? h->d_cov + o_obs : nullptr;
@@ -1684,7 +1657,7 @@ static int window_grad(svs_ba* h, const char* name, int robust, double huber_del
     gcL = gcL ? h->d_cov + o_cLam : nullptr;
     gcam = gcam ? h->d_cov + o_cam : nullptr;
   } else if (n_part) {
-    CK(grow(n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
+    SVS_CK(h, grow(n_part, &h->cov_cap, &h->d_cov, &h->h_cov));
   }
   double* part = n_part ? h->d_cov + o_part : nullptr;
   // the kernels run unconditionally at this lambda; the control block is put back as it was found at the end
@@ -1692,21 +1665,21 @@ static int window_grad(svs_ba* h, const char* name, int robust, double huber_del
   const LmCtl saved = *h->h_ctl;
   h->h_ctl->lambda = lambda;
   h->h_ctl->max_iters = 0;
-  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   if ((rc = clear_system(h))) return rc;
-  CK(cudaEventRecord(h->ev[0], h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev[0], h->stream));
   // H is the Hessian of the cost: never the self-anchor term of SURVEY.md B5, whatever the handle's flags
   BaDev db = d;
   db.flags |= SVS_BA_SKIP_SELF_ANCHOR_HESSIAN;
   launch_build(db, h->Kmax_gen, robust, huber_delta, h->stream);
   // the build summed its own right-hand side into bp / bc: k_grad_rhs overwrites bp and accumulates into bc
-  CK(cudaMemsetAsync(d.bc, 0, 6 * (size_t)P * sizeof(double), h->stream));
+  SVS_CK(h, cudaMemsetAsync(d.bc, 0, 6 * (size_t)P * sizeof(double), h->stream));
   launch_grad_rhs(d, gp, gl, lambda, h->stream);
   const int general = solve(h) ? 1 : 0;
   launch_grad_edges(d, gl, lambda, robust, huber_delta, go, gw, part, gcam, h->stream);
   launch_grad_constraints(d, gcT, gcL, h->stream);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(h->ev[1], h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev[1], h->stream));
   // host arrays: each requested output comes back from its place in the scratch
   struct Back { const double* dst; size_t off, n; };
   const Back back[] = {{out.dL_dobs, o_obs, 3 * (size_t)E}, {out.dL_dinfo, o_info, 3 * (size_t)E},
@@ -1714,13 +1687,13 @@ static int window_grad(svs_ba* h, const char* name, int robust, double huber_del
   if (!on_device)
     for (const Back& k : back)
       if (k.dst && k.n)
-        CK(cudaMemcpyAsync(h->h_cov + k.off, h->d_cov + k.off, k.n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+        SVS_CK(h, cudaMemcpyAsync(h->h_cov + k.off, h->d_cov + k.off, k.n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   if ((rc = read_ctl(h))) return rc;
   const int failed = h->h_ctl->chol_fail;
   if ((rc = clear_system(h))) return rc;
   *h->h_ctl = saved;
-  CK(cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (!on_device)
     for (const Back& k : back)
       if (k.dst && k.n) memcpy(const_cast<double*>(k.dst), h->h_cov + k.off, k.n * sizeof(double));
@@ -1860,12 +1833,12 @@ int svs_ba_get_points_all(svs_ba* h, double* psi) {
   if (!h->comm || h->comm_size == 1) return SVS_OK;
   const NcclApi* nc = nccl_api();
   if (!nc) return fail(h, SVS_ERR_STATE, "NCCL library not loadable");
-  CK(grow(n, &h->psi_all_cap, &h->d_psi_all));
-  CK(cudaMemcpyAsync(h->d_psi_all, psi, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, grow(n, &h->psi_all_cap, &h->d_psi_all));
+  SVS_CK(h, cudaMemcpyAsync(h->d_psi_all, psi, n * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   if (nc->AllReduce(h->d_psi_all, h->d_psi_all, n, kNcclFloat64, kNcclSum, h->comm, h->stream) != 0)
     return fail(h, SVS_ERR_CUDA, "ncclAllReduce failed");
-  CK(cudaMemcpyAsync(psi, h->d_psi_all, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(psi, h->d_psi_all, n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -1890,7 +1863,7 @@ int svs_ba_lm_begin(svs_ba* h, double lambda_init, int max_trials) {
   LmCtl z{};
   z.cur = cur; z.lambda = lambda_init; z.ni = 2; z.max_trials = max_trials;
   *h->h_ctl = z;
-  CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   return clear_system(h);
 }
 
@@ -1898,8 +1871,8 @@ int svs_ba_trial_build(svs_ba* h, int robust, double huber_delta) {
   if (int rc = need_problem(h)) return rc;
   cudaSetDevice(h->device);
   launch_build(h->d, h->Kmax_gen, robust, huber_delta, h->stream);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(h->stream));   // the caller's collective runs on its own stream
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the caller's collective runs on its own stream
   return SVS_OK;
 }
 
@@ -1920,8 +1893,8 @@ int svs_ba_trial_solve(svs_ba* h, int robust, double huber_delta) {
   cudaSetDevice(h->device);
   solve(h);
   launch_update(h->d, robust, huber_delta, 1, h->stream);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -1931,7 +1904,7 @@ int svs_ba_trial_decide(svs_ba* h, int* again, int* stop, int* iter) {
   launch_decide_deferred(h->d, h->stream);
   if (int rc = read_ctl(h)) return rc;
   h->cur_known = h->h_ctl->cur;
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   if (again) *again = h->h_ctl->again;
   if (stop) *stop = h->h_ctl->stop;
   if (iter) *iter = h->h_ctl->iter;
@@ -1974,9 +1947,9 @@ int ba_solve_system(svs_ba* h, int* general, int keep_diag) {
   LmCtl z{};   // lambda = 0, max_iters = 0: the solve runs unconditionally and adds nothing to the diagonal
   z.cur = h->cur_known;
   *h->h_ctl = z;
-  CK(cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d.ctl, h->h_ctl, sizeof(LmCtl), cudaMemcpyHostToDevice, h->stream));
   *general = solve(h, keep_diag) ? 1 : 0;
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 void ba_forget_symbolic(svs_ba* h) {

@@ -18,7 +18,7 @@
 
 #include "../../include/svs_b200.h"
 #include "ba_types.cuh"
-#include "grow.cuh"
+#include "handle.cuh"
 #include "internal.cuh"
 #include "marginals.cuh"
 
@@ -55,9 +55,7 @@ __global__ void k_chol6_scatter(int P, int nnzb, const int2* __restrict__ rc, co
 
 }  // namespace
 
-struct svs_chol6 {
-  int device = 0;
-  std::string err;
+struct svs_chol6 : svs::Handle {
   svs_ba* ba = nullptr;
   // pattern of the problem on the internal BA handle (P < 0: none)
   int P = -1;
@@ -74,20 +72,6 @@ struct svs_chol6 {
 };
 
 namespace {
-
-int fail(svs_chol6* h, int code, const std::string& msg) {
-  h->err = msg;
-  return code;
-}
-
-#define CK(call)                                                        \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
 
 // The checks of the header comment, before anything is enqueued.  `ptrs` are the entry point's array arguments
 // besides the pattern (named `what` in the messages): never null, and on the handle's device when on_device != 0.
@@ -117,14 +101,9 @@ int validate(svs_chol6* h, const char* fn, int P, const int* col_ptr, const int*
       return fail(h, SVS_ERR_INVALID, f + "column " + std::to_string(j) + " has no diagonal block");
   }
   if (on_device) {
-    for (const void* p : ptrs) {
-      cudaPointerAttributes a{};
-      if (cudaPointerGetAttributes(&a, p) != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) ||
-          a.device != h->device) {
-        cudaGetLastError();
+    for (const void* p : ptrs)
+      if (!svs::on_device(h->device, p))
         return fail(h, SVS_ERR_INVALID, f + "on_device = 1 but " + what + " is not memory of the handle's device");
-      }
-    }
   }
   return SVS_OK;
 }
@@ -149,15 +128,15 @@ int set_pattern(svs_chol6* h, const char* fn, int P, const int* col_ptr, const i
                              nullptr, nullptr, nullptr, nullptr, &cam);
   }
   if (rc_ != SVS_OK) return fail(h, rc_, std::string(fn) + ": " + svs_last_error(h->ba));
-  CK(grow((size_t)nnzb, &h->rc_cap, &h->d_rc));
+  SVS_CK(h, grow((size_t)nnzb, &h->rc_cap, &h->d_rc));
   const BaDev* d = nullptr; cudaStream_t st = nullptr; int hits = 0;
   if ((rc_ = ba_system_on_device(h->ba, &d, &st, &hits))) return fail(h, rc_, std::string(fn) + ": no problem on the internal handle");
-  CK(cudaMemcpyAsync(h->d_rc, rc.data(), (size_t)nnzb * sizeof(int2), cudaMemcpyHostToDevice, st));
+  SVS_CK(h, cudaMemcpyAsync(h->d_rc, rc.data(), (size_t)nnzb * sizeof(int2), cudaMemcpyHostToDevice, st));
   h->tbl.resize((size_t)P * P);
   h->pos.resize(P);
-  CK(cudaMemcpyAsync(h->tbl.data(), d->tbl, h->tbl.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h->pos.data(), d->pos, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));   // rc is a pageable temporary
+  SVS_CK(h, cudaMemcpyAsync(h->tbl.data(), d->tbl, h->tbl.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+  SVS_CK(h, cudaMemcpyAsync(h->pos.data(), d->pos, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, st));
+  SVS_CK(h, cudaStreamSynchronize(st));   // rc is a pageable temporary
   h->P = P;
   h->col_ptr.assign(col_ptr, col_ptr + P + 1);
   h->row_idx.assign(row_idx, row_idx + nnzb);
@@ -196,23 +175,23 @@ int factor(svs_chol6* h, const char* fn, int P, const int* col_ptr, const int* r
   const double* d_blocks = blocks;
   const double* d_b = b;
   if (!on_device) {   // staged in pinned memory, one copy
-    CK(grow(nA + n, &h->in_cap, &h->d_in, &h->h_in));
+    SVS_CK(h, grow(nA + n, &h->in_cap, &h->d_in, &h->h_in));
     memcpy(h->h_in, blocks, nA * sizeof(double));
     if (b) memcpy(h->h_in + nA, b, n * sizeof(double));
     else memset(h->h_in + nA, 0, n * sizeof(double));
-    CK(cudaMemcpyAsync(h->d_in, h->h_in, (nA + n) * sizeof(double), cudaMemcpyHostToDevice, st));
+    SVS_CK(h, cudaMemcpyAsync(h->d_in, h->h_in, (nA + n) * sizeof(double), cudaMemcpyHostToDevice, st));
     d_blocks = h->d_in;
     d_b = h->d_in + nA;
   } else if (!b) {
-    CK(grow(n, &h->in_cap, &h->d_in, &h->h_in));
-    CK(cudaMemsetAsync(h->d_in, 0, n * sizeof(double), st));
+    SVS_CK(h, grow(n, &h->in_cap, &h->d_in, &h->h_in));
+    SVS_CK(h, cudaMemsetAsync(h->d_in, 0, n * sizeof(double), st));
     d_b = h->d_in;
   }
-  CK(cudaEventRecord(h->ev[0], st));
-  CK(cudaMemsetAsync(d->S, 0, 36 * (size_t)d->nblk * sizeof(double), st));   // the fill-in blocks start from zero
+  SVS_CK(h, cudaEventRecord(h->ev[0], st));
+  SVS_CK(h, cudaMemsetAsync(d->S, 0, 36 * (size_t)d->nblk * sizeof(double), st));   // the fill-in blocks start from zero
   const long long work = (long long)nA + (long long)n;
   k_chol6_scatter<<<(unsigned)((work + 255) / 256), 256, 0, st>>>(P, nnzb, h->d_rc, d_blocks, d_b, d->tbl, d->S, d->bp, d->bc);
-  CK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   if (int rc = ba_solve_system(h->ba, &f->general, keep_diag)) return fail(h, rc, std::string(fn) + ": " + svs_last_error(h->ba));
   return SVS_OK;
 }
@@ -226,18 +205,18 @@ int invert(svs_chol6* h, const char* fn, int P, const int* col_ptr, const int* r
   const BaDev* d = f.d;
   const cudaStream_t st = f.st;
   int in_pattern = 0, ncols = 0;
-  CK(svs::invert(*d, f.general, h->tbl.data(), h->pos.data(), n, req_r, req_c, &h->inv, st, &in_pattern, &ncols));
-  CK(cudaEventRecord(h->ev[1], st));
+  SVS_CK(h, svs::invert(*d, f.general, h->tbl.data(), h->pos.data(), n, req_r, req_c, &h->inv, st, &in_pattern, &ncols));
+  SVS_CK(h, cudaEventRecord(h->ev[1], st));
   double* d_out = out;
   const size_t nout = 36 * (size_t)n;
   if (!on_device) {
-    CK(grow(nout, &h->out_cap, &h->d_out, &h->h_out));
+    SVS_CK(h, grow(nout, &h->out_cap, &h->d_out, &h->h_out));
     d_out = h->d_out;
   }
-  CK(gather(*d, h->inv, d_out, st));
-  CK(cudaMemcpyAsync(h->h_fail, &d->ctl->chol_fail, sizeof(int), cudaMemcpyDeviceToHost, st));
-  if (!on_device) CK(cudaMemcpyAsync(h->h_out, d_out, nout * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  SVS_CK(h, gather(*d, h->inv, d_out, st));
+  SVS_CK(h, cudaMemcpyAsync(h->h_fail, &d->ctl->chol_fail, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (!on_device) SVS_CK(h, cudaMemcpyAsync(h->h_out, d_out, nout * sizeof(double), cudaMemcpyDeviceToHost, st));
+  SVS_CK(h, cudaStreamSynchronize(st));
   if (!on_device) memcpy(out, h->h_out, nout * sizeof(double));
   if (stats) {
     stats->P = P; stats->nnzb_A = col_ptr[P]; stats->nnzb_L = d->nblk; stats->nbranch = d->nbranch;
@@ -255,17 +234,15 @@ extern "C" {
 int svs_chol6_create(int device, svs_chol6** out) {
   if (!out) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
-  if (device < 0) cudaGetDevice(&device);
-  if (device >= n) return SVS_ERR_INVALID;
-  svs_ba_opts o{device, 0, {0, 0, 0, 0, 0, 0}};
-  svs_ba* ba = nullptr;
-  if (int rc = svs_ba_create(&o, &ba)) return rc;
   svs_chol6* h = new svs_chol6();
-  h->device = device;
-  h->ba = ba;
-  if (cudaSetDevice(device) != cudaSuccess || cudaMallocHost(&h->h_fail, sizeof(int)) != cudaSuccess ||
+  int rc = open_handle(h, device, false);
+  const svs_ba_opts o{device, 0, {0, 0, 0, 0, 0, 0}};
+  if (rc == SVS_OK) rc = svs_ba_create(&o, &h->ba);
+  if (rc != SVS_OK) {
+    delete h;
+    return rc;
+  }
+  if (cudaMallocHost(&h->h_fail, sizeof(int)) != cudaSuccess ||
       cudaEventCreate(&h->ev[0]) != cudaSuccess || cudaEventCreate(&h->ev[1]) != cudaSuccess) {
     svs_chol6_destroy(h);
     return SVS_ERR_CUDA;
@@ -276,7 +253,7 @@ int svs_chol6_create(int device, svs_chol6** out) {
 
 void svs_chol6_destroy(svs_chol6* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
+  begin_close(h);
   if (h->ba) svs_ba_destroy(h->ba);   // waits for the stream
   if (h->d_rc) cudaFree(h->d_rc);
   if (h->d_in) cudaFree(h->d_in);
@@ -291,7 +268,7 @@ void svs_chol6_destroy(svs_chol6* h) {
   delete h;
 }
 
-const char* svs_chol6_last_error(const svs_chol6* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_chol6_last_error(const svs_chol6* h) { return last_error(h); }
 
 int svs_chol6_init(svs_chol6* h) {
   if (!h) return SVS_ERR_INVALID;
@@ -312,15 +289,15 @@ int svs_chol6_solve(svs_chol6* h, int P, const int* col_ptr, const int* row_idx,
   Factor f;
   if (int rc = factor(h, fn, P, col_ptr, row_idx, blocks, b, on_device, 0, &f)) return rc;
   const size_t n = 6 * (size_t)P;
-  CK(cudaEventRecord(h->ev[1], f.st));
-  CK(cudaMemcpyAsync(h->h_fail, &f.d->ctl->chol_fail, sizeof(int), cudaMemcpyDeviceToHost, f.st));
+  SVS_CK(h, cudaEventRecord(h->ev[1], f.st));
+  SVS_CK(h, cudaMemcpyAsync(h->h_fail, &f.d->ctl->chol_fail, sizeof(int), cudaMemcpyDeviceToHost, f.st));
   if (on_device) {
-    CK(cudaMemcpyAsync(x, f.d->x, n * sizeof(double), cudaMemcpyDeviceToDevice, f.st));
+    SVS_CK(h, cudaMemcpyAsync(x, f.d->x, n * sizeof(double), cudaMemcpyDeviceToDevice, f.st));
   } else {
-    CK(grow(n, &h->x_cap, (double**)nullptr, &h->h_x));
-    CK(cudaMemcpyAsync(h->h_x, f.d->x, n * sizeof(double), cudaMemcpyDeviceToHost, f.st));
+    SVS_CK(h, grow(n, &h->x_cap, (double**)nullptr, &h->h_x));
+    SVS_CK(h, cudaMemcpyAsync(h->h_x, f.d->x, n * sizeof(double), cudaMemcpyDeviceToHost, f.st));
   }
-  CK(cudaStreamSynchronize(f.st));
+  SVS_CK(h, cudaStreamSynchronize(f.st));
   if (!on_device) memcpy(x, h->h_x, n * sizeof(double));
   if (stats) {
     stats->P = P; stats->nnzb_A = col_ptr[P]; stats->nnzb_L = f.d->nblk; stats->nbranch = f.d->nbranch;

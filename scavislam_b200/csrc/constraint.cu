@@ -15,6 +15,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "se3_dev.cuh"
 
 namespace {
@@ -107,36 +108,20 @@ __global__ void __launch_bounds__(kThreads) k_compute_constraint(CArgs a) {
 
 }  // namespace
 
-struct svs_constraints {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_constraints : svs::Handle {
   size_t cap_bytes = 0;
   char* d_buf = nullptr;
 };
-
-#define KCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
 
 extern "C" {
 
 int svs_constraints_create(int device, svs_constraints** out) {
   if (!out) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_constraints* h = new svs_constraints();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device;
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
+  if (int rc = svs::open_handle(h, device)) {
     delete h;
-    return SVS_ERR_CUDA;
+    return rc;
   }
   *out = h;
   return SVS_OK;
@@ -144,14 +129,12 @@ int svs_constraints_create(int device, svs_constraints** out) {
 
 void svs_constraints_destroy(svs_constraints* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   cudaFree(h->d_buf);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_constraints_last_error(const svs_constraints* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_constraints_last_error(const svs_constraints* h) { return svs::last_error(h); }
 
 int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_from_world, const int* feat_ptr,
                                 const int* feat_point, int L, const int* point_anchor, const double* xyz_anchor, int npairs,
@@ -191,21 +174,19 @@ int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_fr
   const size_t o_n = off; off += al(sizeof(int) * (size_t)npairs);
   const size_t o_s = off; off += al(sizeof(double) * (size_t)scratch_stride * (size_t)npairs);
   if (off > h->cap_bytes) {
-    KCK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_buf); h->d_buf = nullptr; h->cap_bytes = 0;
-    KCK(cudaMalloc(&h->d_buf, off));
-    h->cap_bytes = off;
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
+    SVS_CK(h, svs::grow(off, &h->cap_bytes, &h->d_buf));
   }
   char* B = h->d_buf;
-  KCK(cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)P, cudaMemcpyHostToDevice, h->stream));
-  KCK(cudaMemcpyAsync(B + o_fptr, feat_ptr, sizeof(int) * ((size_t)P + 1), cudaMemcpyHostToDevice, h->stream));
-  if (nfeat) KCK(cudaMemcpyAsync(B + o_fpt, feat_point, sizeof(int) * (size_t)nfeat, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_fptr, feat_ptr, sizeof(int) * ((size_t)P + 1), cudaMemcpyHostToDevice, h->stream));
+  if (nfeat) SVS_CK(h, cudaMemcpyAsync(B + o_fpt, feat_point, sizeof(int) * (size_t)nfeat, cudaMemcpyHostToDevice, h->stream));
   if (L) {
-    KCK(cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
-    KCK(cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)L, cudaMemcpyHostToDevice, h->stream));
   }
-  KCK(cudaMemcpyAsync(B + o_v1, v1, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
-  KCK(cudaMemcpyAsync(B + o_v2, v2, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_v1, v1, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_v2, v2, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
   CArgs a;
   a.poses = reinterpret_cast<const double*>(B + o_pose);
   a.feat_ptr = reinterpret_cast<const int*>(B + o_fptr); a.feat_point = reinterpret_cast<const int*>(B + o_fpt);
@@ -215,12 +196,12 @@ int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_fr
   a.strength = reinterpret_cast<int*>(B + o_n);
   a.scratch = reinterpret_cast<double*>(B + o_s); a.scratch_stride = scratch_stride;
   k_compute_constraint<<<npairs, kThreads, 0, h->stream>>>(a);
-  KCK(cudaGetLastError());
-  KCK(cudaMemcpyAsync(T_1_from_2, a.T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
-  KCK(cudaMemcpyAsync(Lambda, a.Lambda, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(T_1_from_2, a.T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(Lambda, a.Lambda, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
   if (visibility_strength)
-    KCK(cudaMemcpyAsync(visibility_strength, a.strength, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
-  KCK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpyAsync(visibility_strength, a.strength, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 

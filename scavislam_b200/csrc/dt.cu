@@ -26,6 +26,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "se3_dev.cuh"
 #include "svs_nvtx.hpp"
 
@@ -536,10 +537,7 @@ __global__ void k_dt_pointcloud(M4 TQ, const float* __restrict__ disp, int width
 
 }  // namespace
 
-struct svs_dt {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_dt : svs::Handle {
   int nlevels = 0, w0 = 0, h0 = 0, flags = 0;
   DtLevel lv[kMaxLevels];
   float* img[kMaxLevels][4] = {};   // prev cur dx dy
@@ -558,26 +556,18 @@ struct svs_dt {
   size_t stage_floats = 0;
 };
 
-#define DCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 extern "C" {
 
 int svs_dt_create(int device, int w0, int h0, int nlevels, int flags, svs_dt** out) {
   if (!out || w0 <= 0 || h0 <= 0 || nlevels <= 0 || nlevels > kMaxLevels) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_dt* h = new svs_dt();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device; h->nlevels = nlevels; h->w0 = w0; h->h0 = h0; h->flags = flags;
-  bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
+  h->nlevels = nlevels; h->w0 = w0; h->h0 = h0; h->flags = flags;
+  bool ok = true;
   for (int l = 0; ok && l < nlevels; ++l) {
     const int w = w0 >> l, hh = h0 >> l;
     DtLevel& L = h->lv[l];
@@ -621,8 +611,7 @@ int svs_dt_create(int device, int w0, int h0, int nlevels, int flags, svs_dt** o
 
 void svs_dt_destroy(svs_dt* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   for (int l = 0; l < kMaxLevels; ++l) {
     for (int k = 0; k < 4; ++k) cudaFree(h->img[l][k]);
     cudaFree(h->cloud[l]);
@@ -632,11 +621,10 @@ void svs_dt_destroy(svs_dt* h) {
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
   if (h->stage) cudaFreeHost(h->stage);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_dt_last_error(const svs_dt* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_dt_last_error(const svs_dt* h) { return svs::last_error(h); }
 
 int svs_dt_set_intrinsics(svs_dt* h, int level, float focal_length, float px, float py) {
   if (!h || level < 0 || level >= h->nlevels) return SVS_ERR_INVALID;
@@ -645,8 +633,8 @@ int svs_dt_set_intrinsics(svs_dt* h, int level, float focal_length, float px, fl
 }
 
 static int upload_plane(svs_dt* h, float* dst, int dst_stride, const float* src, int src_stride, int w, int hgt) {
-  DCK(cudaMemcpy2DAsync(dst, sizeof(float) * dst_stride, src, sizeof(float) * src_stride, sizeof(float) * w, hgt,
-                        cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(dst, sizeof(float) * dst_stride, src, sizeof(float) * src_stride, sizeof(float) * w, hgt,
+                              cudaMemcpyHostToDevice, h->stream));
   return SVS_OK;
 }
 
@@ -673,8 +661,8 @@ int svs_dt_set_images_device(svs_dt* h, int level, const float* prev, const floa
   const float* src[4] = {prev, cur, dx, dy};
   for (int k = 0; k < 4; ++k)
     if (src[k])
-      DCK(cudaMemcpy2DAsync(h->img[level][k], sizeof(float) * L.stride, src[k], sizeof(float) * stride_floats,
-                            sizeof(float) * L.w, L.h, cudaMemcpyDeviceToDevice, h->stream));
+      SVS_CK(h, cudaMemcpy2DAsync(h->img[level][k], sizeof(float) * L.stride, src[k], sizeof(float) * stride_floats,
+                                  sizeof(float) * L.w, L.h, cudaMemcpyDeviceToDevice, h->stream));
   return SVS_OK;
 }
 
@@ -699,8 +687,8 @@ int svs_dt_set_point_cloud(svs_dt* h, int level, const float* cloud_xyzw) {
   if (!h || level < 0 || level >= h->nlevels || !cloud_xyzw) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   const DtLevel& L = h->lv[level];
-  DCK(cudaMemcpy2DAsync(h->cloud[level], sizeof(float4) * L.cloud_stride, cloud_xyzw, sizeof(float4) * L.w,
-                        sizeof(float4) * L.w, L.h, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(h->cloud[level], sizeof(float4) * L.cloud_stride, cloud_xyzw, sizeof(float4) * L.w,
+                              sizeof(float4) * L.w, L.h, cudaMemcpyHostToDevice, h->stream));
   return SVS_OK;
 }
 
@@ -708,9 +696,9 @@ int svs_dt_get_point_cloud(svs_dt* h, int level, float* cloud_xyzw) {
   if (!h || level < 0 || level >= h->nlevels || !cloud_xyzw) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   const DtLevel& L = h->lv[level];
-  DCK(cudaMemcpy2DAsync(cloud_xyzw, sizeof(float4) * L.w, h->cloud[level], sizeof(float4) * L.cloud_stride,
-                        sizeof(float4) * L.w, L.h, cudaMemcpyDeviceToHost, h->stream));
-  DCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(cloud_xyzw, sizeof(float4) * L.w, h->cloud[level], sizeof(float4) * L.cloud_stride,
+                              sizeof(float4) * L.w, L.h, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -746,7 +734,7 @@ int svs_dt_compute_point_cloud(svs_dt* h, const double T_cur_from_actkey[7], con
     const dim3 blk(32, 8), grd((L.w + 31) / 32, (L.h + 7) / 8);
     k_dt_pointcloud<<<grd, blk, 0, h->stream>>>(TQ, h->disp, L.w, L.h, h->disp_stride, L.cloud_stride, 1 << l, h->cloud[l]);
   }
-  DCK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 
@@ -755,12 +743,12 @@ static int run_pass(svs_dt* h, int level, const double T[7], int want_jac, doubl
   cudaSetDevice(h->device);
   const DtLevel& L = h->lv[level];
   const int blocks = std::min(h->max_blocks, std::max(1, (L.w * L.h + kThreads - 1) / kThreads));
-  DCK(cudaMemcpyAsync(h->d_T, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_T, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
   k_dt_pass<<<blocks, kThreads, 0, h->stream>>>(L, h->d_T, h->d_partial, (h->flags & SVS_DT_EXACT_BILINEAR) ? 1 : 0, want_jac);
   std::vector<double> part((size_t)blocks * kAcc);
-  DCK(cudaMemcpyAsync(part.data(), h->d_partial, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, h->stream));
-  DCK(cudaStreamSynchronize(h->stream));
-  DCK(cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(part.data(), h->d_partial, sizeof(double) * part.size(), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
   for (int i = 0; i < kAcc; ++i) {
     double s = 0;
     for (int b = 0; b < blocks; ++b) s += part[(size_t)b * kAcc + i];
@@ -791,13 +779,13 @@ int svs_dt_residual_image(svs_dt* h, int level, const double T[7], float* res_rg
   if (!h || level < 0 || level >= h->nlevels || !T || !res_rgba) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   const DtLevel& L = h->lv[level];
-  if (!h->d_res) DCK(cudaMalloc(&h->d_res, sizeof(float4) * (size_t)h->w0 * h->h0));
-  DCK(cudaMemcpyAsync(h->d_T, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+  if (!h->d_res) SVS_CK(h, cudaMalloc(&h->d_res, sizeof(float4) * (size_t)h->w0 * h->h0));
+  SVS_CK(h, cudaMemcpyAsync(h->d_T, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
   const dim3 block(32, 8), grid((L.w + 31) / 32, (L.h + 7) / 8);
   k_dt_residual_image<<<grid, block, 0, h->stream>>>(L, h->d_T, (h->flags & SVS_DT_EXACT_BILINEAR) ? 1 : 0, h->d_res);
-  DCK(cudaMemcpyAsync(res_rgba, h->d_res, sizeof(float4) * (size_t)L.w * L.h, cudaMemcpyDeviceToHost, h->stream));
-  DCK(cudaStreamSynchronize(h->stream));
-  DCK(cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(res_rgba, h->d_res, sizeof(float4) * (size_t)L.w * L.h, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 
@@ -805,7 +793,7 @@ int svs_dt_track(svs_dt* h, double T[7], svs_dt_stats* st) {
   svs::NvtxRange nvtx_("dense tracking");
   if (!h || !T) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  DCK(cudaMemcpyAsync(h->d_ctl, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));   // DtCtl::T is first
+  SVS_CK(h, cudaMemcpyAsync(h->d_ctl, T, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));   // DtCtl::T is first
   cudaEvent_t e0 = h->ev0, e1 = h->ev1;   // created once with the handle: nothing is allocated per frame
   cudaEventRecord(e0, h->stream);
   int exact = (h->flags & SVS_DT_EXACT_BILINEAR) ? 1 : 0;
@@ -819,12 +807,12 @@ int svs_dt_track(svs_dt* h, double T[7], svs_dt_stats* st) {
     static const int prof_on = getenv("SVS_DT_TIMING") ? 1 : 0;
     int prof = prof_on;
     void* args[] = {&L, &ctl, &part, &sync, &exact, &level, &prof};
-    DCK(cudaLaunchCooperativeKernel((void*)k_dt_track_level, dim3(blocks), dim3(kThreads), args, 0, h->stream));
+    SVS_CK(h, cudaLaunchCooperativeKernel((void*)k_dt_track_level, dim3(blocks), dim3(kThreads), args, 0, h->stream));
   }
   cudaEventRecord(e1, h->stream);
-  DCK(cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(DtCtl), cudaMemcpyDeviceToHost, h->stream));
-  DCK(cudaStreamSynchronize(h->stream));
-  DCK(cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(DtCtl), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
   memcpy(T, h->h_ctl->T, sizeof(double) * 7);
   if (getenv("SVS_DT_TIMING")) {   // cumulative over the handle's frames (the control block is only zeroed at creation)
     static const char* names[7] = {"pose load", "pixels+reduce", "ticket", "wait(release)", "last: partial sums", "last: decide+solve", "last: release"};

@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "se3_dev.cuh"
 #include "svs_nvtx.hpp"
 
@@ -242,11 +243,9 @@ __global__ void k_dtc_pointcloud(M4d TQ, const float* __restrict__ disp, int dis
 
 }  // namespace
 
-struct svs_dtc {
-  int device = 0, nlevels = 0, w0 = 0, h0 = 0;
-  cudaStream_t stream = nullptr;
+struct svs_dtc : svs::Handle {
+  int nlevels = 0, w0 = 0, h0 = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  std::string err;
   int w[kMaxLv] = {}, h[kMaxLv] = {}, stride[kMaxLv] = {}, pitch8[kMaxLv] = {};
   unsigned char* prev8[kMaxLv] = {};
   float* img[kMaxLv][3] = {};   // cur dx dy
@@ -257,15 +256,6 @@ struct svs_dtc {
   DtcCtl* h_ctl = nullptr;
 };
 
-#define TCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 extern "C" {
 
 int svs_dtc_create(int device, int w0, int h0, int nlevels, svs_dtc** out) {
@@ -273,13 +263,13 @@ int svs_dtc_create(int device, int w0, int h0, int nlevels, svs_dtc** out) {
   *out = nullptr;
   for (int l = 0; l < nlevels; ++l)   // the reference asserts the same (dense_tracking.cpp:42-43)
     if (((w0 >> l) % kNth) || ((h0 >> l) % kNth) || (w0 >> l) < 8 || (h0 >> l) < 8) return SVS_ERR_INVALID;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_dtc* h = new svs_dtc();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device; h->nlevels = nlevels; h->w0 = w0; h->h0 = h0;
-  bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaEventCreate(&h->ev0) == cudaSuccess && cudaEventCreate(&h->ev1) == cudaSuccess;
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
+  h->nlevels = nlevels; h->w0 = w0; h->h0 = h0;
+  bool ok = cudaEventCreate(&h->ev0) == cudaSuccess && cudaEventCreate(&h->ev1) == cudaSuccess;
   for (int l = 0; ok && l < nlevels; ++l) {
     h->w[l] = w0 >> l; h->h[l] = h0 >> l;
     h->stride[l] = ((h->w[l] + 63) / 64) * 64;
@@ -304,8 +294,7 @@ int svs_dtc_create(int device, int w0, int h0, int nlevels, svs_dtc** out) {
 
 void svs_dtc_destroy(svs_dtc* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   for (int l = 0; l < kMaxLv; ++l) {
     cudaFree(h->prev8[l]); cudaFree(h->cloud[l]);
     for (int k = 0; k < 3; ++k) cudaFree(h->img[l][k]);
@@ -314,18 +303,17 @@ void svs_dtc_destroy(svs_dtc* h) {
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_dtc_last_error(const svs_dtc* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_dtc_last_error(const svs_dtc* h) { return svs::last_error(h); }
 
 int svs_dtc_set_prev_u8(svs_dtc* h, int level, const unsigned char* img, int pitch, int on_device) {
   if (!h || level < 0 || level >= h->nlevels || !img || pitch < h->w[level]) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  TCK(cudaMemcpy2DAsync(h->prev8[level], h->pitch8[level], img, pitch, h->w[level], h->h[level],
-                        on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
-  if (!on_device) TCK(cudaStreamSynchronize(h->stream));   // pageable source may be reused by the caller
+  SVS_CK(h, cudaMemcpy2DAsync(h->prev8[level], h->pitch8[level], img, pitch, h->w[level], h->h[level],
+                              on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+  if (!on_device) SVS_CK(h, cudaStreamSynchronize(h->stream));   // pageable source may be reused by the caller
   return SVS_OK;
 }
 
@@ -335,19 +323,19 @@ int svs_dtc_set_cur(svs_dtc* h, int level, const float* cur, const float* dx, co
   const float* src[3] = {cur, dx, dy};
   for (int k = 0; k < 3; ++k)
     if (src[k])
-      TCK(cudaMemcpy2DAsync(h->img[level][k], sizeof(float) * h->stride[level], src[k], sizeof(float) * stride_floats,
-                            sizeof(float) * h->w[level], h->h[level],
-                            on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
-  if (!on_device) TCK(cudaStreamSynchronize(h->stream));
+      SVS_CK(h, cudaMemcpy2DAsync(h->img[level][k], sizeof(float) * h->stride[level], src[k], sizeof(float) * stride_floats,
+                                  sizeof(float) * h->w[level], h->h[level],
+                                  on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+  if (!on_device) SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
 int svs_dtc_set_disparity(svs_dtc* h, const float* disp, int stride_floats) {
   if (!h || !disp || stride_floats < h->w0) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  TCK(cudaMemcpy2DAsync(h->disp, sizeof(float) * h->disp_stride, disp, sizeof(float) * stride_floats, sizeof(float) * h->w0,
-                        h->h0, cudaMemcpyHostToDevice, h->stream));
-  TCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(h->disp, sizeof(float) * h->disp_stride, disp, sizeof(float) * stride_floats, sizeof(float) * h->w0,
+                              h->h0, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -377,7 +365,7 @@ int svs_computeDensePointCloudCpu(svs_dtc* h, const double T[7], const svs_cam* 
     const dim3 blk(32, 8), grd((gw + 31) / 32, (gh + 7) / 8);
     k_dtc_pointcloud<<<grd, blk, 0, h->stream>>>(TQ, h->disp, h->disp_stride, l, gw, gh, h->cloud[l]);
   }
-  TCK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 
@@ -385,8 +373,8 @@ int svs_dtc_get_point_cloud(svs_dtc* h, int level, float* cloud_xyzw) {
   if (!h || level < 0 || level >= h->nlevels || !cloud_xyzw) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   const size_t npts = (size_t)(h->w[level] / kNth) * (h->h[level] / kNth);
-  TCK(cudaMemcpyAsync(cloud_xyzw, h->cloud[level], sizeof(float4) * npts, cudaMemcpyDeviceToHost, h->stream));
-  TCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(cloud_xyzw, h->cloud[level], sizeof(float4) * npts, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -394,8 +382,8 @@ int svs_dtc_set_point_cloud(svs_dtc* h, int level, const float* cloud_xyzw) {
   if (!h || level < 0 || level >= h->nlevels || !cloud_xyzw) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   const size_t npts = (size_t)(h->w[level] / kNth) * (h->h[level] / kNth);
-  TCK(cudaMemcpyAsync(h->cloud[level], cloud_xyzw, sizeof(float4) * npts, cudaMemcpyHostToDevice, h->stream));
-  TCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->cloud[level], cloud_xyzw, sizeof(float4) * npts, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -404,8 +392,8 @@ int svs_denseTrackingCpu(svs_dtc* h, const svs_cam* cams, double T[7], svs_dt_st
   if (!h || !cams || !T) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   memcpy(h->h_ctl->T, T, sizeof(double) * 7);
-  TCK(cudaMemcpyAsync(h->d_ctl, h->h_ctl, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
-  TCK(cudaEventRecord(h->ev0, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_ctl, h->h_ctl, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev0, h->stream));
   for (int l = h->nlevels - 1; l >= 0; --l) {
     DtcLevel L;
     L.w = h->w[l]; L.h = h->h[l]; L.stride = h->stride[l]; L.pitch_u8 = h->pitch8[l];
@@ -413,10 +401,10 @@ int svs_denseTrackingCpu(svs_dtc* h, const svs_cam* cams, double T[7], svs_dt_st
     L.prev_u8 = h->prev8[l]; L.cur = h->img[l][0]; L.dx = h->img[l][1]; L.dy = h->img[l][2]; L.cloud = h->cloud[l];
     k_dtc_level<<<1, kThreads, 0, h->stream>>>(L, h->d_ctl, l);
   }
-  TCK(cudaGetLastError());
-  TCK(cudaEventRecord(h->ev1, h->stream));
-  TCK(cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(DtcCtl), cudaMemcpyDeviceToHost, h->stream));
-  TCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev1, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(DtcCtl), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   memcpy(T, h->h_ctl->T, sizeof(double) * 7);
   if (st) {
     memset(st, 0, sizeof *st);

@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "internal.cuh"
 #include "svs_nvtx.hpp"
 
@@ -259,10 +260,7 @@ __global__ void k_fast_emit(const uint8_t* __restrict__ score, int pitch, const 
 
 }  // namespace
 
-struct svs_fast {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_fast : svs::Handle {
   int cap_w = 0, cap_h = 0, pitch = 0, w = 0, h = 0;
   uint8_t* d_img = nullptr;
   uint8_t* d_score = nullptr;
@@ -279,15 +277,6 @@ struct svs_fast {
   int last_total = 0, last_ncells = 0;   // result of the last detect call, still on the device (d_xy, d_cell_off)
 };
 
-#define FCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 namespace svs {
 // keypoints of the last detect call where they lie on the device: xy [n][2], cell_off [ncells + 1] (internal.cuh)
 void fast_device_results(svs_fast* f, const int** d_xy, const int** d_cell_off, int* ncells, int* n, int* device) {
@@ -300,17 +289,15 @@ extern "C" {
 int svs_fast_create(int device, int max_w, int max_h, int max_keypoints, svs_fast** out) {
   if (!out || max_w <= 0 || max_h <= 0 || max_keypoints <= 0) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_fast* h = new svs_fast();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device;
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
   h->cap_w = max_w; h->cap_h = max_h;
   h->pitch = ((max_w + 255) / 256) * 256;
   h->cap_xy = max_keypoints;
-  bool ok = cudaSetDevice(device) == cudaSuccess &&
-            cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess &&
-            cudaMalloc(&h->d_img, (size_t)h->pitch * max_h) == cudaSuccess &&
+  bool ok = cudaMalloc(&h->d_img, (size_t)h->pitch * max_h) == cudaSuccess &&
             cudaMalloc(&h->d_score, (size_t)h->pitch * max_h) == cudaSuccess &&
             cudaMalloc(&h->d_cells, sizeof(CellDev) * kMaxCells) == cudaSuccess &&
             cudaMalloc(&h->d_hist, sizeof(int) * 256 * kMaxCells) == cudaSuccess &&
@@ -330,22 +317,20 @@ int svs_fast_create(int device, int max_w, int max_h, int max_keypoints, svs_fas
 
 void svs_fast_destroy(svs_fast* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   cudaFree(h->d_img); cudaFree(h->d_score); cudaFree(h->d_cells); cudaFree(h->d_hist);
   cudaFree(h->d_thr_detect); cudaFree(h->d_row); cudaFree(h->d_cell_off); cudaFree(h->d_xy);
   if (h->h_pinned) cudaFreeHost(h->h_pinned);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_fast_last_error(const svs_fast* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_fast_last_error(const svs_fast* h) { return svs::last_error(h); }
 
 int svs_fast_set_image(svs_fast* h, const unsigned char* img, int pitch, int w, int hgt) {
   if (!h || !img || w <= 0 || hgt <= 0 || pitch < w) return SVS_ERR_INVALID;
   if (w > h->cap_w || hgt > h->cap_h) { h->err = "image larger than the handle's capacity"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  FCK(cudaMemcpy2DAsync(h->d_img, h->pitch, img, pitch, w, hgt, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(h->d_img, h->pitch, img, pitch, w, hgt, cudaMemcpyHostToDevice, h->stream));
   h->w = w; h->h = hgt; h->has_image = true;
   return SVS_OK;
 }
@@ -354,7 +339,7 @@ int svs_fast_set_image_device(svs_fast* h, const unsigned char* d_img, int pitch
   if (!h || !d_img || w <= 0 || hgt <= 0 || pitch < w) return SVS_ERR_INVALID;
   if (w > h->cap_w || hgt > h->cap_h) { h->err = "image larger than the handle's capacity"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  FCK(cudaMemcpy2DAsync(h->d_img, h->pitch, d_img, pitch, w, hgt, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(h->d_img, h->pitch, d_img, pitch, w, hgt, cudaMemcpyDeviceToDevice, h->stream));
   h->w = w; h->h = hgt; h->has_image = true;
   return SVS_OK;
 }
@@ -386,14 +371,14 @@ static int run_detect(svs_fast* h, svs_fast_cell* cells, int ncells, const svs_f
   const int lim = std::min(max_out, h->cap_xy);
   CellDev* hc = reinterpret_cast<CellDev*>(h->h_pinned + (kMaxCells + 1));
   for (int c = 0; c < ncells; ++c) hc[c] = CellDev{cells[c].u0, cells[c].u1, cells[c].v0, cells[c].v1, cells[c].thr};
-  FCK(cudaMemcpyAsync(h->d_cells, hc, sizeof(CellDev) * ncells, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_cells, hc, sizeof(CellDev) * ncells, cudaMemcpyHostToDevice, h->stream));
   if (max_iw > 0 && max_ih > 0) {
     const dim3 blk(kTileW, kTileH), grd((max_iw + kTileW - 1) / kTileW, (max_ih + kTileH - 1) / kTileH, ncells);
-    if (gp) FCK(cudaMemsetAsync(h->d_hist, 0, sizeof(int) * 256 * ncells, h->stream));
+    if (gp) SVS_CK(h, cudaMemsetAsync(h->d_hist, 0, sizeof(int) * 256 * ncells, h->stream));
     k_fast_score<<<grd, blk, 0, h->stream>>>(h->d_img, h->pitch, h->d_cells, gp ? 0 : 1, t0, h->d_score,
                                              gp ? h->d_hist : nullptr);
   } else if (gp) {
-    FCK(cudaMemsetAsync(h->d_hist, 0, sizeof(int) * 256 * ncells, h->stream));
+    SVS_CK(h, cudaMemsetAsync(h->d_hist, 0, sizeof(int) * 256 * ncells, h->stream));
   }
   if (gp) {
     GridParams g{gp->grid_w, gp->grid_h, gp->fast_min, gp->fast_max, gp->min_inner, gp->min_outer, gp->max_inner, gp->max_outer};
@@ -406,10 +391,10 @@ static int run_detect(svs_fast* h, svs_fast_cell* cells, int ncells, const svs_f
   k_fast_scan<<<1, 1024, 0, h->stream>>>(h->d_cells, ncells, h->cap_h, h->d_row, h->d_cell_off);
   k_fast_emit<<<wgrid, 256, 0, h->stream>>>(h->d_score, h->pitch, h->d_cells, thr_det, h->cap_h, h->d_row, h->d_cell_off,
                                             lim, h->d_xy);
-  FCK(cudaGetLastError());
-  FCK(cudaMemcpyAsync(h->h_pinned, h->d_cell_off, sizeof(int) * (ncells + 1), cudaMemcpyDeviceToHost, h->stream));
-  if (write_back_thr) FCK(cudaMemcpyAsync(hc, h->d_cells, sizeof(CellDev) * ncells, cudaMemcpyDeviceToHost, h->stream));
-  FCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(h->h_pinned, h->d_cell_off, sizeof(int) * (ncells + 1), cudaMemcpyDeviceToHost, h->stream));
+  if (write_back_thr) SVS_CK(h, cudaMemcpyAsync(hc, h->d_cells, sizeof(CellDev) * ncells, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int total = h->h_pinned[ncells];
   h->last_total = std::min(total, lim); h->last_ncells = ncells;
   memcpy(cell_off, h->h_pinned, sizeof(int) * (ncells + 1));
@@ -418,8 +403,8 @@ static int run_detect(svs_fast* h, svs_fast_cell* cells, int ncells, const svs_f
   const int ncopy = std::min(total, lim);
   if (ncopy > 0) {
     int* stage = h->h_pinned + (kMaxCells + 1) + kMaxCells * 5;
-    FCK(cudaMemcpyAsync(stage, h->d_xy, sizeof(int) * 2 * (size_t)ncopy, cudaMemcpyDeviceToHost, h->stream));
-    FCK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpyAsync(stage, h->d_xy, sizeof(int) * 2 * (size_t)ncopy, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
     memcpy(out_xy, stage, sizeof(int) * 2 * (size_t)ncopy);
   }
   return total;

@@ -425,14 +425,14 @@ struct svs::FrontState {
   int* d_cnt = nullptr;            // [0] gated count, [1..2] budget counts
   ProcOut* d_proc = nullptr;
   int* d_group_end = nullptr;
-  int group_cap = 0;
+  size_t group_cap = 0;
   // seeding
   void* d_scratch = nullptr;
   SeedScratch sc{};
   svs_new_point* d_out_pts = nullptr;
   svs_match_point* d_out_rows = nullptr;
   int* d_counts = nullptr;
-  int out_cap = 0;
+  size_t pts_cap = 0, rows_cap = 0;
 };
 
 void svs::front_state_free(FrontState* s) {
@@ -442,22 +442,8 @@ void svs::front_state_free(FrontState* s) {
   delete s;
 }
 
-#define FCK(call)                                                                     \
-  do {                                                                                \
-    cudaError_t e_ = (call);                                                          \
-    if (e_ != cudaSuccess) {                                                          \
-      svs::matcher_set_error(m, (std::string(#call) + ": " + cudaGetErrorString(e_)).c_str()); \
-      return SVS_ERR_CUDA;                                                            \
-    }                                                                                 \
-  } while (0)
-
-static int fail(svs_matcher* m, int rc, const char* msg) {
-  svs::matcher_set_error(m, msg);
-  return rc;
-}
-
 // the state with the buffers every call needs (allocated once per handle)
-static int front_state(svs_matcher* m, const svs::MatcherCore& c, svs::FrontState** out) {
+static int front_state(const svs::MatcherCore& c, svs::FrontState** out) {
   if (!*c.front) {
     // published only once every buffer is there: a failed allocation leaves no half-made state behind
     svs::FrontState* s = new svs::FrontState();
@@ -468,7 +454,7 @@ static int front_state(svs_matcher* m, const svs::MatcherCore& c, svs::FrontStat
     if (!ok) {
       svs::front_state_free(s);
       cudaGetLastError();
-      return fail(m, SVS_ERR_CUDA, "frontend: out of device memory for the state buffers");
+      return svs::fail(c.base, SVS_ERR_CUDA, "frontend: out of device memory for the state buffers");
     }
     *c.front = s;
   }
@@ -500,32 +486,26 @@ int svs_match_track(svs_matcher* m, const double T_cur_from_actkey[7], const dou
   svs::matcher_core(m, &c);
   if (!T_cur_from_actkey || !T_actkey_from_w || n < 0 || n > c.max_pts || (n && !pts) || search_radius < 0 ||
       n_groups < 2 || !group_end)
-    return fail(m, SVS_ERR_INVALID, "match_track: bad pose, point count, radius or groups");
+    return svs::fail(c.base, SVS_ERR_INVALID, "match_track: bad pose, point count, radius or groups");
   for (int g = 0; g < n_groups; ++g)
     if (group_end[g] < (g ? group_end[g - 1] : 0) || group_end[g] > n)
-      return fail(m, SVS_ERR_INVALID, "match_track: group_end must be non-decreasing within [0, n]");
-  if (group_end[n_groups - 1] != n) return fail(m, SVS_ERR_INVALID, "match_track: group_end[n_groups-1] != n");
+      return svs::fail(c.base, SVS_ERR_INVALID, "match_track: group_end must be non-decreasing within [0, n]");
+  if (group_end[n_groups - 1] != n) return svs::fail(c.base, SVS_ERR_INVALID, "match_track: group_end[n_groups-1] != n");
   cudaSetDevice(c.device);
   svs::FrontState* s;
-  int rc = front_state(m, c, &s);
+  int rc = front_state(c, &s);
   if (rc != SVS_OK) return rc;
-  if (s->group_cap < n_groups) {
-    cudaFree(s->d_group_end);
-    s->d_group_end = nullptr;
-    s->group_cap = 0;
-    FCK(cudaMalloc(&s->d_group_end, sizeof(int) * (size_t)n_groups));
-    s->group_cap = n_groups;
-  }
-  if (n) FCK(cudaMemcpyAsync(c.d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, c.stream));
-  FCK(cudaMemcpyAsync(s->d_group_end, group_end, sizeof(int) * (size_t)n_groups, cudaMemcpyHostToDevice, c.stream));
+  SVS_CK(c.base, svs::grow((size_t)n_groups, &s->group_cap, &s->d_group_end));
+  if (n) SVS_CK(c.base, cudaMemcpyAsync(c.d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, c.stream));
+  SVS_CK(c.base, cudaMemcpyAsync(s->d_group_end, group_end, sizeof(int) * (size_t)n_groups, cudaMemcpyHostToDevice, c.stream));
   rc = svs::match_enqueue_own(m, T_cur_from_actkey, T_actkey_from_w, n, search_radius, thr_mean, thr_std);
   if (rc != SVS_OK) return rc;
   k_budget<<<1, kCta, 0, c.stream>>>(c.d_res, n_groups, s->d_group_end, num_max_points, s->d_cnt + 1);
-  FCK(cudaGetLastError());
+  SVS_CK(c.base, cudaGetLastError());
   int cnt[2];
-  FCK(cudaMemcpyAsync(cnt, s->d_cnt + 1, sizeof cnt, cudaMemcpyDeviceToHost, c.stream));
-  if (out && n) FCK(cudaMemcpyAsync(out, c.d_res, sizeof(svs_match_result) * (size_t)n, cudaMemcpyDeviceToHost, c.stream));
-  FCK(cudaStreamSynchronize(c.stream));
+  SVS_CK(c.base, cudaMemcpyAsync(cnt, s->d_cnt + 1, sizeof cnt, cudaMemcpyDeviceToHost, c.stream));
+  if (out && n) SVS_CK(c.base, cudaMemcpyAsync(out, c.d_res, sizeof(svs_match_result) * (size_t)n, cudaMemcpyDeviceToHost, c.stream));
+  SVS_CK(c.base, cudaStreamSynchronize(c.stream));
   if (num_new_feat_matched) *num_new_feat_matched = cnt[0];
   if (num_obs) *num_obs = cnt[1];
   return SVS_OK;
@@ -549,13 +529,13 @@ int svs_processMatchedPoints(svs_matcher* m, const double T_cur_from_actkey[7], 
   svs::MatcherCore c;
   svs::matcher_core(m, &c);
   if (!pose_ok(T_cur_from_actkey) || !cam || !params_ok(params) || n_new < 0)
-    return fail(m, SVS_ERR_INVALID, "processMatchedPoints: bad pose, camera, parameters or n_new");
+    return svs::fail(c.base, SVS_ERR_INVALID, "processMatchedPoints: bad pose, camera, parameters or n_new");
   if (!c.match_serial || !c.last_pts_own)
-    return fail(m, SVS_ERR_STATE, "processMatchedPoints: needs a preceding svs_match or svs_match_track on this handle");
-  if (n_new > c.last_n) return fail(m, SVS_ERR_INVALID, "processMatchedPoints: n_new exceeds the candidates of the last match");
+    return svs::fail(c.base, SVS_ERR_STATE, "processMatchedPoints: needs a preceding svs_match or svs_match_track on this handle");
+  if (n_new > c.last_n) return svs::fail(c.base, SVS_ERR_INVALID, "processMatchedPoints: n_new exceeds the candidates of the last match");
   cudaSetDevice(c.device);
   svs::FrontState* s;
-  int rc = front_state(m, c, &s);
+  int rc = front_state(c, &s);
   if (rc != SVS_OK) return rc;
   s->serial = 0;
   ProcArgs a;
@@ -564,14 +544,14 @@ int svs_processMatchedPoints(svs_matcher* m, const double T_cur_from_actkey[7], 
   a.w0 = c.lv[0].w; a.h0 = c.lv[0].h; a.n = c.last_n; a.n_new = n_new;
   a.max_err = params->max_reproj_error; a.min_num_points = params->min_num_points;
   k_process<<<1, kCta, 0, c.stream>>>(c.d_res, c.d_pts, a, s->d_trk, s->d_term, s->d_cnt, s->d_proc);
-  FCK(cudaGetLastError());
+  SVS_CK(c.base, cudaGetLastError());
   ProcOut po;
-  FCK(cudaMemcpyAsync(&po, s->d_proc, sizeof po, cudaMemcpyDeviceToHost, c.stream));
-  FCK(cudaStreamSynchronize(c.stream));
+  SVS_CK(c.base, cudaMemcpyAsync(&po, s->d_proc, sizeof po, cudaMemcpyDeviceToHost, c.stream));
+  SVS_CK(c.base, cudaStreamSynchronize(c.stream));
   const int ng = po.st.num_tracked;
   if (out && ng) {
-    FCK(cudaMemcpyAsync(out, s->d_trk, sizeof(svs_tracked_point) * (size_t)ng, cudaMemcpyDeviceToHost, c.stream));
-    FCK(cudaStreamSynchronize(c.stream));
+    SVS_CK(c.base, cudaMemcpyAsync(out, s->d_trk, sizeof(svs_tracked_point) * (size_t)ng, cudaMemcpyDeviceToHost, c.stream));
+    SVS_CK(c.base, cudaStreamSynchronize(c.stream));
   }
   s->serial = c.match_serial;
   if (stats) *stats = po.st;
@@ -588,19 +568,19 @@ int svs_addMorePoints(svs_matcher* m, int fresh, const double T_newkey_from_cur[
   svs::MatcherCore c;
   svs::matcher_core(m, &c);
   if ((fresh != 0 && fresh != 1) || !pose_ok(T_newkey_from_cur) || !cam || !params_ok(params))
-    return fail(m, SVS_ERR_INVALID, "addMorePoints: bad mode, pose, camera or parameters");
+    return svs::fail(c.base, SVS_ERR_INVALID, "addMorePoints: bad mode, pose, camera or parameters");
   int bound = 0, off[kLv] = {};
   for (int l = 0; l < c.nlevels; ++l) { off[l] = bound; bound += (params->num_max_points >> l) + 1; }
   if ((points || rows) && cap < bound)
-    return fail(m, SVS_ERR_INVALID, "addMorePoints: cap below the sum over levels of (num_max_points >> l) + 1");
+    return svs::fail(c.base, SVS_ERR_INVALID, "addMorePoints: cap below the sum over levels of (num_max_points >> l) + 1");
   for (int l = 0; l < c.nlevels; ++l)
-    if (c.lv[l].w > 65535 || c.lv[l].h > 65535) return fail(m, SVS_ERR_UNSUPPORTED, "addMorePoints: level wider than 65535");
+    if (c.lv[l].w > 65535 || c.lv[l].h > 65535) return svs::fail(c.base, SVS_ERR_UNSUPPORTED, "addMorePoints: level wider than 65535");
   const svs::FrontState* s0 = *c.front;
   if (!fresh && (!s0 || !s0->serial || s0->serial != c.match_serial))
-    return fail(m, SVS_ERR_STATE, "addMorePoints: no svs_processMatchedPoints since the last match");
+    return svs::fail(c.base, SVS_ERR_STATE, "addMorePoints: no svs_processMatchedPoints since the last match");
   cudaSetDevice(c.device);
   svs::FrontState* s;
-  int rc = front_state(m, c, &s);
+  int rc = front_state(c, &s);
   if (rc != SVS_OK) return rc;
   if (!s->d_scratch) {
     int ncell = 0;
@@ -611,7 +591,7 @@ int svs_addMorePoints(svs_matcher* m, int fresh, const double T_newkey_from_cur[
     q.stride_item = (size_t)c.max_kp + c.max_pts;
     const size_t L = (size_t)c.nlevels;
     const size_t bytes = L * (2 * q.stride_kp * 8 + 8 * q.stride_kp * 4 + 2 * q.stride_cell * 4 + q.stride_item * 4) + 14 * 256;
-    FCK(cudaMalloc(&s->d_scratch, bytes));
+    SVS_CK(c.base, cudaMalloc(&s->d_scratch, bytes));
     char* p = static_cast<char*>(s->d_scratch);
     auto take = [&](size_t b) { char* r = p; p += (b + 255) / 256 * 256; return r; };
     q.key = reinterpret_cast<unsigned long long*>(take(L * q.stride_kp * 8));
@@ -627,14 +607,9 @@ int svs_addMorePoints(svs_matcher* m, int fresh, const double T_newkey_from_cur[
     q.cell_cur = reinterpret_cast<int*>(take(L * q.stride_cell * 4));
     q.cell_item = reinterpret_cast<int*>(take(L * q.stride_item * 4));
   }
-  if (s->out_cap < bound) {
-    cudaFree(s->d_out_pts); cudaFree(s->d_out_rows); cudaFree(s->d_counts);
-    s->d_out_pts = nullptr; s->d_out_rows = nullptr; s->d_counts = nullptr; s->out_cap = 0;
-    FCK(cudaMalloc(&s->d_out_pts, sizeof(svs_new_point) * (size_t)bound));
-    FCK(cudaMalloc(&s->d_out_rows, sizeof(svs_match_point) * (size_t)bound));
-    FCK(cudaMalloc(&s->d_counts, sizeof(int) * kLv));
-    s->out_cap = bound;
-  }
+  SVS_CK(c.base, svs::grow((size_t)bound, &s->pts_cap, &s->d_out_pts));
+  SVS_CK(c.base, svs::grow((size_t)bound, &s->rows_cap, &s->d_out_rows));
+  if (!s->d_counts) SVS_CK(c.base, cudaMalloc(&s->d_counts, sizeof(int) * kLv));
   SeedArgs a;
   memset(&a, 0, sizeof a);
   a.w0 = c.lv[0].w; a.h0 = c.lv[0].h;
@@ -648,14 +623,14 @@ int svs_addMorePoints(svs_matcher* m, int fresh, const double T_newkey_from_cur[
   memcpy(a.T.v, T_newkey_from_cur, sizeof(double) * 7);
   a.f = cam->f; a.px = cam->px; a.py = cam->py; a.b = cam->b;
   k_seed<<<c.nlevels, kSeed, 0, c.stream>>>(a, s->sc, s->d_out_pts, s->d_out_rows, s->d_counts);
-  FCK(cudaGetLastError());
+  SVS_CK(c.base, cudaGetLastError());
   int cnt[kLv] = {};
   std::vector<svs_new_point> hp((size_t)bound);
   std::vector<svs_match_point> hr((size_t)bound);
-  FCK(cudaMemcpyAsync(cnt, s->d_counts, sizeof(int) * c.nlevels, cudaMemcpyDeviceToHost, c.stream));
-  if (points) FCK(cudaMemcpyAsync(hp.data(), s->d_out_pts, sizeof(svs_new_point) * (size_t)bound, cudaMemcpyDeviceToHost, c.stream));
-  if (rows) FCK(cudaMemcpyAsync(hr.data(), s->d_out_rows, sizeof(svs_match_point) * (size_t)bound, cudaMemcpyDeviceToHost, c.stream));
-  FCK(cudaStreamSynchronize(c.stream));
+  SVS_CK(c.base, cudaMemcpyAsync(cnt, s->d_counts, sizeof(int) * c.nlevels, cudaMemcpyDeviceToHost, c.stream));
+  if (points) SVS_CK(c.base, cudaMemcpyAsync(hp.data(), s->d_out_pts, sizeof(svs_new_point) * (size_t)bound, cudaMemcpyDeviceToHost, c.stream));
+  if (rows) SVS_CK(c.base, cudaMemcpyAsync(hr.data(), s->d_out_rows, sizeof(svs_match_point) * (size_t)bound, cudaMemcpyDeviceToHost, c.stream));
+  SVS_CK(c.base, cudaStreamSynchronize(c.stream));
   int total = 0;
   for (int l = 0; l < c.nlevels; ++l) {
     if (points) memcpy(points + total, hp.data() + off[l], sizeof(svs_new_point) * (size_t)cnt[l]);

@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "internal.cuh"
 #include "se3_dev.cuh"
 #include "svs_nvtx.hpp"
@@ -288,10 +289,7 @@ __global__ void k_grow_move(MapDev m, int Np_new, int newkey, const int* __restr
 
 }  // namespace
 
-struct svs_map {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_map : svs::Handle {
   int V = 0, Np = 0, nnz = 0;
   char* d_map = nullptr; size_t map_cap = 0;
   MapDev m{};
@@ -308,15 +306,6 @@ struct svs_map {
   char* d_graph = nullptr; size_t graph_cap = 0; GraphDev g{}; int nnzN = 0;   // svs_map_set_graph
   char* d_sel = nullptr; size_t sel_cap = 0;   // work buffers of svs_map_select_window
 };
-
-#define GCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
 
 static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
 
@@ -348,14 +337,10 @@ extern "C" {
 int svs_map_create(int device, svs_map** out) {
   if (!out) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_map* h = new svs_map();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device;
-  if (cudaSetDevice(device) != cudaSuccess || cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess) {
+  if (int rc = svs::open_handle(h, device)) {
     delete h;
-    return SVS_ERR_CUDA;
+    return rc;
   }
   *out = h;
   return SVS_OK;
@@ -363,14 +348,12 @@ int svs_map_create(int device, svs_map** out) {
 
 void svs_map_destroy(svs_map* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   cudaFree(h->d_map); cudaFree(h->d_work); cudaFree(h->d_upd); cudaFree(h->d_graph); cudaFree(h->d_sel);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_map_last_error(const svs_map* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_map_last_error(const svs_map* h) { return svs::last_error(h); }
 
 int svs_map_set(svs_map* h, int V, const double* T_me_from_world, int Np, const int* point_anchor, const double* xyz_anchor,
                 const int* vis_ptr, const int* vis_pose, const double* feat_center, const int* feat_level) {
@@ -391,26 +374,22 @@ int svs_map_set(svs_map* h, int V, const double* T_me_from_world, int Np, const 
   const size_t off = lo.total;
   const size_t o_pose = lo.o_pose, o_anch = lo.o_anch, o_xyz = lo.o_xyz, o_vptr = lo.o_vptr, o_vpose = lo.o_vpose, o_cen = lo.o_cen,
                o_lvl = lo.o_lvl;
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->d_win_last = nullptr;   // a window assembled from the previous map names its rows, not this map's
-  if (off > h->map_cap) {
-    cudaFree(h->d_map); h->d_map = nullptr; h->map_cap = 0;
-    GCK(cudaMalloc(&h->d_map, off + off / 4));
-    h->map_cap = off + off / 4;
-  }
+  SVS_CK(h, svs::grow(off, &h->map_cap, &h->d_map));
   char* B = h->d_map;
-  GCK(cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)V, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)V, cudaMemcpyHostToDevice, h->stream));
   if (Np) {
-    GCK(cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(B + o_vptr, vis_ptr, sizeof(int) * ((size_t)Np + 1), cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_vptr, vis_ptr, sizeof(int) * ((size_t)Np + 1), cudaMemcpyHostToDevice, h->stream));
   }
   if (nnz) {
-    GCK(cudaMemcpyAsync(B + o_vpose, vis_pose, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(B + o_cen, feat_center, sizeof(double) * 3 * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(B + o_lvl, feat_level, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_vpose, vis_pose, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_cen, feat_center, sizeof(double) * 3 * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_lvl, feat_level, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
   }
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   map_bind(h, B, lo, V, Np, nnz);
   h->g = GraphDev{}; h->nnzN = 0;   // a new map: its pose graph comes with svs_map_set_graph
   return SVS_OK;
@@ -425,17 +404,15 @@ static int map_scatter(svs_map* h, double* table, int rows_in_table, int n, cons
   cudaSetDevice(h->device);
   const size_t ib = al256(sizeof(int) * (size_t)n), rb = sizeof(double) * (size_t)n * width;
   if (ib + rb > h->upd_cap) {
-    GCK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_upd); h->d_upd = nullptr; h->upd_cap = 0;
-    GCK(cudaMalloc(&h->d_upd, 2 * (ib + rb)));
-    h->upd_cap = 2 * (ib + rb);
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
+    SVS_CK(h, svs::grow(ib + rb, &h->upd_cap, &h->d_upd));
   }
-  GCK(cudaMemcpyAsync(h->d_upd, index, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  GCK(cudaMemcpyAsync(h->d_upd + ib, rows, rb, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_upd, index, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_upd + ib, rows, rb, cudaMemcpyHostToDevice, h->stream));
   k_scatter_rows<<<(n * width + 255) / 256, 256, 0, h->stream>>>(table, reinterpret_cast<const int*>(h->d_upd),
                                                                  reinterpret_cast<const double*>(h->d_upd + ib), n, width);
-  GCK(cudaGetLastError());
-  GCK(cudaStreamSynchronize(h->stream));   // the caller's arrays may go away
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the caller's arrays may go away
   return SVS_OK;
 }
 
@@ -452,9 +429,9 @@ int svs_map_update_points(svs_map* h, int n, const int* point, const double* xyz
 int svs_map_get(svs_map* h, double* T_me_from_world, double* xyz_anchor) {
   if (!h || !h->d_map) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  if (T_me_from_world) GCK(cudaMemcpyAsync(T_me_from_world, h->m.pose, sizeof(double) * 7 * (size_t)h->V, cudaMemcpyDeviceToHost, h->stream));
-  if (xyz_anchor && h->Np) GCK(cudaMemcpyAsync(xyz_anchor, h->m.xyz, sizeof(double) * 3 * (size_t)h->Np, cudaMemcpyDeviceToHost, h->stream));
-  GCK(cudaStreamSynchronize(h->stream));
+  if (T_me_from_world) SVS_CK(h, cudaMemcpyAsync(T_me_from_world, h->m.pose, sizeof(double) * 7 * (size_t)h->V, cudaMemcpyDeviceToHost, h->stream));
+  if (xyz_anchor && h->Np) SVS_CK(h, cudaMemcpyAsync(xyz_anchor, h->m.xyz, sizeof(double) * 3 * (size_t)h->Np, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -472,12 +449,12 @@ int svs_map_absorb(svs_map* h, svs_ba* ba) {
     return SVS_ERR_STATE;
   }
   cudaSetDevice(h->device);
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int n = std::max(7 * P, L);
   k_absorb<<<(n + 255) / 256, 256, 0, st>>>(const_cast<double*>(h->m.pose), const_cast<double*>(h->m.xyz), pose[0], pose[1], psi[0], psi[1],
                                             lm_user, cur, h->d_win_last, h->d_act_last, P, L);
-  GCK(cudaGetLastError());
-  GCK(cudaStreamSynchronize(st));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(st));
   return SVS_OK;
 }
 
@@ -520,12 +497,10 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   const size_t o_cj = off; off += al256(sizeof(int) * (size_t)C);
   const size_t o_cT = off; off += al256(sizeof(double) * 7 * (size_t)C);
   const size_t o_cL = off; off += al256(sizeof(double) * 36 * (size_t)C);
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (off > h->work_cap) {
     h->last_E = 0; h->d_oi_last = nullptr; h->d_ep_last = h->d_es_last = h->d_ea_last = nullptr;   // they lay in the old arena
-    cudaFree(h->d_work); h->d_work = nullptr; h->work_cap = 0;
-    GCK(cudaMalloc(&h->d_work, off + off / 4));
-    h->work_cap = off + off / 4;
+    SVS_CK(h, svs::grow(off, &h->work_cap, &h->d_work));
   }
   char* W = h->d_work;
   int* d_wp = reinterpret_cast<int*>(W + o_wp); int* d_win = reinterpret_cast<int*>(W + o_win);
@@ -534,31 +509,31 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   double* d_pose = reinterpret_cast<double*>(W + o_pose); double* d_psi = reinterpret_cast<double*>(W + o_psi);
   int* d_ep = reinterpret_cast<int*>(W + o_ep); int* d_es = reinterpret_cast<int*>(W + o_es); int* d_ea = reinterpret_cast<int*>(W + o_ea);
   double* d_oi = reinterpret_cast<double*>(W + o_oi);
-  GCK(cudaMemcpyAsync(d_wp, h->h_winpos.data(), sizeof(int) * (size_t)h->V, cudaMemcpyHostToDevice, h->stream));
-  GCK(cudaMemcpyAsync(d_win, window_vertex, sizeof(int) * (size_t)P, cudaMemcpyHostToDevice, h->stream));
-  if (L) GCK(cudaMemcpyAsync(d_act, active_point, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
-  GCK(cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream));
-  if (fixed) GCK(cudaMemcpyAsync(W + o_fx, fixed, (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d_wp, h->h_winpos.data(), sizeof(int) * (size_t)h->V, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d_win, window_vertex, sizeof(int) * (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(d_act, active_point, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream));
+  if (fixed) SVS_CK(h, cudaMemcpyAsync(W + o_fx, fixed, (size_t)P, cudaMemcpyHostToDevice, h->stream));
   if (C) {
-    GCK(cudaMemcpyAsync(W + o_ci, c_i, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(W + o_cj, c_j, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(W + o_cT, c_T, sizeof(double) * 7 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    GCK(cudaMemcpyAsync(W + o_cL, c_Lambda, sizeof(double) * 36 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(W + o_ci, c_i, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(W + o_cj, c_j, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(W + o_cT, c_T, sizeof(double) * 7 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(W + o_cL, c_Lambda, sizeof(double) * 36 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
   }
   int E = 0, bad = 0;
   if (L) {
     k_count<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, d_wp, d_act, L, d_cnt, d_bad);
     k_scan<<<1, 1024, 0, h->stream>>>(d_cnt, L, d_ptr);
-    GCK(cudaMemcpyAsync(&E, d_ptr + L, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpyAsync(&E, d_ptr + L, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
     if (bad) { h->err = "an active point is anchored in a frame outside the window"; return SVS_ERR_INVALID; }
     // obs_info = [E][3] observations followed by [E][3] weights: the emit kernel needs E for the second half
     k_emit<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, d_wp, d_act, L, d_ptr, E, d_ep, d_es, d_ea, d_oi, d_psi);
   }
   k_gather_poses<<<(7 * P + 255) / 256, 256, 0, h->stream>>>(h->m, d_win, P, d_pose);
-  GCK(cudaGetLastError());
-  GCK(cudaStreamSynchronize(h->stream));   // the BA handle reads the window on its own stream
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the BA handle reads the window on its own stream
   if (num_edges) *num_edges = E;
   h->d_oi_last = d_oi; h->last_E = E;
   h->d_ep_last = d_ep; h->d_es_last = d_es; h->d_ea_last = d_ea;
@@ -590,22 +565,18 @@ int svs_map_set_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const d
   const size_t o_id = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
   const size_t o_T = off; off += al256(sizeof(double) * 7 * (size_t)std::max(nn, 1));
   const size_t o_L = off; off += al256(sizeof(double) * 36 * (size_t)std::max(nn, 1));
-  GCK(cudaStreamSynchronize(h->stream));
-  if (off > h->graph_cap) {
-    cudaFree(h->d_graph); h->d_graph = nullptr; h->graph_cap = 0;
-    GCK(cudaMalloc(&h->d_graph, off + off / 4));
-    h->graph_cap = off + off / 4;
-  }
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->graph_cap, &h->d_graph));
   char* B = h->d_graph;
-  GCK(cudaMemcpyAsync(B + o_ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + o_ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
   if (nn) {
-    GCK(cudaMemcpyAsync(B + o_id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + o_id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     if (nbr_T) {
-      GCK(cudaMemcpyAsync(B + o_T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
-      GCK(cudaMemcpyAsync(B + o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(B + o_T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(B + o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     }
   }
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->g.nbr_ptr = reinterpret_cast<const int*>(B + o_ptr); h->g.nbr_id = reinterpret_cast<const int*>(B + o_id);
   h->g.nbr_T = nbr_T ? reinterpret_cast<const double*>(B + o_T) : nullptr;
   h->g.nbr_Lam = nbr_T ? reinterpret_cast<const double*>(B + o_L) : nullptr;
@@ -634,16 +605,12 @@ int svs_map_select_window(svs_map* h, int root, int inner_window_size, int doubl
   const size_t o_q = take(sizeof(int) * ((size_t)nn + 1)), o_cc = take(sizeof(int) * V), o_cp = take(sizeof(int) * ((size_t)V + 1));
   const size_t o_ci = take(sizeof(int) * (size_t)std::max(nn, 1)), o_cj = take(sizeof(int) * (size_t)std::max(nn, 1));
   const size_t o_cT = take(sizeof(double) * 7 * (size_t)std::max(nn, 1)), o_cL = take(sizeof(double) * 36 * (size_t)std::max(nn, 1));
-  GCK(cudaStreamSynchronize(h->stream));
-  if (off > h->sel_cap) {
-    cudaFree(h->d_sel); h->d_sel = nullptr; h->sel_cap = 0;
-    GCK(cudaMalloc(&h->d_sel, off + off / 4));
-    h->sel_cap = off + off / 4;
-  }
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
   char* W = h->d_sel;
   auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  GCK(cudaMemsetAsync(I(o_type), 0, sizeof(int) * V, h->stream));
-  GCK(cudaMemsetAsync(I(o_ext), 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(I(o_type), 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(I(o_ext), 0, sizeof(int) * V, h->stream));
   const int bV = (V + 255) / 256, bP = (std::max(Np, 1) + 255) / 256;
   k_bfs<<<1, 32, 0, h->stream>>>(V, h->g, root, inner_window_size, double_window_size, I(o_type), I(o_q), nn + 1);
   if (Np) k_active<<<bP, 256, 0, h->stream>>>(h->m, h->g, I(o_type), I(o_ext), I(o_act));
@@ -658,27 +625,27 @@ int svs_map_select_window(svs_map* h, int root, int inner_window_size, int doubl
   k_scan<<<1, 1024, 0, h->stream>>>(I(o_cc), V, I(o_cp));
   k_pair_emit<<<bV, 256, 0, h->stream>>>(V, h->g, I(o_wtype), I(o_pos), I(o_cp), I(o_ci), I(o_cj),
                                         reinterpret_cast<double*>(W + o_cT), reinterpret_cast<double*>(W + o_cL));
-  GCK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   int P = 0, L = 0, C = 0;
-  GCK(cudaMemcpyAsync(&P, I(o_ptrV) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (Np) GCK(cudaMemcpyAsync(&L, I(o_ptrP) + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  GCK(cudaMemcpyAsync(&C, I(o_cp) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&P, I(o_ptrV) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (Np) SVS_CK(h, cudaMemcpyAsync(&L, I(o_ptrP) + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&C, I(o_cp) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   *P_out = P; *L_out = L;
   if (C_out) *C_out = C;
   if (P > cap_P || L > cap_L || (c_i && C > cap_C)) { h->err = "window, active points or constraints exceed the caller's capacity"; return SVS_ERR_INVALID; }
-  GCK(cudaMemcpyAsync(window_vertex, I(o_win), sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
-  if (L) GCK(cudaMemcpyAsync(active_point, I(o_actl), sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(window_vertex, I(o_win), sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(active_point, I(o_actl), sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
   h->h_winpos.resize(V);
-  GCK(cudaMemcpyAsync(h->h_winpos.data(), I(o_wtype), sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_winpos.data(), I(o_wtype), sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
   if (c_i && C) {
     if (!c_j || !c_T || !c_Lambda) return SVS_ERR_INVALID;
-    GCK(cudaMemcpyAsync(c_i, I(o_ci), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(c_j, I(o_cj), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(c_T, W + o_cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    GCK(cudaMemcpyAsync(c_Lambda, W + o_cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_i, I(o_ci), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_j, I(o_cj), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_T, W + o_cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_Lambda, W + o_cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
   }
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (inner)
     for (int i = 0; i < P; ++i) inner[i] = h->h_winpos[window_vertex[i]] == 1;
   return SVS_OK;
@@ -709,11 +676,11 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
       }
   }
   cudaSetDevice(h->device);
-  GCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int V2 = V + 1, Np2 = Np + n_new, nnz2 = nnz + n_track + 2 * n_new;
   const MapLayout lo = map_layout(V2, Np2, nnz2);
   char* B2 = nullptr;
-  GCK(cudaMalloc(&B2, lo.total + lo.total / 4));
+  SVS_CK(h, cudaMalloc(&B2, lo.total + lo.total / 4));
   // staging: everything the kernels read from the caller, in one pinned-less copy (keyframe rate, a few 10 KB)
   std::vector<char> st;
   auto push = [&](const void* src, size_t bytes) { const size_t o = st.size(); st.resize(o + al256(bytes)); if (bytes) memcpy(st.data() + o, src, bytes); return o; };
@@ -725,11 +692,7 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
   const size_t s_tl = push(track_level, sizeof(int) * (size_t)n_track);
   const size_t s_add = st.size(); st.resize(s_add + al256(sizeof(int) * (size_t)Np2));
   const size_t s_cnt = st.size(); st.resize(s_cnt + al256(sizeof(int) * (size_t)Np2));
-  if (st.size() > h->upd_cap) {
-    cudaFree(h->d_upd); h->d_upd = nullptr; h->upd_cap = 0;
-    if (cudaMalloc(&h->d_upd, 2 * st.size()) != cudaSuccess) { cudaFree(B2); h->err = "cudaMalloc"; return SVS_ERR_CUDA; }
-    h->upd_cap = 2 * st.size();
-  }
+  if (svs::grow(st.size(), &h->upd_cap, &h->d_upd) != cudaSuccess) { cudaFree(B2); h->err = "cudaMalloc"; return SVS_ERR_CUDA; }
   char* U = h->d_upd;
   cudaError_t e = cudaMemcpyAsync(U, st.data(), s_add, cudaMemcpyHostToDevice, h->stream);
   auto D = [&](size_t o) { return reinterpret_cast<double*>(U + o); };
@@ -771,11 +734,11 @@ int svs_map_last_edges(svs_map* h, int E, int* e_point, int* e_pose, int* e_anch
   if (!h || E != h->last_E || !h->d_work) return SVS_ERR_INVALID;
   if (E == 0) return SVS_OK;
   cudaSetDevice(h->device);
-  if (e_point) GCK(cudaMemcpy(e_point, h->d_ep_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
-  if (e_pose) GCK(cudaMemcpy(e_pose, h->d_es_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
-  if (e_anchor) GCK(cudaMemcpy(e_anchor, h->d_ea_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
-  if (e_obs) GCK(cudaMemcpy(e_obs, h->d_oi_last, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
-  if (e_info) GCK(cudaMemcpy(e_info, h->d_oi_last + 3 * (size_t)E, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_point) SVS_CK(h, cudaMemcpy(e_point, h->d_ep_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_pose) SVS_CK(h, cudaMemcpy(e_pose, h->d_es_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_anchor) SVS_CK(h, cudaMemcpy(e_anchor, h->d_ea_last, sizeof(int) * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_obs) SVS_CK(h, cudaMemcpy(e_obs, h->d_oi_last, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
+  if (e_info) SVS_CK(h, cudaMemcpy(e_info, h->d_oi_last + 3 * (size_t)E, sizeof(double) * 3 * (size_t)E, cudaMemcpyDeviceToHost));
   return SVS_OK;
 }
 
@@ -784,12 +747,10 @@ int svs_map_last_edges(svs_map* h, int E, int* e_point, int* e_pose, int* e_anch
 // ------------------------------------------------------------------ hooks of loop.cu (internal.cuh)
 
 void svs::map_view(svs_map* h, MapView* v) {
-  v->V = h->V; v->Np = h->Np; v->nnz = h->nnz; v->device = h->device; v->stream = h->stream;
+  v->V = h->V; v->Np = h->Np; v->nnz = h->nnz; v->device = h->device; v->stream = h->stream; v->base = h;
   v->pose = h->m.pose; v->anchor = h->m.anchor; v->xyz = h->m.xyz; v->vis_ptr = h->m.vis_ptr; v->vis_pose = h->m.vis_pose;
   v->center = h->m.center; v->level = h->m.level;
 }
-
-void svs::map_set_error(svs_map* h, const char* msg) { h->err = msg; }
 
 bool svs::map_graph(svs_map* h, const int** nbr_ptr, const int** nbr_id, int* nnzN) {
   *nbr_ptr = h->g.nbr_ptr; *nbr_id = h->g.nbr_id; *nnzN = h->nnzN;
@@ -806,14 +767,10 @@ int svs::map_add_observations(svs_map* h, int vertex, int n, const int* d_point,
   // observes gains none)
   const MapLayout lo = map_layout(V, Np, nnz + n);
   const size_t s_add = 0, s_cnt = al256(sizeof(int) * (size_t)Np), need = 2 * s_cnt;
-  GCK(cudaStreamSynchronize(h->stream));
-  if (need > h->upd_cap) {
-    cudaFree(h->d_upd); h->d_upd = nullptr; h->upd_cap = 0;
-    GCK(cudaMalloc(&h->d_upd, 2 * need));
-    h->upd_cap = 2 * need;
-  }
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(need, &h->upd_cap, &h->d_upd));
   char* B2 = nullptr;
-  GCK(cudaMalloc(&B2, lo.total + lo.total / 4));
+  SVS_CK(h, cudaMalloc(&B2, lo.total + lo.total / 4));
   int* add = reinterpret_cast<int*>(h->d_upd + s_add);
   int* cnt = reinterpret_cast<int*>(h->d_upd + s_cnt);
   int nnz2 = 0;

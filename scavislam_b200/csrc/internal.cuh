@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 
 namespace svs {
 #ifdef __CUDACC__
@@ -38,9 +39,9 @@ struct MatcherCore {
   int last_pts_own;                // the last match read its candidates from d_pts (svs_match / svs_match_track)
   unsigned long long match_serial; // counts every match on the handle
   FrontState** front;
+  Handle* base;                    // the matcher's error text
 };
 __attribute__((visibility("hidden"))) void matcher_core(svs_matcher* m, MatcherCore* c);
-__attribute__((visibility("hidden"))) void matcher_set_error(svs_matcher* m, const char* msg);
 // k_match on n candidates already in the handle's d_pts, enqueued on its stream (no wait); the results become the
 // handle's last match (last_n = n) once the caller has synchronised
 __attribute__((visibility("hidden"))) int match_enqueue_own(svs_matcher* m, const double T_cur_from_actkey[7],
@@ -109,9 +110,9 @@ struct MapView {
   const int* vis_pose;      // [nnz]
   const double* center;     // [nnz][3]
   const int* level;         // [nnz]
+  Handle* base;             // the map's error text
 };
 __attribute__((visibility("hidden"))) void map_view(svs_map* h, MapView* v);
-__attribute__((visibility("hidden"))) void map_set_error(svs_map* h, const char* msg);
 // the pose graph of svs_map_set_graph on the map's device (nbr_ptr [V+1], nbr_id [nnzN], strongest first); false when
 // none is set
 __attribute__((visibility("hidden"))) bool map_graph(svs_map* h, const int** nbr_ptr, const int** nbr_id, int* nnzN);

@@ -455,13 +455,13 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
                                      int* track_level) {
   svs::NvtxRange nvtx_("globalLoopClosure");
   if (!map) return SVS_ERR_INVALID;
-  auto refuse = [&](const char* msg) { svs::map_set_error(map, msg); return SVS_ERR_INVALID; };
+  svs::MapView m;
+  svs::map_view(map, &m);
+  auto refuse = [&](const char* msg) { return svs::fail(m.base, SVS_ERR_INVALID, msg); };
   if (!mt || !po || !cam || !T_query_from_loop || !res || !vertex_slot || P < 0 || (P && !window_vertex) || cap < 0 ||
       (cap && (!track_point || !track_uvu || !track_level)))
     return refuse("svs_globalLoopClosure: null argument or negative size");
   memset(res, 0, sizeof *res);
-  svs::MapView m;
-  svs::map_view(map, &m);
   svs::MatcherView mv;
   svs::matcher_view(mt, &mv);
   int pdev = -1, max_obs = 0;
@@ -569,7 +569,7 @@ done:
     cudaStreamSynchronize(st);
   }
   if (W) { cudaStreamSynchronize(st); cudaFree(W); }
-  if (rc != SVS_OK) svs::map_set_error(map, cerr.c_str());
+  if (rc != SVS_OK) m.base->err = cerr;
   return rc;
 }
 
@@ -579,7 +579,9 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
                                       double* track_uvu, int* track_level, int* track_committed) {
   svs::NvtxRange nvtx_("localRegisterFrame");
   if (!map) return SVS_ERR_INVALID;
-  auto refuse = [&](const char* msg) { svs::map_set_error(map, msg); return SVS_ERR_INVALID; };
+  svs::MapView m;
+  svs::map_view(map, &m);
+  auto refuse = [&](const char* msg) { return svs::fail(m.base, SVS_ERR_INVALID, msg); };
   if (!mt || !po || !cam || !res || !vertex_slot || P < 0 || (P && !window_vertex) || cap_stats < 0 || cap_tracks < 0 ||
       (cap_stats && !stats) || (cap_tracks && (!track_point || !track_uvu || !track_level || !track_committed)))
     return refuse("svs_localRegisterFrame: null argument or negative size");
@@ -587,12 +589,8 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
   const int* nbr_ptr = nullptr;
   const int* nbr_id = nullptr;
   int nnzN = 0;
-  if (!svs::map_graph(map, &nbr_ptr, &nbr_id, &nnzN)) {
-    svs::map_set_error(map, "svs_map_set_graph has not been called for this map");
-    return SVS_ERR_STATE;
-  }
-  svs::MapView m;
-  svs::map_view(map, &m);
+  if (!svs::map_graph(map, &nbr_ptr, &nbr_id, &nnzN))
+    return svs::fail(m.base, SVS_ERR_STATE, "svs_map_set_graph has not been called for this map");
   svs::MatcherView mv;
   svs::matcher_view(mt, &mv);
   int pdev = -1, max_obs = 0;
@@ -728,7 +726,7 @@ done:
     cudaStreamSynchronize(st);
   }
   if (W) { cudaStreamSynchronize(st); cudaFree(W); }
-  if (rc != SVS_OK) svs::map_set_error(map, cerr.c_str());
+  if (rc != SVS_OK) m.base->err = cerr;
   return rc;
 }
 #undef LCK

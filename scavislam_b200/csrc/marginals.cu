@@ -12,7 +12,7 @@
 #include <cstring>
 #include <vector>
 
-#include "grow.cuh"
+#include "handle.cuh"
 #include "marginals.cuh"
 
 namespace svs {

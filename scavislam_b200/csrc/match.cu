@@ -20,6 +20,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "internal.cuh"
 #include "se3_dev.cuh"
 #include "svs_nvtx.hpp"
@@ -251,10 +252,7 @@ __global__ void k_bucket_fill(const int* __restrict__ xy, int n, int bw, int* __
 
 }  // namespace
 
-struct svs_matcher {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_matcher : svs::Handle {
   int nlevels = 0, max_kf = 0, max_pts = 0, max_kp = 0;
   svs_match_level lv[kMaxLv];
   int pitch[kMaxLv] = {};
@@ -278,15 +276,6 @@ struct svs_matcher {
   svs::FrontState* front = nullptr;     // frontend_points.cu's state, allocated on first use
 };
 
-#define MCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 namespace svs {
 void matcher_device_results(svs_matcher* m, const svs_match_result** d_res, int* n, int* device) {
   *d_res = m->d_res; *n = m->last_n; *device = m->device;
@@ -301,8 +290,8 @@ void matcher_core(svs_matcher* m, MatcherCore* c) {
   c->d_disp = m->d_disp; c->disp_pitch = m->disp_pitch;
   c->last_n = m->last_n; c->last_pts_own = m->last_pts_own; c->match_serial = m->match_serial;
   c->front = &m->front;
+  c->base = m;
 }
-void matcher_set_error(svs_matcher* m, const char* msg) { m->err = msg; }
 void matcher_view(svs_matcher* m, MatcherView* v) {
   v->device = m->device; v->nlevels = m->nlevels; v->max_kf = m->max_kf; v->max_pts = m->max_pts;
   for (int l = 0; l < kMaxLv; ++l) v->lv[l] = l < m->nlevels ? m->lv[l] : svs_match_level{};
@@ -331,7 +320,7 @@ static int match_launch(svs_matcher* h, const double T_cur_from_actkey[7], const
   memcpy(a.T_cur_from_actkey, T_cur_from_actkey, sizeof(double) * 7);
   memcpy(a.T_actkey_from_w, T_actkey_from_w, sizeof(double) * 7);
   k_match<<<(n + kWarps - 1) / kWarps, kWarps * 32, 0, h->stream>>>(a, d_pts, n, h->d_res);
-  MCK(cudaGetLastError());
+  SVS_CK(h, cudaGetLastError());
   return SVS_OK;
 }
 
@@ -346,7 +335,7 @@ int svs::match_device(svs_matcher* h, const double T_cur_from_actkey[7], const d
   cudaSetDevice(h->device);
   const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, d_pts, n, search_radius, thr_mean, thr_std);
   if (rc != SVS_OK) return rc;
-  MCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->last_n = n;
   return SVS_OK;
 }
@@ -370,12 +359,13 @@ int svs_matcher_create(int device, int nlevels, const svs_match_level* levels, i
   if (!out || !levels || nlevels <= 0 || nlevels > kMaxLv || max_keyframes <= 0 || max_points <= 0 || max_keypoints <= 0)
     return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
-  svs_matcher * h = new svs_matcher();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device; h->nlevels = nlevels; h->max_kf = max_keyframes; h->max_pts = max_points; h->max_kp = max_keypoints;
-  bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
+  svs_matcher* h = new svs_matcher();
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
+  h->nlevels = nlevels; h->max_kf = max_keyframes; h->max_pts = max_points; h->max_kp = max_keypoints;
+  bool ok = true;
   h->d_kfimg.assign((size_t)max_keyframes * nlevels, nullptr);
   h->h_kf.assign(max_keyframes, KfDev{});
   for (int l = 0; ok && l < nlevels; ++l) {
@@ -414,8 +404,7 @@ int svs_matcher_create(int device, int nlevels, const svs_match_level* levels, i
 
 void svs_matcher_destroy(svs_matcher * h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   for (int l = 0; l < kMaxLv; ++l) {
     cudaFree(h->d_cur[l]); cudaFree(h->d_kp_xy[l]); cudaFree(h->d_kp_content[l]);
     cudaFree(h->d_bucket_ptr[l]); cudaFree(h->d_bucket_item[l]); cudaFree(h->d_bucket_tmp[l]);
@@ -423,11 +412,10 @@ void svs_matcher_destroy(svs_matcher * h) {
   for (unsigned char* p : h->d_kfimg) cudaFree(p);
   cudaFree(h->d_kf); cudaFree(h->d_disp); cudaFree(h->d_pts); cudaFree(h->d_res);
   svs::front_state_free(h->front);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_matcher_last_error(const svs_matcher * h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_matcher_last_error(const svs_matcher * h) { return svs::last_error(h); }
 
 int svs_matcher_set_keyframe(svs_matcher * h, int slot, const double T_me_from_w[7], const unsigned char* const* pyr,
                            const int* pitch) {
@@ -435,10 +423,10 @@ int svs_matcher_set_keyframe(svs_matcher * h, int slot, const double T_me_from_w
   cudaSetDevice(h->device);
   memcpy(h->h_kf[slot].T, T_me_from_w, sizeof(double) * 7);
   for (int l = 0; l < h->nlevels; ++l)
-    MCK(cudaMemcpy2DAsync(h->d_kfimg[(size_t)slot * h->nlevels + l], h->pitch[l], pyr[l], pitch[l], h->lv[l].w, h->lv[l].h,
-                          cudaMemcpyHostToDevice, h->stream));
-  MCK(cudaMemcpyAsync(h->d_kf + slot, &h->h_kf[slot], sizeof(KfDev), cudaMemcpyHostToDevice, h->stream));
-  MCK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpy2DAsync(h->d_kfimg[(size_t)slot * h->nlevels + l], h->pitch[l], pyr[l], pitch[l], h->lv[l].w, h->lv[l].h,
+                                cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_kf + slot, &h->h_kf[slot], sizeof(KfDev), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -447,11 +435,11 @@ int svs_matcher_set_current(svs_matcher * h, const unsigned char* const* pyr, co
   if (!h || (pyr && !pitch) || (!pyr && !disp)) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
   for (int l = 0; pyr && l < h->nlevels; ++l)
-    MCK(cudaMemcpy2DAsync(h->d_cur[l], h->pitch[l], pyr[l], pitch[l], h->lv[l].w, h->lv[l].h, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpy2DAsync(h->d_cur[l], h->pitch[l], pyr[l], pitch[l], h->lv[l].w, h->lv[l].h, cudaMemcpyHostToDevice, h->stream));
   if (disp)
-    MCK(cudaMemcpy2DAsync(h->d_disp, sizeof(float) * h->disp_pitch, disp, sizeof(float) * disp_pitch_floats,
-                          sizeof(float) * h->lv[0].w, h->lv[0].h, cudaMemcpyHostToDevice, h->stream));
-  MCK(cudaStreamSynchronize(h->stream));
+    SVS_CK(h, cudaMemcpy2DAsync(h->d_disp, sizeof(float) * h->disp_pitch, disp, sizeof(float) * disp_pitch_floats,
+                                sizeof(float) * h->lv[0].w, h->lv[0].h, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -463,13 +451,13 @@ int svs_matcher_set_pyramid_device(svs_matcher * h, int which, const double T_me
   cudaSetDevice(h->device);
   for (int l = 0; l < h->nlevels; ++l) {
     unsigned char* dst = which < 0 ? h->d_cur[l] : h->d_kfimg[(size_t)which * h->nlevels + l];
-    MCK(cudaMemcpy2DAsync(dst, h->pitch[l], d_pyr[l], pitch[l], h->lv[l].w, h->lv[l].h, cudaMemcpyDeviceToDevice, h->stream));
+    SVS_CK(h, cudaMemcpy2DAsync(dst, h->pitch[l], d_pyr[l], pitch[l], h->lv[l].w, h->lv[l].h, cudaMemcpyDeviceToDevice, h->stream));
   }
   if (which >= 0) {
     memcpy(h->h_kf[which].T, T_me_from_w, sizeof(double) * 7);
-    MCK(cudaMemcpyAsync(h->d_kf + which, &h->h_kf[which], sizeof(KfDev), cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->d_kf + which, &h->h_kf[which], sizeof(KfDev), cudaMemcpyHostToDevice, h->stream));
   }
-  MCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }
 
@@ -483,18 +471,18 @@ int svs_matcher_set_features(svs_matcher * h, int level, const int* xy, const in
   cudaSetDevice(h->device);
   const int nb = h->bw[level] * h->bh[level];
   h->nkp[level] = n;
-  MCK(cudaMemsetAsync(h->d_bucket_tmp[level], 0, sizeof(int) * 2 * nb, h->stream));
+  SVS_CK(h, cudaMemsetAsync(h->d_bucket_tmp[level], 0, sizeof(int) * 2 * nb, h->stream));
   if (n) {
-    MCK(cudaMemcpyAsync(h->d_kp_xy[level], xy, sizeof(int) * 2 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-    MCK(cudaMemcpyAsync(h->d_kp_content[level], content, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->d_kp_xy[level], xy, sizeof(int) * 2 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(h->d_kp_content[level], content, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
     k_bucket_count<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_kp_xy[level], n, h->bw[level], h->d_bucket_tmp[level]);
   }
   k_bucket_scan<<<1, 32, 0, h->stream>>>(h->d_bucket_tmp[level], nb, h->d_bucket_ptr[level], h->d_bucket_tmp[level] + nb);
   if (n)
     k_bucket_fill<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_kp_xy[level], n, h->bw[level], h->d_bucket_tmp[level] + nb,
                                                           h->d_bucket_item[level]);
-  MCK(cudaGetLastError());
-  MCK(cudaStreamSynchronize(h->stream));   // host arrays may go away
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // host arrays may go away
   return SVS_OK;
 }
 
@@ -519,7 +507,7 @@ int svs_matcher_set_features_from_fast(svs_matcher * h, int level, svs_fast* fas
   cudaSetDevice(h->device);
   const int nb = h->bw[level] * h->bh[level];
   h->nkp[level] = n;
-  MCK(cudaMemsetAsync(h->d_bucket_tmp[level], 0, sizeof(int) * 2 * nb, h->stream));
+  SVS_CK(h, cudaMemsetAsync(h->d_bucket_tmp[level], 0, sizeof(int) * 2 * nb, h->stream));
   if (n) {
     // the detect call synchronised the FAST handle's stream before it returned: its results are complete
     k_kp_from_fast<<<(n + 255) / 256, 256, 0, h->stream>>>(d_xy, d_off, ncells, n, h->d_kp_xy[level], h->d_kp_content[level]);
@@ -529,8 +517,8 @@ int svs_matcher_set_features_from_fast(svs_matcher * h, int level, svs_fast* fas
   if (n)
     k_bucket_fill<<<(n + 255) / 256, 256, 0, h->stream>>>(h->d_kp_xy[level], n, h->bw[level], h->d_bucket_tmp[level] + nb,
                                                           h->d_bucket_item[level]);
-  MCK(cudaGetLastError());
-  MCK(cudaStreamSynchronize(h->stream));   // the FAST handle may detect again
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // the FAST handle may detect again
   return SVS_OK;
 }
 
@@ -544,11 +532,11 @@ int svs_match(svs_matcher * h, const double T_cur_from_actkey[7], const double T
   ++h->match_serial;
   if (n == 0) return 0;
   cudaSetDevice(h->device);
-  MCK(cudaMemcpyAsync(h->d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_pts, pts, sizeof(svs_match_point) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
   const int rc = match_launch(h, T_cur_from_actkey, T_actkey_from_w, h->d_pts, n, search_radius, thr_mean, thr_std);
   if (rc != SVS_OK) return rc;
-  MCK(cudaMemcpyAsync(out, h->d_res, sizeof(svs_match_result) * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
-  MCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(out, h->d_res, sizeof(svs_match_result) * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->last_n = n;
   int nm = 0;
   for (int i = 0; i < n; ++i) nm += out[i].matched;

@@ -19,6 +19,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 
 // named (not anonymous) so the kernels keep stable symbol names in traces: place::k_place_nn, ...
 namespace place {
@@ -565,12 +566,10 @@ struct DevArr {             // device array that grows geometrically and keeps i
   void release() { cudaFree(p); p = nullptr; cap = 0; }
 };
 
-struct svs_place {
-  int device = 0, W = 0, sms = 132;
+struct svs_place : svs::Handle {
+  int W = 0, sms = 132;
   Cam cam{};
-  cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  std::string err;
   // vocabulary and per-word state
   float* d_words = nullptr;
   int* d_cw = nullptr;          // places holding each word
@@ -596,15 +595,6 @@ struct svs_place {
   int last_n = 0, last_L = 0, last_scored = 0;
 };
 
-#define PCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 // the split of the nearest-neighbour kernel: query blocks of kTile rows; the train tiles are divided over enough
 // CTAs that the grid covers about two waves of the device, never more slices than tiles
 static dim3 nn_grid(int n, int m, int sms) {
@@ -619,18 +609,16 @@ int svs_place_create(int device, int num_words, const float* words, const svs_ca
   if (!out) return SVS_ERR_INVALID;
   *out = nullptr;
   if (num_words <= 0 || !words || !cam) return SVS_ERR_INVALID;
-  int nd = 0;
-  if (cudaGetDeviceCount(&nd) != cudaSuccess || nd == 0) return SVS_ERR_NOGPU;
-  if (device < 0) cudaGetDevice(&device);
   svs_place* h = new svs_place();
-  h->device = device;
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
   h->W = num_words;
   h->cam = Cam{cam->f, cam->px, cam->py, cam->b};
   auto fail = [&]() { svs_place_destroy(h); return SVS_ERR_CUDA; };
-  if (cudaSetDevice(device) != cudaSuccess) return fail();
   cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device);
-  if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess ||
+  if (cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess ||
       cudaMalloc(&h->d_words, sizeof(float) * kDim * (size_t)num_words) != cudaSuccess ||
       cudaMalloc(&h->d_cw, sizeof(int) * (size_t)num_words) != cudaSuccess ||
       cudaMalloc(&h->d_first_row, sizeof(int) * (size_t)num_words) != cudaSuccess ||
@@ -650,8 +638,7 @@ int svs_place_create(int device, int num_words, const float* words, const svs_ca
 
 void svs_place_destroy(svs_place* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   for (auto* a : {&h->desc, &h->score, &h->dist}) a->release();
   for (auto* a : {&h->xyz, &h->uvu, &h->hyp_RT}) a->release();
   for (auto* a : {&h->wl_word, &h->wl_count, &h->p_row_off, &h->p_nrows, &h->p_wl_off, &h->p_wl_n, &h->p_nwords,
@@ -661,11 +648,10 @@ void svs_place_destroy(svs_place* h) {
   cudaFree(h->d_words); cudaFree(h->d_cw); cudaFree(h->d_first_row); cudaFree(h->d_kf_count); cudaFree(h->d_res);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_place_last_error(const svs_place* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_place_last_error(const svs_place* h) { return svs::last_error(h); }
 
 int svs_place_add_location(svs_place* h, int keyframe_id, int n, const float* desc, const double* uvu,
                            int do_loop_detection, int n_exclude, const int* exclude_ids, const svs_place_params* p,
@@ -678,27 +664,27 @@ int svs_place_add_location(svs_place* h, int keyframe_id, int n, const float* de
   if (prm.num_ransac < 0) { h->err = "num_ransac < 0"; return SVS_ERR_INVALID; }
   if (!(prm.pixel_thr > 0.0) || !std::isfinite(prm.pixel_thr)) { h->err = "pixel_thr not > 0 and finite"; return SVS_ERR_INVALID; }
   if (h->index_of.count(keyframe_id)) { h->err = "keyframe id already in the database"; return SVS_ERR_INVALID; }
-  PCK(cudaSetDevice(h->device));
+  SVS_CK(h, cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   const int L = h->L, H = prm.num_ransac;
   const size_t n1 = (size_t)std::max(n, 1);
   // storage: the database grows geometrically; the per-call buffers keep their largest size
-  PCK(h->desc.reserve(((size_t)h->rows + n1) * kDim, s));
-  PCK(h->xyz.reserve(((size_t)h->rows + n1) * 3, s));
-  PCK(h->wl_word.reserve((size_t)h->wl + n1, s));
-  PCK(h->wl_count.reserve((size_t)h->wl + n1, s));
+  SVS_CK(h, h->desc.reserve(((size_t)h->rows + n1) * kDim, s));
+  SVS_CK(h, h->xyz.reserve(((size_t)h->rows + n1) * 3, s));
+  SVS_CK(h, h->wl_word.reserve((size_t)h->wl + n1, s));
+  SVS_CK(h, h->wl_count.reserve((size_t)h->wl + n1, s));
   for (auto* a : {&h->p_row_off, &h->p_nrows, &h->p_wl_off, &h->p_wl_n, &h->p_nwords, &h->p_id})
-    PCK(a->reserve((size_t)L + 1, s));
-  PCK(h->score.reserve((size_t)L + 1, s));
-  PCK(h->excluded.reserve((size_t)L + 1, s));
-  PCK(h->uvu.reserve(3 * n1, s));
-  PCK(h->best_word.reserve(n1, s));
-  PCK(h->best_match.reserve(n1, s));
-  for (auto* a : {&h->word, &h->train_idx, &h->inl_q, &h->inl_t}) PCK(a->reserve(n1, s));
-  PCK(h->dist.reserve(n1, s));
-  PCK(h->hyp_triple.reserve(3 * (size_t)std::max(H, 1), s));
-  PCK(h->hyp_inl.reserve((size_t)std::max(H, 1), s));
-  PCK(h->hyp_RT.reserve(12 * (size_t)std::max(H, 1), s));
+    SVS_CK(h, a->reserve((size_t)L + 1, s));
+  SVS_CK(h, h->score.reserve((size_t)L + 1, s));
+  SVS_CK(h, h->excluded.reserve((size_t)L + 1, s));
+  SVS_CK(h, h->uvu.reserve(3 * n1, s));
+  SVS_CK(h, h->best_word.reserve(n1, s));
+  SVS_CK(h, h->best_match.reserve(n1, s));
+  for (auto* a : {&h->word, &h->train_idx, &h->inl_q, &h->inl_t}) SVS_CK(h, a->reserve(n1, s));
+  SVS_CK(h, h->dist.reserve(n1, s));
+  SVS_CK(h, h->hyp_triple.reserve(3 * (size_t)std::max(H, 1), s));
+  SVS_CK(h, h->hyp_inl.reserve((size_t)std::max(H, 1), s));
+  SVS_CK(h, h->hyp_RT.reserve(12 * (size_t)std::max(H, 1), s));
 
   std::vector<unsigned char> excl((size_t)L + 1, 0);
   for (int e = 0; e < n_exclude; ++e) {
@@ -709,24 +695,24 @@ int svs_place_add_location(svs_place* h, int keyframe_id, int n, const float* de
   init.best_place = -1; init.best_kf = -1; init.best_h = -1;
   init.T[3] = 1.0;
   float* q = h->desc.p + (size_t)h->rows * kDim;   // the new rows go straight into the database
-  PCK(cudaEventRecord(h->ev0, s));
-  PCK(cudaMemcpyAsync(h->d_res, &init, sizeof init, cudaMemcpyHostToDevice, s));
+  SVS_CK(h, cudaEventRecord(h->ev0, s));
+  SVS_CK(h, cudaMemcpyAsync(h->d_res, &init, sizeof init, cudaMemcpyHostToDevice, s));
   if (n > 0) {
-    PCK(cudaMemcpyAsync(q, desc, sizeof(float) * kDim * (size_t)n, cudaMemcpyHostToDevice, s));
-    PCK(cudaMemcpyAsync(h->uvu.p, uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, s));
-    PCK(cudaMemsetAsync(h->best_word.p, 0xff, sizeof(unsigned long long) * (size_t)n, s));
+    SVS_CK(h, cudaMemcpyAsync(q, desc, sizeof(float) * kDim * (size_t)n, cudaMemcpyHostToDevice, s));
+    SVS_CK(h, cudaMemcpyAsync(h->uvu.p, uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, s));
+    SVS_CK(h, cudaMemsetAsync(h->best_word.p, 0xff, sizeof(unsigned long long) * (size_t)n, s));
     k_place_nn<<<nn_grid(n, h->W, h->sms), kNNThreads, 0, s>>>(q, n, h->d_words, h->W, nullptr, nullptr, nullptr,
                                                                  h->best_word.p);
     k_place_assign<<<(n + 255) / 256, 256, 0, s>>>(h->best_word.p, n, h->word.p, h->d_first_row, h->d_kf_count, h->d_res);
   }
   const bool scored = do_loop_detection && L > 0 && n > 0;
   if (scored) {
-    PCK(cudaMemcpyAsync(h->excluded.p, excl.data(), (size_t)L, cudaMemcpyHostToDevice, s));
+    SVS_CK(h, cudaMemcpyAsync(h->excluded.p, excl.data(), (size_t)L, cudaMemcpyHostToDevice, s));
     k_place_score<<<(L + 7) / 8, 256, 0, s>>>(L, n, h->word.p, h->d_first_row, h->d_cw, h->p_wl_off.p, h->p_wl_n.p,
                                               h->wl_word.p, h->wl_count.p, h->p_nwords.p, h->excluded.p, h->score.p);
     k_place_select<<<1, 1024, 0, s>>>(L, h->score.p, h->p_id.p, h->d_res);
     // the match and the geometric check read the candidate from device memory and return at once without one
-    PCK(cudaMemsetAsync(h->best_match.p, 0xff, sizeof(unsigned long long) * (size_t)n, s));
+    SVS_CK(h, cudaMemsetAsync(h->best_match.p, 0xff, sizeof(unsigned long long) * (size_t)n, s));
     k_place_nn<<<nn_grid(n, h->max_rows, h->sms), kNNThreads, 0, s>>>(q, n, h->desc.p, 0, &h->d_res->best_place,
                                                                        h->p_row_off.p, h->p_nrows.p, h->best_match.p);
     k_place_match_fin<<<(n + 255) / 256, 256, 0, s>>>(h->best_match.p, n, h->p_nrows.p, h->d_res, h->train_idx.p,
@@ -745,15 +731,15 @@ int svs_place_add_location(svs_place* h, int keyframe_id, int n, const float* de
   ia.p_row_off = h->p_row_off.p; ia.p_nrows = h->p_nrows.p; ia.p_wl_off = h->p_wl_off.p; ia.p_wl_n = h->p_wl_n.p;
   ia.p_nwords = h->p_nwords.p; ia.p_id = h->p_id.p; ia.res = h->d_res;
   k_place_insert<<<1, 1024, 0, s>>>(ia);
-  PCK(cudaGetLastError());
-  PCK(cudaEventRecord(h->ev1, s));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev1, s));
   PlaceRes r{};
-  PCK(cudaMemcpyAsync(&r, h->d_res, sizeof r, cudaMemcpyDeviceToHost, s));
-  PCK(cudaStreamSynchronize(s));
+  SVS_CK(h, cudaMemcpyAsync(&r, h->d_res, sizeof r, cudaMemcpyDeviceToHost, s));
+  SVS_CK(h, cudaStreamSynchronize(s));
   if (r.num_inliers > 0 && inlier_query)
-    PCK(cudaMemcpy(inlier_query, h->inl_q.p, sizeof(int) * (size_t)r.num_inliers, cudaMemcpyDeviceToHost));
+    SVS_CK(h, cudaMemcpy(inlier_query, h->inl_q.p, sizeof(int) * (size_t)r.num_inliers, cudaMemcpyDeviceToHost));
   if (r.num_inliers > 0 && inlier_train)
-    PCK(cudaMemcpy(inlier_train, h->inl_t.p, sizeof(int) * (size_t)r.num_inliers, cudaMemcpyDeviceToHost));
+    SVS_CK(h, cudaMemcpy(inlier_train, h->inl_t.p, sizeof(int) * (size_t)r.num_inliers, cudaMemcpyDeviceToHost));
   // the place is in the database: update the host's view of it
   h->index_of[keyframe_id] = L;
   h->ids.push_back(keyframe_id);

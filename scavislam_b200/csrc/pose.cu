@@ -24,6 +24,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 #include "internal.cuh"
 #include "se3_dev.cuh"
 #include "svs_nvtx.hpp"
@@ -611,11 +612,9 @@ __global__ void __launch_bounds__(kGradThreads) k_point_ranges(const int* __rest
 
 }  // namespace
 
-struct svs_pose {
-  int device = 0, max_obs = 0;
-  cudaStream_t stream = nullptr;
+struct svs_pose : svs::Handle {
+  int max_obs = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  std::string err;
   int* d_pid = nullptr;
   double* d_obs = nullptr;
   double* d_xyz = nullptr;
@@ -638,23 +637,7 @@ struct svs_pose {
   size_t cub_bytes = 0;
 };
 
-#define QCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 void svs::pose_capacity(const svs_pose* h, int* device, int* max_obs) { *device = h->device; *max_obs = h->max_obs; }
-
-// true when p is device (or managed) memory of the handle's device
-static bool on_handle_device(const svs_pose* h, const void* p) {
-  cudaPointerAttributes a{};
-  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-  return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == h->device;
-}
 
 // after a successful array or device call: the problem svs_pose_grad differentiates
 static void keep_problem(svs_pose* h, const PoseArgs& a, int npoints) {
@@ -672,9 +655,9 @@ static int run(svs_pose* h, PoseArgs& a, const svs_cam* cam, const svs_pose_para
   a.initial_mu = p->initial_mu; a.tau = p->tau;
   memcpy(h->h_ctl->T, T, sizeof(double) * 7);
   h->h_ctl->bad_pid = 0;
-  QCK(cudaMemcpyAsync(h->d_ctl, h->h_ctl, offsetof(PoseCtl, bad_pid) + sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_ctl, h->h_ctl, offsetof(PoseCtl, bad_pid) + sizeof(int), cudaMemcpyHostToDevice, h->stream));
   if (src_pid) k_pose_ingest<<<(unsigned)((a.n + 255) / 256), 256, 0, h->stream>>>(src_pid, a.n, npoints, h->d_pid, h->d_ctl);
-  QCK(cudaEventRecord(h->ev0, h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev0, h->stream));
   if (a.n > kClusterMinObs) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(kCl, 1, 1);
@@ -693,10 +676,10 @@ static int run(svs_pose* h, PoseArgs& a, const svs_cam* cam, const svs_pose_para
   } else {
     k_pose_lm<kCtaThreads, false><<<1, kCtaThreads, 0, h->stream>>>(a, h->d_ctl);
   }
-  QCK(cudaGetLastError());
-  QCK(cudaEventRecord(h->ev1, h->stream));
-  QCK(cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PoseCtl), cudaMemcpyDeviceToHost, h->stream));
-  QCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev1, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PoseCtl), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   const PoseCtl& c = *h->h_ctl;
   if (c.bad_pid) { h->err = "obs.point_id outside point_list"; return SVS_ERR_INVALID; }
   if (c.nan_error) { h->err = "Res is NaN!"; return SVS_ERR_NUMERIC; }
@@ -714,14 +697,13 @@ extern "C" {
 int svs_pose_create(int device, int max_obs, svs_pose** out) {
   if (!out || max_obs <= 0) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_pose* h = new svs_pose();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device; h->max_obs = max_obs;
-  const bool ok = cudaSetDevice(device) == cudaSuccess &&
-                  cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess &&
-                  cudaEventCreate(&h->ev0) == cudaSuccess && cudaEventCreate(&h->ev1) == cudaSuccess &&
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
+  h->max_obs = max_obs;
+  const bool ok = cudaEventCreate(&h->ev0) == cudaSuccess && cudaEventCreate(&h->ev1) == cudaSuccess &&
                   cudaMalloc(&h->d_pid, sizeof(int) * (size_t)max_obs) == cudaSuccess &&
                   cudaMalloc(&h->d_obs, sizeof(double) * 3 * (size_t)max_obs) == cudaSuccess &&
                   cudaMalloc(&h->d_xyz, sizeof(double) * 3 * (size_t)max_obs) == cudaSuccess &&
@@ -734,19 +716,17 @@ int svs_pose_create(int device, int max_obs, svs_pose** out) {
 
 void svs_pose_destroy(svs_pose* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   cudaFree(h->d_pid); cudaFree(h->d_obs); cudaFree(h->d_xyz); cudaFree(h->d_ctl);
   cudaFree(h->d_gctl); cudaFree(h->d_gout); cudaFree(h->d_q); cudaFree(h->d_c); cudaFree(h->d_sort); cudaFree(h->d_cub);
   if (h->h_gout) cudaFreeHost(h->h_gout);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_pose_last_error(const svs_pose* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_pose_last_error(const svs_pose* h) { return svs::last_error(h); }
 
 int svs_calcFastMotionOnly(svs_pose* h, int n, const int* obs_point_id, const double* obs_uvu, int npoints,
                            const double* point_xyz, const svs_cam* cam, const svs_pose_params* params, double T_frame[7],
@@ -760,9 +740,9 @@ int svs_calcFastMotionOnly(svs_pose* h, int n, const int* obs_point_id, const do
   for (int i = 0; i < n; ++i)
     if (obs_point_id[i] < 0 || obs_point_id[i] >= npoints) { h->err = "obs.point_id outside point_list"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  QCK(cudaMemcpyAsync(h->d_pid, obs_point_id, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  QCK(cudaMemcpyAsync(h->d_obs, obs_uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  QCK(cudaMemcpyAsync(h->d_xyz, point_xyz, sizeof(double) * 3 * (size_t)npoints, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_pid, obs_point_id, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_obs, obs_uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_xyz, point_xyz, sizeof(double) * 3 * (size_t)npoints, cudaMemcpyHostToDevice, h->stream));
   PoseArgs a;
   memset(&a, 0, sizeof a);
   a.pid = h->d_pid; a.obs = reinterpret_cast<const char*>(h->d_obs); a.xyz = reinterpret_cast<const char*>(h->d_xyz);
@@ -782,13 +762,13 @@ int svs_calcFastMotionOnly_device(svs_pose* h, int n, const int* obs_point_id, c
     return SVS_ERR_INVALID;
   if (n > h->max_obs || npoints > h->max_obs) { h->err = "more observations/points than the handle's capacity"; return SVS_ERR_INVALID; }
   for (const void* p : {(const void*)obs_point_id, (const void*)obs_uvu, (const void*)point_xyz})
-    if (!on_handle_device(h, p)) {
+    if (!svs::on_device(h->device, p)) {
       h->err = "svs_calcFastMotionOnly_device: an array is not device memory of the handle's device";
       return SVS_ERR_INVALID;
     }
   cudaSetDevice(h->device);
-  QCK(cudaMemcpyAsync(h->d_obs, obs_uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
-  QCK(cudaMemcpyAsync(h->d_xyz, point_xyz, sizeof(double) * 3 * (size_t)npoints, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_obs, obs_uvu, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->d_xyz, point_xyz, sizeof(double) * 3 * (size_t)npoints, cudaMemcpyDeviceToDevice, h->stream));
   PoseArgs a;
   memset(&a, 0, sizeof a);
   a.pid = h->d_pid; a.obs = reinterpret_cast<const char*>(h->d_obs); a.xyz = reinterpret_cast<const char*>(h->d_xyz);
@@ -811,7 +791,7 @@ int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_
   if (!std::isfinite(lambda) || lambda < 0.) { h->err = "svs_pose_grad: lambda must be finite and >= 0"; return SVS_ERR_INVALID; }
   if (on_device)
     for (const void* p : {(const void*)dL_dT, (const void*)dL_dobs, (const void*)dL_dxyz, (const void*)dL_dcam})
-      if (p && !on_handle_device(h, p)) {
+      if (p && !svs::on_device(h->device, p)) {
         h->err = "svs_pose_grad: on_device = 1 but an array is not device memory of the handle's device";
         return SVS_ERR_INVALID;
       }
@@ -819,12 +799,12 @@ int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_
   const int n = h->last.n, np = h->npoints, cap = h->max_obs;
   const size_t o_xyz = 3 * (size_t)cap, o_cam = 6 * (size_t)cap, o_ctl = o_cam + 4;   // offsets in d_gout / h_gout
   if (!h->d_gctl) {   // first gradient call on this handle (d_gctl last: it marks the set complete)
-    if (!h->d_gout) QCK(cudaMalloc(&h->d_gout, sizeof(double) * o_ctl));
-    if (!h->h_gout) QCK(cudaMallocHost(&h->h_gout, sizeof(double) * o_ctl + sizeof(PoseGradCtl)));
-    if (!h->d_q) QCK(cudaMalloc(&h->d_q, sizeof(double) * 3 * (size_t)cap));
-    if (!h->d_c) QCK(cudaMalloc(&h->d_c, sizeof(double) * 4 * (size_t)cap));
-    if (!h->d_sort) QCK(cudaMalloc(&h->d_sort, sizeof(int) * 5 * (size_t)cap));
-    QCK(cudaMalloc(&h->d_gctl, sizeof(PoseGradCtl)));
+    if (!h->d_gout) SVS_CK(h, cudaMalloc(&h->d_gout, sizeof(double) * o_ctl));
+    if (!h->h_gout) SVS_CK(h, cudaMallocHost(&h->h_gout, sizeof(double) * o_ctl + sizeof(PoseGradCtl)));
+    if (!h->d_q) SVS_CK(h, cudaMalloc(&h->d_q, sizeof(double) * 3 * (size_t)cap));
+    if (!h->d_c) SVS_CK(h, cudaMalloc(&h->d_c, sizeof(double) * 4 * (size_t)cap));
+    if (!h->d_sort) SVS_CK(h, cudaMalloc(&h->d_sort, sizeof(int) * 5 * (size_t)cap));
+    SVS_CK(h, cudaMalloc(&h->d_gctl, sizeof(PoseGradCtl)));
   }
   PoseGradCtl* h_gctl = reinterpret_cast<PoseGradCtl*>(h->h_gout + o_ctl);
   int* keys = h->d_sort; int* iota = keys + cap; int* order = iota + cap; int* start = order + cap; int* end = start + cap;
@@ -834,18 +814,18 @@ int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_
     int bits = 1;
     while (bits < 31 && (1 << bits) < np) ++bits;
     size_t need = 0;
-    QCK(cub::DeviceRadixSort::SortPairs(nullptr, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(nullptr, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
     if (need > h->cub_bytes) {
-      QCK(cudaFree(h->d_cub));
+      SVS_CK(h, cudaFree(h->d_cub));
       h->d_cub = nullptr; h->cub_bytes = 0;
-      QCK(cudaMalloc(&h->d_cub, need));
+      SVS_CK(h, cudaMalloc(&h->d_cub, need));
       h->cub_bytes = need;
     }
     k_iota<<<nblk, kGradThreads, 0, h->stream>>>(n, iota);
-    QCK(cub::DeviceRadixSort::SortPairs(h->d_cub, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
-    QCK(cudaMemsetAsync(start, 0, sizeof(int) * 2 * (size_t)cap, h->stream));   // start | end
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(h->d_cub, need, h->last.pid, keys, iota, order, n, 0, bits, h->stream));
+    SVS_CK(h, cudaMemsetAsync(start, 0, sizeof(int) * 2 * (size_t)cap, h->stream));   // start | end
     k_point_ranges<<<nblk, kGradThreads, 0, h->stream>>>(keys, n, start, end);
-    QCK(cudaGetLastError());
+    SVS_CK(h, cudaGetLastError());
     h->sorted = true;
   }
   const double* g = dL_dT;
@@ -853,14 +833,14 @@ int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_
   if (!on_device) {
     if (dL_dT) {
       memcpy(h_gctl->g, dL_dT, 6 * sizeof(double));
-      QCK(cudaMemcpyAsync(h->d_gctl->g, h_gctl->g, 6 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(h->d_gctl->g, h_gctl->g, 6 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
       g = h->d_gctl->g;
     }
     go = go ? h->d_gout : nullptr;
     gx = gx ? h->d_gout + o_xyz : nullptr;
     gcam = gcam ? h->d_gout + o_cam : nullptr;
   }
-  QCK(cudaEventRecord(h->ev0, h->stream));
+  SVS_CK(h, cudaEventRecord(h->ev0, h->stream));
   const PoseArgs& a = h->last;
   if (n > kClusterMinObs) {   // the forward's launch shapes
     cudaLaunchConfig_t cfg = {};
@@ -886,15 +866,15 @@ int svs_pose_grad(svs_pose* h, double lambda, const double dL_dT[6], double* dL_
     k_pose_grad_points<<<(unsigned)((np + kGradThreads - 1) / kGradThreads), kGradThreads, 0, h->stream>>>(
         order, start, end, h->d_q, np, h->d_gctl, gx);
   if (gcam) k_pose_grad_cam<<<1, kGradThreads, 0, h->stream>>>(h->d_c, n, h->d_gctl, gcam);
-  QCK(cudaGetLastError());
-  QCK(cudaEventRecord(h->ev1, h->stream));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaEventRecord(h->ev1, h->stream));
   if (!on_device) {
-    if (go) QCK(cudaMemcpyAsync(h->h_gout, go, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
-    if (gx) QCK(cudaMemcpyAsync(h->h_gout + o_xyz, gx, sizeof(double) * 3 * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
-    if (gcam) QCK(cudaMemcpyAsync(h->h_gout + o_cam, gcam, sizeof(double) * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (go) SVS_CK(h, cudaMemcpyAsync(h->h_gout, go, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToHost, h->stream));
+    if (gx) SVS_CK(h, cudaMemcpyAsync(h->h_gout + o_xyz, gx, sizeof(double) * 3 * (size_t)np, cudaMemcpyDeviceToHost, h->stream));
+    if (gcam) SVS_CK(h, cudaMemcpyAsync(h->h_gout + o_cam, gcam, sizeof(double) * 4, cudaMemcpyDeviceToHost, h->stream));
   }
-  QCK(cudaMemcpyAsync(h_gctl, h->d_gctl, sizeof(PoseGradCtl), cudaMemcpyDeviceToHost, h->stream));
-  QCK(cudaStreamSynchronize(h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h_gctl, h->d_gctl, sizeof(PoseGradCtl), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (!on_device) {
     if (dL_dobs) memcpy(dL_dobs, h->h_gout, sizeof(double) * 3 * (size_t)n);
     if (dL_dxyz) memcpy(dL_dxyz, h->h_gout + o_xyz, sizeof(double) * 3 * (size_t)np);

@@ -15,6 +15,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
+#include "handle.cuh"
 
 namespace {
 
@@ -71,36 +72,25 @@ __global__ void k_deriv(const float* __restrict__ src, int stride, int w, int h,
 
 }  // namespace
 
-struct svs_prep {
-  int device = 0;
-  cudaStream_t stream = nullptr;
-  std::string err;
+struct svs_prep : svs::Handle {
   int nlevels = 0, w[kMaxLv] = {}, h[kMaxLv] = {}, pitch8[kMaxLv] = {}, stride32[kMaxLv] = {};
   unsigned char* u8[kMaxLv] = {};
   float* f32[kMaxLv][3] = {};   // image, dx, dy
   unsigned char* stage = nullptr;
 };
 
-#define PCK(call)                                                       \
-  do {                                                                  \
-    cudaError_t e_ = (call);                                            \
-    if (e_ != cudaSuccess) {                                            \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);      \
-      return SVS_ERR_CUDA;                                              \
-    }                                                                   \
-  } while (0)
-
 extern "C" {
 
 int svs_prep_create(int device, int w, int hgt, int nlevels, svs_prep** out) {
   if (!out || w <= 0 || hgt <= 0 || nlevels <= 0 || nlevels > kMaxLv) return SVS_ERR_INVALID;
   *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) return SVS_ERR_NOGPU;
   svs_prep* h = new svs_prep();
-  if (device < 0) cudaGetDevice(&device);
-  h->device = device; h->nlevels = nlevels;
-  bool ok = cudaSetDevice(device) == cudaSuccess && cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) == cudaSuccess;
+  if (int rc = svs::open_handle(h, device)) {
+    delete h;
+    return rc;
+  }
+  h->nlevels = nlevels;
+  bool ok = true;
   for (int l = 0; ok && l < nlevels; ++l) {
     h->w[l] = l ? (h->w[l - 1] + 1) / 2 : w;
     h->h[l] = l ? (h->h[l - 1] + 1) / 2 : hgt;
@@ -117,22 +107,20 @@ int svs_prep_create(int device, int w, int hgt, int nlevels, svs_prep** out) {
 
 void svs_prep_destroy(svs_prep* h) {
   if (!h) return;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
+  svs::begin_close(h);
   for (int l = 0; l < kMaxLv; ++l) { cudaFree(h->u8[l]); for (int k = 0; k < 3; ++k) cudaFree(h->f32[l][k]); }
   if (h->stage) cudaFreeHost(h->stage);
-  if (h->stream) cudaStreamDestroy(h->stream);
   delete h;
 }
 
-const char* svs_prep_last_error(const svs_prep* h) { return h ? h->err.c_str() : "null handle"; }
+const char* svs_prep_last_error(const svs_prep* h) { return svs::last_error(h); }
 
 int svs_prep_process(svs_prep* h, const unsigned char* img, int pitch) {
   if (!h || !img || pitch < h->w[0]) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  PCK(cudaStreamSynchronize(h->stream));   // staging buffer reuse
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // staging buffer reuse
   for (int y = 0; y < h->h[0]; ++y) memcpy(h->stage + (size_t)y * h->w[0], img + (size_t)y * pitch, h->w[0]);
-  PCK(cudaMemcpy2DAsync(h->u8[0], h->pitch8[0], h->stage, h->w[0], h->w[0], h->h[0], cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpy2DAsync(h->u8[0], h->pitch8[0], h->stage, h->w[0], h->w[0], h->h[0], cudaMemcpyHostToDevice, h->stream));
   const dim3 blk(32, 8);
   auto grid = [&](int w, int hh) { return dim3((w + 31) / 32, (hh + 7) / 8); };
   k_u8_to_f32<<<grid(h->w[0], h->h[0]), blk, 0, h->stream>>>(h->u8[0], h->pitch8[0], h->f32[0][0], h->stride32[0], h->w[0], h->h[0]);
@@ -144,8 +132,8 @@ int svs_prep_process(svs_prep* h, const unsigned char* img, int pitch) {
     }
     k_deriv<<<grid(h->w[l], h->h[l]), blk, 0, h->stream>>>(h->f32[l][0], h->stride32[l], h->w[l], h->h[l], h->f32[l][1], h->f32[l][2]);
   }
-  PCK(cudaGetLastError());
-  PCK(cudaStreamSynchronize(h->stream));   // consumers run on their own streams
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));   // consumers run on their own streams
   return SVS_OK;
 }
 
@@ -166,15 +154,15 @@ int svs_prep_level(svs_prep* h, int level, int* w, int* hgt, const unsigned char
 int svs_prep_get_u8(svs_prep* h, int level, unsigned char* out) {
   if (!h || level < 0 || level >= h->nlevels || !out) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  PCK(cudaMemcpy2D(out, h->w[level], h->u8[level], h->pitch8[level], h->w[level], h->h[level], cudaMemcpyDeviceToHost));
+  SVS_CK(h, cudaMemcpy2D(out, h->w[level], h->u8[level], h->pitch8[level], h->w[level], h->h[level], cudaMemcpyDeviceToHost));
   return SVS_OK;
 }
 
 int svs_prep_get_f32(svs_prep* h, int level, int which, float* out) {
   if (!h || level < 0 || level >= h->nlevels || which < 0 || which > 2 || !out) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);
-  PCK(cudaMemcpy2D(out, sizeof(float) * h->w[level], h->f32[level][which], sizeof(float) * h->stride32[level],
-                   sizeof(float) * h->w[level], h->h[level], cudaMemcpyDeviceToHost));
+  SVS_CK(h, cudaMemcpy2D(out, sizeof(float) * h->w[level], h->f32[level][which], sizeof(float) * h->stride32[level],
+                         sizeof(float) * h->w[level], h->h[level], cudaMemcpyDeviceToHost));
   return SVS_OK;
 }
 
