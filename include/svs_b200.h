@@ -684,6 +684,40 @@ int svs_dt_swap_prev_cur(svs_dt *h);
 int svs_matcher_set_pyramid_device(svs_matcher *h, int which, const double T_me_from_w[7],
                                    const unsigned char *const *d_pyr, const int *pitch);
 
+/* ------------------------------------------------------------------ stereo disparity */
+
+typedef struct svs_stereo svs_stereo;
+/* calcDisparityCpu (stereo_frontend.cpp:620-653) and method 1 of calcDisparityGpu (:539-565): cv::StereoBM with the
+ * reference's settings -- preFilterCap 31 (x-Sobel pre-filter), SADWindowSize 7, minDisparity 0, textureThreshold 10,
+ * uniquenessRatio 15, speckleWindowSize 100, speckleRange 32, disp12MaxDiff 1 -- and numberOfDisparities =
+ * num_disparities (16 * ui.num_disp16: a multiple of 16 in 16..160, else SVS_ERR_INVALID).  The result is
+ * frame_data_->disp: float, the 1/16-px fixed-point disparity / 16, -1 where a stage filtered the pixel.  It equals
+ * OpenCV 4.x's StereoBM bit for bit, including its invalid border (x < num_disparities + 2, x >= w - 3, three rows top
+ * and bottom).  An image at most num_disparities + 5 wide, or at most 6 rows high, has no valid pixel: the map is all
+ * -1 (OpenCV returns -1 up to num_disparities - 1 columns and leaves wider such maps unwritten).
+ * Deviations from the reference: it links OpenCV 2.4.2; whether 2.4's StereoBM differs from 4.x's is not verified.
+ * The default of the reference's CUDA build, method 2 (cv::gpu::StereoBM_GPU: another algorithm, integer output, 0 for
+ * invalid), methods 3 and 4 (BP, CSBP) and the color_disp visualisation are not provided.
+ * Buffers are sized at create for w x height; w and height above 65535, or w * height of 2^31 or more, are
+ * SVS_ERR_INVALID. */
+int svs_stereo_create(int device, int w, int height, int num_disparities, svs_stereo **out);
+void svs_stereo_destroy(svs_stereo *h);
+const char *svs_stereo_last_error(const svs_stereo *h);
+/* left = cur_left().pyr_uint8[0], right = right.uint8 (uint8, w x height, `pitch` bytes per row).  *_on_device != 0:
+ * the image is device memory of the handle's device (e.g. svs_prep_level 0), else SVS_ERR_INVALID; so is a pitch
+ * smaller than w.  A refused call keeps the previous map.  Returns when the map is complete. */
+int svs_stereo_compute(svs_stereo *h, const unsigned char *left, int left_pitch, int left_on_device,
+                       const unsigned char *right, int right_pitch, int right_on_device);
+/* the map on the device: *d_disp with *stride_floats floats per row; valid until the next compute or destroy */
+int svs_stereo_disparity(svs_stereo *h, const float **d_disp, int *stride_floats);
+int svs_stereo_get(svs_stereo *h, float *out);   /* w*height, tightly packed */
+/* device-to-device hand-over of a level-0 disparity map into the consumers (the host setters stay as they are).
+ * The map must be device memory of the consumer's device, else SVS_ERR_INVALID and the consumer keeps its map.  Each
+ * returns when the copy is done, so the source may then change. */
+int svs_dt_set_disparity_device(svs_dt *h, const float *d_disp, int stride_floats, int w, int height);
+int svs_dtc_set_disparity_device(svs_dtc *h, const float *d_disp, int stride_floats);
+int svs_matcher_set_disparity_device(svs_matcher *h, const float *d_disp, int pitch_floats);
+
 /* ------------------------------------------------------------------ motion-only pose refinement
  * ("next" row, SURVEY.md 8f-1).  BA_SE3_XYZ_STEREO::calcFastMotionOnly (pose_optimizer.h:135-298) with
  * SE3XYZ_STEREO (transformations.h:414-460): 6-DoF Levenberg-Marquardt over fixed 3-D points with the

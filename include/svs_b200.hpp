@@ -285,6 +285,10 @@ class DenseTracker {
     memcpy(T, T_cur_from_actkey.q, 32); memcpy(T + 4, T_cur_from_actkey.t, 24);
     return ok_ && svs_dt_compute_point_cloud(h_, T, level_cams) == SVS_OK;
   }
+  // frame_data_->gpu_disp_32f from a map on the device (StereoBM::disparityDevice)
+  bool setDisparityDevice(const float* d_disp, int stride_floats, int w, int h) {
+    return ok_ && svs_dt_set_disparity_device(h_, d_disp, stride_floats, w, h) == SVS_OK;
+  }
   // GpuTracker::residualImage of one level at T_cur_from_prev (dev_residual_img[l], dense_tracking.cpp:180-188):
   // res_rgba receives w_l * h_l float4
   bool residualImage(int level, const SE3d& T_cur_from_prev, std::vector<float>* res_rgba, int w_l, int h_l) {
@@ -313,6 +317,10 @@ class DenseTrackerCpuVariant {
     const double t7[7] = {T.q[0], T.q[1], T.q[2], T.q[3], T.t[0], T.t[1], T.t[2]};
     return ok_ && svs_computeDensePointCloudCpu(h_, t7, cam_vec.data()) == SVS_OK;
   }
+  // frame_data_->disp from a map on the device (StereoBM::disparityDevice)
+  bool setDisparityDevice(const float* d_disp, int stride_floats) {
+    return ok_ && svs_dtc_set_disparity_device(h_, d_disp, stride_floats) == SVS_OK;
+  }
   // denseTrackingCpu(&T_cur_from_actkey)
   bool denseTrackingCpu(SE3d* T, const std::vector<svs_cam>& cam_vec, svs_dt_stats* stats = nullptr) {
     double t7[7] = {T->q[0], T->q[1], T->q[2], T->q[3], T->t[0], T->t[1], T->t[2]};
@@ -340,6 +348,10 @@ class GuidedMatcher {
   GuidedMatcher& operator=(const GuidedMatcher&) = delete;
   bool valid() const { return ok_; }
   svs_matcher* handle() { return h_; }
+  // cur_frame.disp from a map on the device (StereoBM::disparityDevice)
+  bool setCurrentDisparityDevice(const float* d_disp, int pitch_floats) {
+    return ok_ && svs_matcher_set_disparity_device(h_, d_disp, pitch_floats) == SVS_OK;
+  }
   // feature_tree of one pyramid level = the corners FastGrid::detect* left on the device
   bool setFeatureTree(int level, FastGrid& fast_grid) { return ok_ && svs_matcher_set_features_from_fast(h_, level, fast_grid.handle()) == SVS_OK; }
   // match(keyframe_map, T_cur_from_actkey, cur_frame, feature_tree, cam_vec, actkey_id, vertex_map, ap_map,
@@ -497,6 +509,33 @@ class FramePreprocessor {
 
  private:
   svs_prep* h_ = nullptr;
+  bool ok_ = false;
+};
+
+// StereoFrontend::calcDisparityCpu (stereo_frontend.cpp:620-653): cv::StereoBM with the reference's settings, the
+// map kept on the device (svs_stereo_* in svs_b200.h states the semantics)
+class StereoBM {
+ public:
+  StereoBM(int w, int h, int num_disparities = 32) { ok_ = svs_stereo_create(-1, w, h, num_disparities, &h_) == SVS_OK; }
+  ~StereoBM() { if (h_) svs_stereo_destroy(h_); }
+  StereoBM(const StereoBM&) = delete;
+  StereoBM& operator=(const StereoBM&) = delete;
+  bool valid() const { return ok_; }
+  svs_stereo* handle() { return h_; }
+  // left / right uint8 images; *_on_device: the image is device memory (e.g. FramePreprocessor level 0)
+  bool calcDisparity(const unsigned char* left, int left_pitch, const unsigned char* right, int right_pitch,
+                     bool left_on_device = false, bool right_on_device = false) {
+    return ok_ && svs_stereo_compute(h_, left, left_pitch, left_on_device, right, right_pitch, right_on_device) == SVS_OK;
+  }
+  // the map on the device, for DenseTracker / DenseTrackerCpuVariant / GuidedMatcher ::set*DisparityDevice
+  bool disparityDevice(const float** d_disp, int* stride_floats) {
+    return ok_ && svs_stereo_disparity(h_, d_disp, stride_floats) == SVS_OK;
+  }
+  bool disparity(float* out) { return ok_ && svs_stereo_get(h_, out) == SVS_OK; }   // w*h, tightly packed
+  const char* last_error() const { return svs_stereo_last_error(h_); }
+
+ private:
+  svs_stereo* h_ = nullptr;
   bool ok_ = false;
 };
 

@@ -245,6 +245,8 @@ EXPORTS = [
     "svs_place_last_words", "svs_place_last_scores", "svs_place_last_matches", "svs_place_last_hypotheses",
     "svs_globalLoopClosure", "svs_localRegisterFrame",
     "svs_match_track", "svs_processMatchedPoints", "svs_shallWeDropNewKeyframe", "svs_addMorePoints",
+    "svs_stereo_create", "svs_stereo_destroy", "svs_stereo_last_error", "svs_stereo_compute", "svs_stereo_disparity",
+    "svs_stereo_get", "svs_dt_set_disparity_device", "svs_dtc_set_disparity_device", "svs_matcher_set_disparity_device",
 ]
 
 
@@ -266,7 +268,8 @@ def lib():
         raise RuntimeError(f"{LIB_PATH} missing: run `python -c 'import __graft_entry__ as g; g.build()'`")
     L = C.CDLL(LIB_PATH)
     vp = C.c_void_p
-    for prefix in ("ba", "chol6", "fast", "dt", "dtc", "prep", "matcher", "pose", "place", "map", "constraints"):
+    for prefix in ("ba", "chol6", "fast", "dt", "dtc", "prep", "matcher", "pose", "place", "map", "constraints",
+                   "stereo"):
         destroy = getattr(L, f"svs_{prefix}_destroy")
         destroy.argtypes, destroy.restype = [vp], None
         last_error = getattr(L, "svs_last_error" if prefix == "ba" else f"svs_{prefix}_last_error")
@@ -341,6 +344,13 @@ def lib():
     L.svs_dt_set_images_device.argtypes = [vp, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
     L.svs_dt_swap_prev_cur.argtypes = [vp]
     L.svs_matcher_set_pyramid_device.argtypes = [vp, C.c_int, c_dp, C.POINTER(C.c_void_p), c_ip]
+    L.svs_stereo_create.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]
+    L.svs_stereo_compute.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int, C.c_int]
+    L.svs_stereo_disparity.argtypes = [vp, pvp, c_ip]
+    L.svs_stereo_get.argtypes = [vp, c_fp]
+    L.svs_dt_set_disparity_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int]
+    L.svs_dtc_set_disparity_device.argtypes = [vp, vp, C.c_int]
+    L.svs_matcher_set_disparity_device.argtypes = [vp, vp, C.c_int]
     L.svs_map_create.argtypes = [C.c_int, C.POINTER(vp)]
     L.svs_map_set.argtypes = [vp, C.c_int, c_dp, C.c_int, c_ip, c_dp, c_ip, c_ip, c_dp, c_ip]
     L.svs_map_update_poses.argtypes = [vp, C.c_int, c_ip, c_dp]
@@ -914,6 +924,11 @@ class DenseTracker(_Handle):
         d = np.ascontiguousarray(disp, np.float32)
         self._ck(lib().svs_dt_set_disparity(self._h, self._fp(d), d.shape[1], d.shape[1], d.shape[0]))
 
+    def set_disparity_device(self, ptr, stride, w=None, h=None):
+        """The level-0 map from device memory, e.g. StereoMatcher.device_disparity(); (w, h) default to the frame's."""
+        self._ck(lib().svs_dt_set_disparity_device(self._h, ptr, stride, self.w0 if w is None else w,
+                                                   self.h0 if h is None else h))
+
     def compute_point_cloud(self, T, cams):
         arr = (SvsCam * len(cams))(*[SvsCam(*map(float, c)) for c in cams])
         T = np.ascontiguousarray(T, np.float64)
@@ -989,6 +1004,10 @@ class GuidedMatcher(_Handle):
     def set_current_disparity(self, disp):
         d = np.ascontiguousarray(disp, np.float32)
         self._ck(lib().svs_matcher_set_current(self._h, None, None, d.ctypes.data_as(C.POINTER(C.c_float)), d.shape[1]))
+
+    def set_current_disparity_device(self, ptr, pitch):
+        """cur_frame.disp from device memory, e.g. StereoMatcher.device_disparity()."""
+        self._ck(lib().svs_matcher_set_disparity_device(self._h, ptr, pitch))
 
     def set_pyramid_device(self, which, ptrs, pitches, T_me_from_w=None):
         """which = -1: current frame, >= 0: keyframe slot (needs T_me_from_w); device pointers per level."""
@@ -1114,6 +1133,54 @@ class FramePreprocessor(_Handle):
         lv = self.level(l)
         out = np.zeros((lv["h"], lv["w"]), np.float32)
         self._ck(lib().svs_prep_get_f32(self._h, l, which, out.ctypes.data_as(C.POINTER(C.c_float))))
+        return out
+
+
+class StereoMatcher(_Handle):
+    """StereoFrontend::calcDisparityCpu (reference stereo_frontend.cpp:620-653): cv::StereoBM with the reference's
+    settings on the device, bit for bit OpenCV 4.x's output (svs_stereo_* in svs_b200.h).  The map stays on the GPU
+    for the tracker and the matcher; disparity() reads it back."""
+
+    _destroy, _last_error = "svs_stereo_destroy", "svs_stereo_last_error"
+
+    def __init__(self, w, h, num_disparities=32, device=-1):
+        self._open("svs_stereo_create", device, w, h, num_disparities)
+        self.w, self.h, self.num_disparities = w, h, num_disparities
+
+    def _image(self, img):
+        """(pointer, pitch, on_device, keep-alive) of an (h, w) uint8 image: a numpy array (host), a
+        FramePreprocessor.level() dict or a CUDA torch tensor (device)."""
+        if isinstance(img, dict):
+            if (img["w"], img["h"]) != (self.w, self.h):
+                raise SvsError(-1, f"a {img['w']}x{img['h']} level for a {self.w}x{self.h} stereo handle")
+            return img["u8"], img["pitch_u8"], 1, None
+        if _is_torch_tensor(img) and img.is_cuda:
+            import torch
+            if img.dtype != torch.uint8 or tuple(img.shape) != (self.h, self.w) or img.stride(1) != 1:
+                raise SvsError(-1, f"a device image must be a ({self.h}, {self.w}) torch.uint8 tensor with unit column "
+                                   f"stride, not {img.dtype} {tuple(img.shape)}")
+            torch.cuda.current_stream(img.device).synchronize()   # the handle reads the image on its own stream
+            return img.data_ptr(), img.stride(0), 1, img
+        a = np.ascontiguousarray(img)
+        if a.dtype != np.uint8 or a.shape != (self.h, self.w):
+            raise SvsError(-1, f"a host image must be a ({self.h}, {self.w}) uint8 array, not {a.dtype} {a.shape}")
+        return a.ctypes.data, a.strides[0], 0, a
+
+    def compute(self, left, right):
+        """left / right: (h, w) uint8 numpy arrays, or device images (FramePreprocessor.level(0), CUDA tensors)."""
+        lp, lpitch, ldev, lkeep = self._image(left)
+        rp, rpitch, rdev, rkeep = self._image(right)
+        self._ck(lib().svs_stereo_compute(self._h, lp, lpitch, ldev, rp, rpitch, rdev))
+
+    def device_disparity(self):
+        """(device pointer, floats per row) of the last map."""
+        p, s = C.c_void_p(), C.c_int()
+        self._ck(lib().svs_stereo_disparity(self._h, C.byref(p), C.byref(s)))
+        return p.value, s.value
+
+    def disparity(self):
+        out = np.empty((self.h, self.w), np.float32)
+        self._ck(lib().svs_stereo_get(self._h, out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
 
 
@@ -1247,6 +1314,10 @@ class DenseTrackerCpuVariant(_Handle):
     def set_disparity(self, disp):
         d = np.ascontiguousarray(disp, np.float32)
         self._ck(lib().svs_dtc_set_disparity(self._h, d.ctypes.data_as(C.POINTER(C.c_float)), d.shape[1]))
+
+    def set_disparity_device(self, ptr, stride):
+        """frame_data_->disp from device memory, e.g. StereoMatcher.device_disparity()."""
+        self._ck(lib().svs_dtc_set_disparity_device(self._h, ptr, stride))
 
     def compute_point_cloud(self, T, cams):
         T = np.ascontiguousarray(T, np.float64)

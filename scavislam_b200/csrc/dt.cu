@@ -683,6 +683,18 @@ int svs_dt_set_disparity(svs_dt* h, const float* disp, int stride_floats, int w,
   return upload_plane(h, h->disp, h->disp_stride, disp, stride_floats, w, hgt);
 }
 
+// the same map already on this device (svs_stereo_disparity): a device-to-device copy; on return the source may change
+int svs_dt_set_disparity_device(svs_dt* h, const float* d_disp, int stride_floats, int w, int hgt) {
+  if (!h || !d_disp || w <= 0 || hgt <= 0 || w > h->w0 || hgt > h->h0 || stride_floats < w) return SVS_ERR_INVALID;
+  if (!svs::on_device(h->device, d_disp)) return svs::fail(h, SVS_ERR_INVALID, "svs_dt_set_disparity_device: not device memory of this handle's device");
+  cudaSetDevice(h->device);
+  SVS_CK(h, cudaMemcpy2DAsync(h->disp, sizeof(float) * h->disp_stride, d_disp, sizeof(float) * stride_floats, sizeof(float) * w, hgt,
+                              cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  h->disp_w = w; h->disp_h = hgt;
+  return SVS_OK;
+}
+
 int svs_dt_set_point_cloud(svs_dt* h, int level, const float* cloud_xyzw) {
   if (!h || level < 0 || level >= h->nlevels || !cloud_xyzw) return SVS_ERR_INVALID;
   cudaSetDevice(h->device);

@@ -339,6 +339,17 @@ int svs_dtc_set_disparity(svs_dtc* h, const float* disp, int stride_floats) {
   return SVS_OK;
 }
 
+// the same map already on this device (svs_stereo_disparity): a device-to-device copy; on return the source may change
+int svs_dtc_set_disparity_device(svs_dtc* h, const float* d_disp, int stride_floats) {
+  if (!h || !d_disp || stride_floats < h->w0) return SVS_ERR_INVALID;
+  if (!svs::on_device(h->device, d_disp)) return svs::fail(h, SVS_ERR_INVALID, "svs_dtc_set_disparity_device: not device memory of this handle's device");
+  cudaSetDevice(h->device);
+  SVS_CK(h, cudaMemcpy2DAsync(h->disp, sizeof(float) * h->disp_stride, d_disp, sizeof(float) * stride_floats, sizeof(float) * h->w0,
+                              h->h0, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  return SVS_OK;
+}
+
 int svs_computeDensePointCloudCpu(svs_dtc* h, const double T[7], const svs_cam* cams) {
   svs::NvtxRange nvtx_("dense point cloud");
   if (!h || !T || !cams) return SVS_ERR_INVALID;

@@ -443,6 +443,17 @@ int svs_matcher_set_current(svs_matcher * h, const unsigned char* const* pyr, co
   return SVS_OK;
 }
 
+// cur_frame.disp already on this device (svs_stereo_disparity): a device-to-device copy; on return the source may change
+int svs_matcher_set_disparity_device(svs_matcher * h, const float* d_disp, int pitch_floats) {
+  if (!h || !d_disp || pitch_floats < h->lv[0].w) return SVS_ERR_INVALID;
+  if (!svs::on_device(h->device, d_disp)) return svs::fail(h, SVS_ERR_INVALID, "svs_matcher_set_disparity_device: not device memory of this handle's device");
+  cudaSetDevice(h->device);
+  SVS_CK(h, cudaMemcpy2DAsync(h->d_disp, sizeof(float) * h->disp_pitch, d_disp, sizeof(float) * pitch_floats,
+                              sizeof(float) * h->lv[0].w, h->lv[0].h, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  return SVS_OK;
+}
+
 // Same as set_keyframe / set_current, but the pyramid already lives on this device (svs_prep_level):
 // a device-to-device copy into the handle's own buffers, so a keyframe outlives the preprocessor's frame.
 int svs_matcher_set_pyramid_device(svs_matcher * h, int which, const double T_me_from_w[7], const unsigned char* const* d_pyr,

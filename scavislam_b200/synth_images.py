@@ -18,7 +18,8 @@ def _value_noise(u, v, seed, octaves=5):
         lat = rng.uniform(0, 1, (n + 1, n + 1))
         x = (u * n) % n
         y = (v * n) % n
-        x0 = np.floor(x).astype(int); y0 = np.floor(y).astype(int)
+        # (u * n) % n rounds to n for u just below a multiple of 1: keep the cell index in range (fx = 1 there)
+        x0 = np.minimum(np.floor(x).astype(int), n - 1); y0 = np.minimum(np.floor(y).astype(int), n - 1)
         fx = x - x0; fy = y - y0
         sx = fx * fx * (3 - 2 * fx); sy = fy * fy * (3 - 2 * fy)
         a = lat[y0, x0]; b = lat[y0, x0 + 1]; c = lat[y0 + 1, x0]; d = lat[y0 + 1, x0 + 1]
@@ -28,11 +29,12 @@ def _value_noise(u, v, seed, octaves=5):
     return out / tot
 
 
-def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H, cam=None):
+def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H, cam=None, noise_seed=None):
     """Render the left image (uint8) and disparity (float32) seen from camera centre t_wc (x,y,z)
     with heading yaw (rotation about the y axis).  Scene: ground plane y = 1.5 m (y down) and a far
     wall z = 25 m, plus a few boxes (fronto-parallel quads) -- all textured with value noise.
-    cam = (f, px, py, baseline) of the left camera; None is the default 640x480 camera of synth."""
+    cam = (f, px, py, baseline) of the left camera; None is the default 640x480 camera of synth.
+    noise_seed seeds the sensor noise; None is seed + 100."""
     f, px, py, b = (CAM_F, CAM_PX, CAM_PY, CAM_B) if cam is None else cam
     uu, vv = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
     dx = (uu - px) / f; dy = (vv - py) / f; dz = np.ones_like(dx)
@@ -77,10 +79,22 @@ def render_frame(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H, cam=None):
     img = np.clip(255.0 * (0.15 + 0.8 * tex), 0, 255)
     img[~np.isfinite(depth)] = 30
     # sensor noise, deterministic
-    img = img + np.random.default_rng(seed + 100).normal(0, 1.0, img.shape)
+    img = img + np.random.default_rng(seed + 100 if noise_seed is None else noise_seed).normal(0, 1.0, img.shape)
     img8 = np.clip(np.rint(img), 0, 255).astype(np.uint8)
     disp = np.where(np.isfinite(depth), f * b / np.maximum(depth, 1e-6), 0.0).astype(np.float32)
     return img8, disp
+
+
+def render_stereo_pair(t_wc, yaw, seed=77, w=CAM_W, h=CAM_H, cam=None):
+    """A rectified stereo pair: the left image and its ground-truth disparity as render_frame gives them, and the right
+    image seen from t_wc + b (cos yaw, 0, -sin yaw), the left camera's x axis.  The right image has its own sensor
+    noise (seed + 200): with the left image's noise the same at every pixel, a matcher would be flattered."""
+    f, px, py, b = (CAM_F, CAM_PX, CAM_PY, CAM_B) if cam is None else cam
+    t_wc = np.asarray(t_wc, dtype=np.float64)
+    left, disp = render_frame(t_wc, yaw, seed, w, h, cam)
+    t_r = t_wc + b * np.array([np.cos(yaw), 0.0, -np.sin(yaw)])
+    right, _ = render_frame(t_r, yaw, seed, w, h, cam, noise_seed=seed + 200)
+    return left, right, disp
 
 
 def _render_job(args):
