@@ -879,12 +879,76 @@ int svs_map_select_window(svs_map *h, int root, int inner_window_size, int doubl
  * so a pose absorbed from the optimiser never visits the host); n_new points, each anchored in an EXISTING frame and seen
  * by that frame (new_anchor_center at level 0, new_anchor_level) and by the new keyframe (new_center, new_level); n_track
  * existing points gain an observation by the new keyframe.  The observation lists are rebuilt by kernels (count, scan,
- * move); the strength bookkeeping of computeStrength / addNewEdges stays with the caller, who passes the new pose graph
- * with svs_map_set_graph.  *vertex_index = index of the new vertex, *first_new_point = index of the first new point. */
+ * move).  This call drops the pose graph: the strength bookkeeping of computeStrength / addNewEdges stays with the
+ * caller, who passes the new pose graph with svs_map_set_graph, or uses svs_map_add_keyframe_graph instead.  *vertex_index = index of the new vertex, *first_new_point = index of the first new point. */
 int svs_map_add_keyframe(svs_map *h, int oldkey, const double *T_newkey_from_oldkey, int n_new, const int *new_anchor,
                          const double *new_xyz_anchor, const double *new_anchor_center, const int *new_anchor_level,
                          const double *new_center, const int *new_level, int n_track, const int *track_point,
                          const double *track_center, const int *track_level, int *vertex_index, int *first_new_point);
+/* ------------------------------------------------------------------ the pose graph grown on the device
+ * SlamGraph::addKeyframe's computeStrength / addNewEdges (slam_graph.cpp:144-186, 424-552), registerKeyframes' METRIC
+ * edges (:189-205) and addLoopClosure's APPEARANCE edge (:208-254) on the device graph, so that no caller needs a host
+ * copy of the observation lists or a full graph upload after a keyframe, a registration or a loop.
+ *
+ * svs_map_set_pose_graph: the lists of svs_map_set_graph plus nbr_strength[nnzN], the int key of
+ *   Vertex::neighbor_ids_ordered_by_strength (Edge::strength).  Each list must be non-increasing in strength (strongest
+ *   first), else SVS_ERR_INVALID.  nbr_strength, nbr_T and nbr_Lambda are required (unless the graph has no entries):
+ *   edges created on the device store constraints computed there.  A graph set with svs_map_set_graph has no strengths; the growth calls refuse it (SVS_ERR_STATE),
+ *   as they refuse a map without a graph.
+ * svs_map_get_graph: reads the graph back: nbr_ptr[V+1], nbr_id / nbr_strength [nnzN], nbr_T [nnzN][7],
+ *   nbr_Lambda [nnzN][36]; any output may be NULL.  *nnzN is always set; SVS_ERR_INVALID when an entry array is asked
+ *   for and cap < nnzN.  A graph without strengths reads strength 0, without constraints the identity and Lambda = 0.
+ *   SVS_ERR_STATE when the map has no graph.
+ * Insertion rule (std::multimap::insert, read through rbegin): a new entry of strength s goes in front of the first
+ *   entry of the list with strength <= s.  Both directed entries of an edge (v1, v2) are inserted in that order: v2
+ *   into v1's list, then v1 into v2's.  setConstraint(v1, v2, T_1_from_2, Lambda, Lambda): v2's entry for v1 stores
+ *   T_1_from_2 (T_nbr_from_me), v1's entry for v2 stores its inverse; both store Lambda.
+ * Constraints: computeConstraint(v1, v2) as svs_computeConstraint_batch computes it, on the feature tables of the
+ *   map where it lies.  DEVIATION (as for svs_computeConstraint_batch): every anchor pose comes from the map; for an
+ *   anchor outside the double window the reference chains computeAbsolutePose along the graph.
+ *
+ * svs_map_add_keyframe_graph: the whole of SlamGraph::addKeyframe.  Arguments and refusals of svs_map_add_keyframe,
+ *   plus covis_thr (>= 1) and the level-0 image width, height.  In order, on the map's stream:
+ *   1 computeStrength (:468-552) on the map before the growth.  New point q adds 1 to new_anchor[q].  Tracked point t,
+ *     in the order given, adds 1 to every vertex of its point's observer list, and 1 to that vertex's left (else
+ *     right) count when u < (int)(width * 0.5), top (else bottom) when v < (int)(height * 0.5), (u, v) =
+ *     track_center[t].  QUIRK B15 (SURVEY Appendix B) is kept: the zeroing loop runs inside the track loop.  In closed
+ *     form: with n_track = 0 a vertex's strength is its new-point count; otherwise it is the number of tracks t >= t*
+ *     that observe it, t* the first track after which all four of its counts are present and >= covis_thr / 2
+ *     (integer division), and 0 when there is no t*.  So with any track at all, new-point counts vanish.  The table
+ *     holds every vertex a new point or a track touched, in ascending vertex order; then strength_to_oldkey =
+ *     max(strength, covis_thr).  oldkey not in the table: SVS_ERR_INVALID (the reference asserts).
+ *   2 The growth of svs_map_add_keyframe (new vertex V, new points, new observations).
+ *   3 addNewEdges(LOCAL) (:424-465): every table row with strength >= covis_thr becomes the edge (v1 = row vertex,
+ *     v2 = V) with that strength, its constraint computed on the grown map.  DEVIATION (a defined order): the
+ *     reference walks a tr1::unordered_map; here rows are inserted in ascending vertex id, which fixes the order of
+ *     equal strengths in the new vertex's list.
+ *   The graph survives with V + 1 lists.  Outputs (each may be NULL): *vertex_index, *first_new_point as for
+ *   svs_map_add_keyframe; table[*n_table][2] the rows (vertex, strength) after the oldkey bump (room for V rows, V
+ *   before the call); *n_edges the edges added.  A refused call leaves the map and its graph bit-identical.  A CUDA
+ *   error after the growth (step 3) returns SVS_ERR_CUDA with the grown map and no pose graph, as after
+ *   svs_map_add_keyframe.
+ *
+ * svs_map_add_edges: for k = 0..n-1 the edge (v1[k], v2[k]) with strength[k] is inserted into both lists, its
+ *   constraint computeConstraint(v1, v2) computed and stored by setConstraint(v1, v2, ...).  moved_vertex (or -1)
+ *   is placed at T_moved_from_w[7] while the constraints are computed, as the reference does before restoring it; its
+ *   map pose is not changed.  computeConstraint measures depths in v1's frame, so the callers pass:
+ *     registration (registerKeyframes): v1 = stats[i].vertex of each qualified row, v2 = root, moved = root at
+ *       res.T_newroot_from_w, strength = stats[i].strength;
+ *     loop (addLoopClosure): v1 = loop, v2 = query, strength = res.n_tracks, moved = loop at res.T_newloop_from_w.
+ *   Refused with SVS_ERR_INVALID, the map and its graph unchanged: an index outside [0, V), v1 == v2, an edge already
+ *   in the graph (insertEdge asserts) or listed twice, moved_vertex outside [-1, V) or without its pose. */
+int svs_map_set_pose_graph(svs_map *h, const int *nbr_ptr, const int *nbr_id, const int *nbr_strength, const double *nbr_T,
+                           const double *nbr_Lambda);
+int svs_map_get_graph(svs_map *h, int cap, int *nnzN, int *nbr_ptr, int *nbr_id, int *nbr_strength, double *nbr_T,
+                      double *nbr_Lambda);
+int svs_map_add_keyframe_graph(svs_map *h, int oldkey, const double *T_newkey_from_oldkey, int n_new, const int *new_anchor,
+                               const double *new_xyz_anchor, const double *new_anchor_center, const int *new_anchor_level,
+                               const double *new_center, const int *new_level, int n_track, const int *track_point,
+                               const double *track_center, const int *track_level, int covis_thr, int width, int height,
+                               int *vertex_index, int *first_new_point, int *n_table, int *table, int *n_edges);
+int svs_map_add_edges(svs_map *h, int n, const int *v1, const int *v2, const int *strength, int moved_vertex,
+                      const double *T_moved_from_w);
 /* the edge list of the last assembly (any output may be NULL); E must equal *num_edges */
 int svs_map_last_edges(svs_map *h, int E, int *e_point, int *e_pose, int *e_anchor, double *e_obs, double *e_info);
 
@@ -917,7 +981,7 @@ int svs_map_last_edges(svs_map *h, int E, int *e_point, int *e_pose, int *e_anch
  *     its ascending-vertex position in the point's list; where loop already observes the point its observation stays
  *     (std::map::insert), the track is still listed and counted.  Like svs_map_add_keyframe this forgets the last
  *     assembled window; the pose graph stays (V is unchanged).  The neighbour lists, the edge and the loop constraint
- *     stay with the caller (svs_computeConstraint_batch with loop placed at T_newloop_from_w, INTEGRATION.md).
+ *     are one svs_map_add_edges call (v1 = loop, v2 = query, moved = loop at T_newloop_from_w, INTEGRATION.md).
  *   Output.  res: the counts of every stage reached; tracks: track_point / track_uvu [.][3] / track_level, in match
  *     order, whenever the gate ran (cap >= n_candidates always suffices).  Returns SVS_OK whether or not the loop
  *     was verified.  Device-side findings come back through one control word; the host reads counts, poses and
@@ -975,8 +1039,8 @@ int svs_globalLoopClosure(svs_map *map, svs_matcher *m, svs_pose *po, const svs_
  *     observation of root (uvu at level 0, anchor_level) at its ascending-vertex position, once per point; where root
  *     already observes the point its observation stays.  Root's map pose is not changed (the reference restores it);
  *     T_newroot_from_w = T_newroot_from_oldroot * T_root_from_w is returned.  Like svs_map_add_keyframe this forgets
- *     the last assembled window; the pose graph stays.  addNewEdges stays with the caller: the neighbour lists, the
- *     METRIC edges and each constraint with root placed at T_newroot_from_w (INTEGRATION.md).
+ *     the last assembled window; the pose graph stays.  addNewEdges is one svs_map_add_edges call: v1 = each
+ *     qualified stats vertex, v2 = root, moved = root at T_newroot_from_w (INTEGRATION.md).
  *   Output.  res: the counts of every stage reached.  stats[n_stats]: one row per counted vertex in ascending vertex
  *     order (the reference's ImageStatsTable order is unspecified).  tracks: track_point / track_uvu [.][3] /
  *     track_level / track_committed, in match order (the reference's trackpoint-list order is unspecified), whenever

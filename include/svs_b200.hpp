@@ -698,6 +698,60 @@ class DeviceMap {
     V_ += 1; Np_ += (int)new_anchor.size(); nn_ = 0;
     return v;
   }
+  // the pose graph with strengths and constraints (svs_map_set_pose_graph): what the growth calls below extend
+  struct PoseGraph { std::vector<int> nbr_ptr, nbr_id, nbr_strength; std::vector<double> nbr_T, nbr_Lambda; };
+  bool setPoseGraph(const PoseGraph& g) {
+    if (!ok_ || svs_map_set_pose_graph(h_, g.nbr_ptr.data(), g.nbr_id.data(), g.nbr_strength.data(), g.nbr_T.data(),
+                                       g.nbr_Lambda.data()) != SVS_OK)
+      return false;
+    nn_ = (int)g.nbr_id.size();
+    return true;
+  }
+  // the pose graph as it lies on the device (svs_map_get_graph)
+  bool poseGraph(PoseGraph* g) {
+    int nn = 0;
+    if (!ok_ || svs_map_get_graph(h_, 0, &nn, nullptr, nullptr, nullptr, nullptr, nullptr) != SVS_OK) return false;
+    const size_t cap = nn > 0 ? (size_t)nn : 1;
+    g->nbr_ptr.resize((size_t)V_ + 1); g->nbr_id.resize(cap); g->nbr_strength.resize(cap);
+    g->nbr_T.resize(7 * cap); g->nbr_Lambda.resize(36 * cap);
+    if (svs_map_get_graph(h_, nn, &nn, g->nbr_ptr.data(), g->nbr_id.data(), g->nbr_strength.data(), g->nbr_T.data(),
+                          g->nbr_Lambda.data()) != SVS_OK)
+      return false;
+    g->nbr_id.resize(nn); g->nbr_strength.resize(nn); g->nbr_T.resize(7 * (size_t)nn); g->nbr_Lambda.resize(36 * (size_t)nn);
+    return true;
+  }
+  // the whole of addKeyframe (slam_graph.cpp:144-186) with computeStrength and addNewEdges(LOCAL) on the device graph
+  // (svs_map_add_keyframe_graph); `table` (may be NULL) receives the (vertex, strength) rows.  Returns the index of the
+  // new vertex, < 0 on error.
+  int addKeyframe(int oldkey_id, const double T_newkey_from_oldkey[7], const std::vector<int>& new_anchor,
+                  const std::vector<double>& new_xyz_anchor, const std::vector<double>& new_anchor_center,
+                  const std::vector<int>& new_anchor_level, const std::vector<double>& new_center, const std::vector<int>& new_level,
+                  const std::vector<int>& track_point, const std::vector<double>& track_center, const std::vector<int>& track_level,
+                  int covis_thr, int width, int height, std::vector<int>* table = nullptr, int* n_edges = nullptr) {
+    if (!ok_) return SVS_ERR_NOGPU;
+    int v = -1, q = -1, nt = 0, ne = 0;
+    std::vector<int> rows(2 * (size_t)(V_ > 0 ? V_ : 1));
+    const int rc = svs_map_add_keyframe_graph(h_, oldkey_id, T_newkey_from_oldkey, (int)new_anchor.size(), new_anchor.data(),
+                                              new_xyz_anchor.data(), new_anchor_center.data(), new_anchor_level.data(),
+                                              new_center.data(), new_level.data(), (int)track_point.size(), track_point.data(),
+                                              track_center.data(), track_level.data(), covis_thr, width, height, &v, &q, &nt,
+                                              rows.data(), &ne);
+    if (rc != SVS_OK) return rc;
+    V_ += 1; Np_ += (int)new_anchor.size(); nn_ += 2 * ne;
+    if (table) table->assign(rows.begin(), rows.begin() + 2 * (size_t)nt);
+    if (n_edges) *n_edges = ne;
+    return v;
+  }
+  // registerKeyframes' METRIC edges and addLoopClosure's APPEARANCE edge (svs_map_add_edges): (v1[k], v2[k]) with
+  // strength[k], computeConstraint(v1, v2) with moved_vertex (or -1) placed at T_moved_from_w
+  bool addEdges(const std::vector<int>& v1, const std::vector<int>& v2, const std::vector<int>& strength, int moved_vertex = -1,
+                const double* T_moved_from_w = nullptr) {
+    if (!ok_ || v1.size() != v2.size() || v1.size() != strength.size()) return false;
+    if (svs_map_add_edges(h_, (int)v1.size(), v1.data(), v2.data(), strength.data(), moved_vertex, T_moved_from_w) != SVS_OK)
+      return false;
+    nn_ += 2 * (int)v1.size();
+    return true;
+  }
   // Backend::globalLoopClosure (backend.cpp:830-1001) on this map; semantics: svs_globalLoopClosure.  The matcher holds
   // the loop keyframe as its current frame and the keyframe pyramids in the slots vertex_slot names.  Returns true when
   // the loop was verified and the map grew; *res (when given) holds the counts of every stage reached, *tracks the gated

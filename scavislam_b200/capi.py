@@ -236,7 +236,7 @@ EXPORTS = [
     "svs_constraints_create", "svs_constraints_destroy", "svs_constraints_last_error", "svs_computeConstraint_batch",
     "svs_map_create", "svs_map_destroy", "svs_map_last_error", "svs_map_set", "svs_map_update_poses",
     "svs_map_update_points", "svs_map_get", "svs_map_absorb", "svs_map_set_graph", "svs_map_select_window",
-    "svs_map_add_keyframe",
+    "svs_map_add_keyframe", "svs_map_set_pose_graph", "svs_map_get_graph", "svs_map_add_keyframe_graph", "svs_map_add_edges",
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
@@ -362,6 +362,11 @@ def lib():
                                         c_ip, c_ip, c_dp, c_dp]
     L.svs_map_add_keyframe.argtypes = [vp, C.c_int, c_dp, C.c_int, c_ip, c_dp, c_dp, c_ip, c_dp, c_ip, C.c_int, c_ip, c_dp, c_ip,
                                        c_ip, c_ip]
+    L.svs_map_set_pose_graph.argtypes = [vp, c_ip, c_ip, c_ip, c_dp, c_dp]
+    L.svs_map_get_graph.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, c_ip, c_dp, c_dp]
+    L.svs_map_add_keyframe_graph.argtypes = [vp, C.c_int, c_dp, C.c_int, c_ip, c_dp, c_dp, c_ip, c_dp, c_ip, C.c_int, c_ip, c_dp,
+                                             c_ip, C.c_int, C.c_int, C.c_int, c_ip, c_ip, c_ip, c_ip, c_ip]
+    L.svs_map_add_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, C.c_int, c_dp]
     L.svs_ba_set_problem_from_map.argtypes = [vp, vp, C.c_int, c_ip, c_up, C.c_int, c_ip, C.c_int, c_ip, c_ip, c_dp, c_dp,
                                               C.POINTER(SvsCam), c_ip]
     L.svs_map_last_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp]
@@ -1425,9 +1430,9 @@ class DeviceMap(_Handle):
         return dict(window_vertex=win[:P].copy(), inner=inner[:P].copy(), active_point=act[:L].copy(), c_i=ci[:Cn].copy(),
                     c_j=cj[:Cn].copy(), c_T=cT[:Cn].copy(), c_Lambda=cL[:Cn].copy())
 
-    def add_keyframe(self, oldkey, T_newkey_from_oldkey, new_anchor=(), new_xyz=None, new_anchor_center=None,
-                     new_anchor_level=(), new_center=None, new_level=(), track_point=(), track_center=None, track_level=()):
-        """SlamGraph::addKeyframe on the device tables.  Returns (index of the new vertex, index of the first new point)."""
+    @staticmethod
+    def _keyframe_args(T_newkey_from_oldkey, new_anchor, new_xyz, new_anchor_center, new_anchor_level, new_center, new_level,
+                       track_point, track_center, track_level):
         T = np.ascontiguousarray(T_newkey_from_oldkey, np.float64).reshape(7)
         na = np.ascontiguousarray(new_anchor, np.int32)
         d3 = lambda a, n: np.zeros((n, 3)) if a is None else np.ascontiguousarray(a, np.float64).reshape(n, 3)
@@ -1435,12 +1440,68 @@ class DeviceMap(_Handle):
         nal, nl = np.ascontiguousarray(new_anchor_level, np.int32), np.ascontiguousarray(new_level, np.int32)
         tp = np.ascontiguousarray(track_point, np.int32)
         tc, tl = d3(track_center, len(tp)), np.ascontiguousarray(track_level, np.int32)
+        keep = (T, na, nx, nac, nal, nc, nl, tp, tc, tl)
+        return keep, [_dp(T), len(na), _ip(na), _dp(nx), _dp(nac), _ip(nal), _dp(nc), _ip(nl), len(tp), _ip(tp), _dp(tc), _ip(tl)]
+
+    def add_keyframe(self, oldkey, T_newkey_from_oldkey, new_anchor=(), new_xyz=None, new_anchor_center=None,
+                     new_anchor_level=(), new_center=None, new_level=(), track_point=(), track_center=None, track_level=()):
+        """SlamGraph::addKeyframe on the device tables.  Returns (index of the new vertex, index of the first new point)."""
+        keep, args = self._keyframe_args(T_newkey_from_oldkey, new_anchor, new_xyz, new_anchor_center, new_anchor_level,
+                                         new_center, new_level, track_point, track_center, track_level)
         v, q = C.c_int(), C.c_int()
-        self._ck(lib().svs_map_add_keyframe(self._h, int(oldkey), _dp(T), len(na), _ip(na), _dp(nx), _dp(nac), _ip(nal), _dp(nc),
-                                            _ip(nl), len(tp), _ip(tp), _dp(tc), _ip(tl), C.byref(v), C.byref(q)))
+        self._ck(lib().svs_map_add_keyframe(self._h, int(oldkey), *args, C.byref(v), C.byref(q)))
         self.V += 1
-        self.Np += len(na)
+        self.Np += len(keep[1])
         return v.value, q.value
+
+    def set_pose_graph(self, nbr_ptr, nbr_id, nbr_strength, nbr_T, nbr_Lambda):
+        """The pose graph with the strength of every directed entry (each list strongest first) and its constraint
+        (T_nbr_from_me [7], Lambda [36]): the graph add_keyframe_graph and add_edges grow."""
+        ptr = np.ascontiguousarray(nbr_ptr, np.int32)
+        ids, st = np.ascontiguousarray(nbr_id, np.int32), np.ascontiguousarray(nbr_strength, np.int32)
+        T = np.ascontiguousarray(nbr_T, np.float64).reshape(-1, 7)
+        Lm = np.ascontiguousarray(nbr_Lambda, np.float64).reshape(-1, 36)
+        if not len(ids) == len(st) == len(T) == len(Lm):
+            raise ValueError("nbr_id, nbr_strength, nbr_T and nbr_Lambda must have one row per entry")
+        self._ck(lib().svs_map_set_pose_graph(self._h, _ip(ptr), _ip(ids), _ip(st), _dp(T), _dp(Lm)))
+        self._nn = len(ids)
+
+    def get_graph(self):
+        """The pose graph as it lies on the device: dict(nbr_ptr, nbr_id, nbr_strength, nbr_T, nbr_Lambda)."""
+        nn = C.c_int()
+        self._ck(lib().svs_map_get_graph(self._h, 0, C.byref(nn), None, None, None, None, None))
+        n = nn.value
+        ptr, ids, st = np.zeros(self.V + 1, np.int32), np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+        T, Lm = np.zeros((max(n, 1), 7)), np.zeros((max(n, 1), 36))
+        self._ck(lib().svs_map_get_graph(self._h, n, C.byref(nn), _ip(ptr), _ip(ids), _ip(st), _dp(T), _dp(Lm)))
+        return dict(nbr_ptr=ptr, nbr_id=ids[:n], nbr_strength=st[:n], nbr_T=T[:n], nbr_Lambda=Lm[:n])
+
+    def add_keyframe_graph(self, oldkey, T_newkey_from_oldkey, covis_thr, width, height, new_anchor=(), new_xyz=None,
+                           new_anchor_center=None, new_anchor_level=(), new_center=None, new_level=(), track_point=(),
+                           track_center=None, track_level=()):
+        """The whole of SlamGraph::addKeyframe on the device: computeStrength (quirk B15 kept), the growth of add_keyframe
+        and addNewEdges(LOCAL) with the constraints.  Returns (index of the new vertex, index of the first new point,
+        strength table [n, 2] of (vertex, strength) rows in ascending vertex order, number of edges added)."""
+        keep, args = self._keyframe_args(T_newkey_from_oldkey, new_anchor, new_xyz, new_anchor_center, new_anchor_level,
+                                         new_center, new_level, track_point, track_center, track_level)
+        v, q, nt, ne = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        table = np.zeros((max(self.V, 1), 2), np.int32)
+        self._ck(lib().svs_map_add_keyframe_graph(self._h, int(oldkey), *args, int(covis_thr), int(width), int(height), C.byref(v),
+                                                  C.byref(q), C.byref(nt), _ip(table), C.byref(ne)))
+        self.V += 1
+        self.Np += len(keep[1])
+        self._nn = getattr(self, "_nn", 0) + 2 * ne.value
+        return v.value, q.value, table[:nt.value].copy(), ne.value
+
+    def add_edges(self, v1, v2, strength, moved_vertex=-1, T_moved_from_w=None):
+        """registerKeyframes' / addLoopClosure's edges: (v1[k], v2[k]) with strength[k] into both lists, the constraint
+        computeConstraint(v1, v2) with moved_vertex placed at T_moved_from_w."""
+        a, b, s = (np.ascontiguousarray(x, np.int32) for x in (v1, v2, strength))
+        if not len(a) == len(b) == len(s):
+            raise ValueError("v1, v2 and strength must have one entry per edge")
+        T = None if T_moved_from_w is None else np.ascontiguousarray(T_moved_from_w, np.float64).reshape(7)
+        self._ck(lib().svs_map_add_edges(self._h, len(a), _ip(a), _ip(b), _ip(s), int(moved_vertex), None if T is None else _dp(T)))
+        self._nn = getattr(self, "_nn", 0) + 2 * len(a)
 
     def set_problem(self, ba, window_vertex, active_point, cam, fixed=None, c_i=(), c_j=(), c_T=None, c_Lambda=None):
         """Assembles the window on the device and loads it into `ba` (a BundleAdjuster).  Returns E."""

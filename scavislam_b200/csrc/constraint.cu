@@ -16,6 +16,7 @@
 
 #include "../../include/svs_b200.h"
 #include "handle.cuh"
+#include "internal.cuh"
 #include "se3_dev.cuh"
 
 namespace {
@@ -108,6 +109,18 @@ __global__ void __launch_bounds__(kThreads) k_compute_constraint(CArgs a) {
 
 }  // namespace
 
+int svs::constraint_scratch_stride(int max_feat) { return max_feat > kSmemDepths ? max_feat : 0; }
+
+void svs::launch_compute_constraint(const double* poses, const int* feat_ptr, const int* feat_point, const int* point_anchor,
+                                    const double* xyz, int npairs, const int* v1, const int* v2, double* T_1_from_2,
+                                    double* Lambda, int* strength, double* scratch, int scratch_stride, cudaStream_t stream) {
+  CArgs a;
+  a.poses = poses; a.feat_ptr = feat_ptr; a.feat_point = feat_point; a.point_anchor = point_anchor; a.xyz = xyz;
+  a.v1 = v1; a.v2 = v2; a.T12 = T_1_from_2; a.Lambda = Lambda; a.strength = strength;
+  a.scratch = scratch; a.scratch_stride = scratch_stride;
+  k_compute_constraint<<<npairs, kThreads, 0, stream>>>(a);
+}
+
 struct svs_constraints : svs::Handle {
   size_t cap_bytes = 0;
   char* d_buf = nullptr;
@@ -158,7 +171,7 @@ int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_fr
   for (int k = 0; k < npairs; ++k)
     if (v1[k] < 0 || v1[k] >= P || v2[k] < 0 || v2[k] >= P) { h->err = "pair names a pose outside [0, P)"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  const int scratch_stride = max_feat > kSmemDepths ? max_feat : 0;
+  const int scratch_stride = svs::constraint_scratch_stride(max_feat);
   // one arena: inputs, outputs, scratch
   auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   size_t off = 0;
@@ -187,20 +200,19 @@ int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_fr
   }
   SVS_CK(h, cudaMemcpyAsync(B + o_v1, v1, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
   SVS_CK(h, cudaMemcpyAsync(B + o_v2, v2, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
-  CArgs a;
-  a.poses = reinterpret_cast<const double*>(B + o_pose);
-  a.feat_ptr = reinterpret_cast<const int*>(B + o_fptr); a.feat_point = reinterpret_cast<const int*>(B + o_fpt);
-  a.point_anchor = reinterpret_cast<const int*>(B + o_anch); a.xyz = reinterpret_cast<const double*>(B + o_xyz);
-  a.v1 = reinterpret_cast<const int*>(B + o_v1); a.v2 = reinterpret_cast<const int*>(B + o_v2);
-  a.T12 = reinterpret_cast<double*>(B + o_T); a.Lambda = reinterpret_cast<double*>(B + o_L);
-  a.strength = reinterpret_cast<int*>(B + o_n);
-  a.scratch = reinterpret_cast<double*>(B + o_s); a.scratch_stride = scratch_stride;
-  k_compute_constraint<<<npairs, kThreads, 0, h->stream>>>(a);
+  double* T12 = reinterpret_cast<double*>(B + o_T);
+  double* Lm = reinterpret_cast<double*>(B + o_L);
+  int* n = reinterpret_cast<int*>(B + o_n);
+  svs::launch_compute_constraint(reinterpret_cast<const double*>(B + o_pose), reinterpret_cast<const int*>(B + o_fptr),
+                                 reinterpret_cast<const int*>(B + o_fpt), reinterpret_cast<const int*>(B + o_anch),
+                                 reinterpret_cast<const double*>(B + o_xyz), npairs, reinterpret_cast<const int*>(B + o_v1),
+                                 reinterpret_cast<const int*>(B + o_v2), T12, Lm, n, reinterpret_cast<double*>(B + o_s),
+                                 scratch_stride, h->stream);
   SVS_CK(h, cudaGetLastError());
-  SVS_CK(h, cudaMemcpyAsync(T_1_from_2, a.T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(Lambda, a.Lambda, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(T_1_from_2, T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(Lambda, Lm, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
   if (visibility_strength)
-    SVS_CK(h, cudaMemcpyAsync(visibility_strength, a.strength, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(visibility_strength, n, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }

@@ -17,6 +17,7 @@
 #include <string>
 #include <vector>
 
+#include <cub/cub.cuh>
 #include <cuda_runtime.h>
 
 #include "../../include/svs_b200.h"
@@ -141,6 +142,7 @@ __global__ void k_scatter_rows(double* __restrict__ table, const int* __restrict
 struct GraphDev {
   const int* nbr_ptr;       // [V+1]
   const int* nbr_id;        // [nnzN] neighbours of a vertex, strongest first (the order computeInitialDoubleWin pushes them)
+  const int* nbr_str;       // [nnzN] the strength key of neighbor_ids_ordered_by_strength (or nullptr)
   const double* nbr_T;      // [nnzN][7]  T_nbr_from_me of the directed entry (or nullptr)
   const double* nbr_Lam;    // [nnzN][36]
 };
@@ -287,6 +289,174 @@ __global__ void k_grow_move(MapDev m, int Np_new, int newkey, const int* __restr
   }
 }
 
+// ------------------------------------------------------------------ growth of the pose graph
+// computeStrength (slam_graph.cpp:468-552), one record per (track, observer) pair: key (vertex, track), the quadrant
+// bits of the track's centre (1 left / 2 right by u < half_width, 4 top / 8 bottom by v < half_height)
+__global__ void k_str_count(MapDev m, int n_track, const int* __restrict__ track_point, int* __restrict__ cnt) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n_track) cnt[t] = m.vis_ptr[track_point[t] + 1] - m.vis_ptr[track_point[t]];
+}
+__global__ void k_str_emit(MapDev m, int n_track, const int* __restrict__ track_point, const double* __restrict__ track_center,
+                           double half_w, double half_h, const int* __restrict__ ptr, unsigned long long* __restrict__ key,
+                           unsigned char* __restrict__ quad, int* __restrict__ vcnt) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_track) return;
+  const int p = track_point[t];
+  const unsigned char q = (track_center[3 * (size_t)t] < half_w ? 1 : 2) | (track_center[3 * (size_t)t + 1] < half_h ? 4 : 8);
+  int at = ptr[t];
+  for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i, ++at) {
+    const int v = m.vis_pose[i];
+    key[at] = (unsigned long long)v << 32 | (unsigned)t;
+    quad[at] = q;
+    atomicAdd(vcnt + v, 1);
+  }
+}
+__global__ void k_str_new(int n_new, const int* __restrict__ new_anchor, int* __restrict__ newcnt) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q < n_new) atomicAdd(newcnt + new_anchor[q], 1);
+}
+// Quirk B15 in closed form, one warp per vertex over its records in track order: the zeroing loop runs after every
+// track, so a frame keeps only the tracks from t* on, t* = the first track after which its four quadrant counts are all
+// >= need = max(1, covis_thr / 2); none: 0.  Without tracks the zeroing never runs and the new points stay.
+__global__ void k_str_closed(int V, int n_track, int need, const int* __restrict__ vptr, const unsigned char* __restrict__ quad,
+                             const int* __restrict__ newcnt, int* __restrict__ strength, int* __restrict__ in_table) {
+  const int v = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (v >= V) return;
+  const int s0 = vptr[v], s1 = vptr[v + 1];
+  int tstar = -1, c0 = 0, c1 = 0, c2 = 0, c3 = 0;
+  for (int base = s0; n_track && base < s1 && tstar < 0; base += 32) {
+    const int i = base + lane;
+    const int q = i < s1 ? quad[i] : 0;
+    int a0 = q & 1, a1 = (q >> 1) & 1, a2 = (q >> 2) & 1, a3 = (q >> 3) & 1;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int b0 = __shfl_up_sync(0xffffffffu, a0, o), b1 = __shfl_up_sync(0xffffffffu, a1, o);
+      const int b2 = __shfl_up_sync(0xffffffffu, a2, o), b3 = __shfl_up_sync(0xffffffffu, a3, o);
+      if (lane >= o) { a0 += b0; a1 += b1; a2 += b2; a3 += b3; }
+    }
+    a0 += c0; a1 += c1; a2 += c2; a3 += c3;
+    const unsigned ok = __ballot_sync(0xffffffffu, i < s1 && a0 >= need && a1 >= need && a2 >= need && a3 >= need);
+    if (ok) tstar = base + __ffs(ok) - 1;
+    c0 = __shfl_sync(0xffffffffu, a0, 31); c1 = __shfl_sync(0xffffffffu, a1, 31);
+    c2 = __shfl_sync(0xffffffffu, a2, 31); c3 = __shfl_sync(0xffffffffu, a3, 31);
+  }
+  if (lane == 0) {
+    strength[v] = n_track == 0 ? newcnt[v] : (tstar < 0 ? 0 : s1 - tstar);
+    in_table[v] = newcnt[v] > 0 || s1 > s0;
+  }
+}
+// the table in ascending vertex order after the oldkey bump, and the LOCAL edges (other, newkey) of addNewEdges
+__global__ void k_str_table(int V, int oldkey, int covis_thr, const int* __restrict__ in_table, const int* __restrict__ tptr,
+                            int* __restrict__ strength, int* __restrict__ qual, int* __restrict__ rows) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V) return;
+  int s = strength[v];
+  if (v == oldkey && s < covis_thr) s = covis_thr;   // slam_graph.cpp:172-175
+  strength[v] = s;
+  qual[v] = in_table[v] && s >= covis_thr;
+  if (in_table[v]) { rows[2 * (size_t)tptr[v]] = v; rows[2 * (size_t)tptr[v] + 1] = s; }
+}
+__global__ void k_str_edges(int V, int newkey, const int* __restrict__ qual, const int* __restrict__ eptr,
+                            const int* __restrict__ strength, int* __restrict__ v1, int* __restrict__ v2, int* __restrict__ es) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= V || !qual[v]) return;
+  v1[eptr[v]] = v; v2[eptr[v]] = newkey; es[eptr[v]] = strength[v];
+}
+
+// an edge of the request already in the graph, or a pair listed twice (insertEdge asserts, slam_graph.hpp:349-353)
+__global__ void k_edge_exists(GraphDev g, int gV, int n, const int* __restrict__ v1, const int* __restrict__ v2, int* __restrict__ bad) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  if (v1[k] < gV && v2[k] < gV && has_edge(g, v1[k], v2[k])) atomicAdd(bad, 1);
+}
+
+// the feature tables (points in ascending id) of the vertices the new edges touch: flag, count, emit, sort
+__global__ void k_touch(int n, const int* __restrict__ v1, const int* __restrict__ v2, int* __restrict__ touched) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) { touched[v1[k]] = 1; touched[v2[k]] = 1; }
+}
+__global__ void k_feat_count(MapDev m, const int* __restrict__ touched, int* __restrict__ fcnt) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m.Np) return;
+  for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i)
+    if (touched[m.vis_pose[i]]) atomicAdd(fcnt + m.vis_pose[i], 1);
+}
+__global__ void k_feat_emit(MapDev m, const int* __restrict__ touched, const int* __restrict__ fptr, int* __restrict__ fcur,
+                            unsigned long long* __restrict__ key) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= m.Np) return;
+  for (int i = m.vis_ptr[p]; i < m.vis_ptr[p + 1]; ++i) {
+    const int v = m.vis_pose[i];
+    if (touched[v]) key[fptr[v] + atomicAdd(fcur + v, 1)] = (unsigned long long)v << 32 | (unsigned)p;
+  }
+}
+__global__ void k_feat_unpack(int n, const unsigned long long* __restrict__ key, int* __restrict__ point) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) point[i] = (int)(unsigned)key[i];
+}
+__global__ void k_max(int n, const int* __restrict__ x, int* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) atomicMax(out, x[i]);
+}
+
+// neighbour-list insertion.  Edge k inserts (strength[k], v2) into v1's list (sequence 2k) and then (strength[k], v1)
+// into v2's (2k + 1), each as std::multimap::insert does (after the equal keys; lists are read through rbegin): in the
+// stored order, strongest first, a new entry goes in front of the first entry with strength <= its own.
+__global__ void k_ins_keys(int n, const int* __restrict__ v1, const int* __restrict__ v2, int* __restrict__ target,
+                           int* __restrict__ seq, int* __restrict__ icnt) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 2 * n) return;
+  const int t = (j & 1) ? v2[j >> 1] : v1[j >> 1];
+  target[j] = t; seq[j] = j;
+  atomicAdd(icnt + t, 1);
+}
+__global__ void k_ins_count(int V, int gV, const int* __restrict__ old_ptr, const int* __restrict__ icnt, int* __restrict__ cnt) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v < V) cnt[v] = (v < gV ? old_ptr[v + 1] - old_ptr[v] : 0) + icnt[v];
+}
+struct InsArgs {
+  int n, gV, nn_old;
+  GraphDev g;                     // the graph before the call (gV lists)
+  const int *iptr, *iseq;         // the inserts grouped by target vertex, in sequence order inside a group
+  const int *v1, *v2, *es;        // the edges
+  const double *T12, *Lam;        // their constraints: T_1_from_2, Lambda
+  const int* nptr;                // the new lists
+  int *id, *str; double *T, *L;
+};
+__global__ void k_ins_move_old(InsArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.nn_old) return;
+  int lo = 0, hi = a.gV;          // the vertex whose list holds entry i: nbr_ptr[v] <= i < nbr_ptr[v + 1]
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (a.g.nbr_ptr[mid] <= i) lo = mid; else hi = mid; }
+  const int v = lo, s = a.g.nbr_str[i];
+  int at = a.nptr[v] + (i - a.g.nbr_ptr[v]);
+  for (int j = a.iptr[v]; j < a.iptr[v + 1]; ++j) at += a.es[a.iseq[j] >> 1] >= s;
+  a.id[at] = a.g.nbr_id[i]; a.str[at] = s;
+  for (int q = 0; q < 7; ++q) a.T[7 * (size_t)at + q] = a.g.nbr_T[7 * (size_t)i + q];
+  for (int q = 0; q < 36; ++q) a.L[36 * (size_t)at + q] = a.g.nbr_Lam[36 * (size_t)i + q];
+}
+__global__ void k_ins_move_new(InsArgs a, int V) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 2 * a.n) return;
+  const int sq = a.iseq[j], k = sq >> 1, s = a.es[k];
+  int lo = 0, hi = V;             // the target vertex: iptr[v] <= j < iptr[v + 1]
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (a.iptr[mid] <= j) lo = mid; else hi = mid; }
+  const int v = lo;
+  int at = a.nptr[v];
+  if (v < a.gV)
+    for (int i = a.g.nbr_ptr[v]; i < a.g.nbr_ptr[v + 1]; ++i) at += a.g.nbr_str[i] > s;
+  for (int r = a.iptr[v]; r < a.iptr[v + 1]; ++r) {
+    const int s2 = a.es[a.iseq[r] >> 1];
+    at += s2 > s || (s2 == s && a.iseq[r] > sq);
+  }
+  // setConstraint(v1, v2, T_1_from_2, Lambda, Lambda): v2's entry for v1 holds T_1_from_2, v1's entry its inverse
+  a.id[at] = (sq & 1) ? a.v1[k] : a.v2[k]; a.str[at] = s;
+  double Ti[7];
+  const double* T12 = a.T12 + 7 * (size_t)k;
+  if (!(sq & 1)) svs::se3_inv(T12, Ti);
+  for (int q = 0; q < 7; ++q) a.T[7 * (size_t)at + q] = (sq & 1) ? T12[q] : Ti[q];
+  for (int q = 0; q < 36; ++q) a.L[36 * (size_t)at + q] = a.Lam[36 * (size_t)k + q];
+}
+
 }  // namespace
 
 struct svs_map : svs::Handle {
@@ -304,6 +474,10 @@ struct svs_map : svs::Handle {
   unsigned long long last_serial = 0;
   char* d_upd = nullptr; size_t upd_cap = 0;   // staging of svs_map_update_*
   char* d_graph = nullptr; size_t graph_cap = 0; GraphDev g{}; int nnzN = 0;   // svs_map_set_graph
+  char* d_graph2 = nullptr; size_t graph2_cap = 0;   // the next graph while the growth calls build it (then swapped)
+  char* d_gw = nullptr; size_t gw_cap = 0;           // work of the growth calls: strengths and staged edge lists
+  char* d_ge = nullptr; size_t ge_cap = 0;           // ... feature tables, constraints and list insertion
+  char* d_cs = nullptr; size_t cs_cap = 0;           // ... median scratch of the constraint kernel
   char* d_sel = nullptr; size_t sel_cap = 0;   // work buffers of svs_map_select_window
 };
 
@@ -350,6 +524,7 @@ void svs_map_destroy(svs_map* h) {
   if (!h) return;
   svs::begin_close(h);
   cudaFree(h->d_map); cudaFree(h->d_work); cudaFree(h->d_upd); cudaFree(h->d_graph); cudaFree(h->d_sel);
+  cudaFree(h->d_graph2); cudaFree(h->d_gw); cudaFree(h->d_ge); cudaFree(h->d_cs);
   delete h;
 }
 
@@ -551,36 +726,93 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
 
 // ------------------------------------------------------------------ pose graph, window selection, growth
 
-int svs_map_set_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const double* nbr_T, const double* nbr_Lambda) {
+struct GraphLayout { size_t o_ptr, o_id, o_str, o_T, o_L, total; };
+static GraphLayout graph_layout(int V, int nn) {
+  GraphLayout lo{};
+  size_t off = 0;
+  lo.o_ptr = off; off += al256(sizeof(int) * ((size_t)V + 1));
+  lo.o_id = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
+  lo.o_str = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
+  lo.o_T = off; off += al256(sizeof(double) * 7 * (size_t)std::max(nn, 1));
+  lo.o_L = off; off += al256(sizeof(double) * 36 * (size_t)std::max(nn, 1));
+  lo.total = off;
+  return lo;
+}
+static void graph_bind(svs_map* h, char* B, const GraphLayout& lo, int nn, bool strength, bool constraints) {
+  h->g.nbr_ptr = reinterpret_cast<const int*>(B + lo.o_ptr); h->g.nbr_id = reinterpret_cast<const int*>(B + lo.o_id);
+  h->g.nbr_str = strength ? reinterpret_cast<const int*>(B + lo.o_str) : nullptr;
+  h->g.nbr_T = constraints ? reinterpret_cast<const double*>(B + lo.o_T) : nullptr;
+  h->g.nbr_Lam = constraints ? reinterpret_cast<const double*>(B + lo.o_L) : nullptr;
+  h->nnzN = nn;
+}
+
+// pose_graph: the lists come with strengths and constraints (svs_map_set_pose_graph), all required when there are entries
+static int upload_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const int* nbr_strength, const double* nbr_T,
+                        const double* nbr_Lambda, bool pose_graph) {
   if (!h || !h->d_map || !nbr_ptr) return SVS_ERR_INVALID;
   const int V = h->V, nn = nbr_ptr[V];
   if (nbr_ptr[0] != 0 || nn < 0 || (nn && !nbr_id) || ((nbr_T == nullptr) != (nbr_Lambda == nullptr))) return SVS_ERR_INVALID;
+  if (pose_graph && nn && (!nbr_strength || !nbr_T)) return SVS_ERR_INVALID;
   for (int v = 0; v < V; ++v)
     if (nbr_ptr[v + 1] < nbr_ptr[v]) { h->err = "nbr_ptr not ascending"; return SVS_ERR_INVALID; }
   for (int i = 0; i < nn; ++i)
     if (nbr_id[i] < 0 || nbr_id[i] >= V) { h->err = "neighbour outside [0, V)"; return SVS_ERR_INVALID; }
+  if (pose_graph)
+    for (int v = 0; v < V; ++v)
+      for (int i = nbr_ptr[v] + 1; i < nbr_ptr[v + 1]; ++i)
+        if (nbr_strength[i] > nbr_strength[i - 1]) { h->err = "a neighbour list is not ordered strongest first"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  size_t off = 0;
-  const size_t o_ptr = off; off += al256(sizeof(int) * ((size_t)V + 1));
-  const size_t o_id = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
-  const size_t o_T = off; off += al256(sizeof(double) * 7 * (size_t)std::max(nn, 1));
-  const size_t o_L = off; off += al256(sizeof(double) * 36 * (size_t)std::max(nn, 1));
+  const GraphLayout lo = graph_layout(V, nn);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->graph_cap, &h->d_graph));
+  SVS_CK(h, svs::grow(lo.total, &h->graph_cap, &h->d_graph));
   char* B = h->d_graph;
-  SVS_CK(h, cudaMemcpyAsync(B + o_ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(B + lo.o_ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
   if (nn) {
-    SVS_CK(h, cudaMemcpyAsync(B + o_id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(B + lo.o_id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+    if (pose_graph) SVS_CK(h, cudaMemcpyAsync(B + lo.o_str, nbr_strength, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     if (nbr_T) {
-      SVS_CK(h, cudaMemcpyAsync(B + o_T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
-      SVS_CK(h, cudaMemcpyAsync(B + o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(B + lo.o_T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(B + lo.o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     }
   }
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  h->g.nbr_ptr = reinterpret_cast<const int*>(B + o_ptr); h->g.nbr_id = reinterpret_cast<const int*>(B + o_id);
-  h->g.nbr_T = nbr_T ? reinterpret_cast<const double*>(B + o_T) : nullptr;
-  h->g.nbr_Lam = nbr_T ? reinterpret_cast<const double*>(B + o_L) : nullptr;
-  h->nnzN = nn;
+  graph_bind(h, B, lo, nn, pose_graph, pose_graph || nbr_T != nullptr);
+  return SVS_OK;
+}
+
+int svs_map_set_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const double* nbr_T, const double* nbr_Lambda) {
+  return upload_graph(h, nbr_ptr, nbr_id, nullptr, nbr_T, nbr_Lambda, false);
+}
+
+int svs_map_set_pose_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const int* nbr_strength, const double* nbr_T,
+                           const double* nbr_Lambda) {
+  return upload_graph(h, nbr_ptr, nbr_id, nbr_strength, nbr_T, nbr_Lambda, true);
+}
+
+int svs_map_get_graph(svs_map* h, int cap, int* nnzN, int* nbr_ptr, int* nbr_id, int* nbr_strength, double* nbr_T,
+                      double* nbr_Lambda) {
+  if (!h || !h->d_map || !nnzN) return SVS_ERR_INVALID;
+  if (!h->g.nbr_ptr) { h->err = "the map has no pose graph"; return SVS_ERR_STATE; }
+  const int V = h->V, nn = h->nnzN;
+  *nnzN = nn;
+  if ((nbr_id || nbr_strength || nbr_T || nbr_Lambda) && cap < nn) { h->err = "nnzN exceeds the caller's capacity"; return SVS_ERR_INVALID; }
+  cudaSetDevice(h->device);
+  if (nbr_ptr) SVS_CK(h, cudaMemcpyAsync(nbr_ptr, h->g.nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyDeviceToHost, h->stream));
+  if (nn) {
+    if (nbr_id) SVS_CK(h, cudaMemcpyAsync(nbr_id, h->g.nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyDeviceToHost, h->stream));
+    if (nbr_strength && h->g.nbr_str)
+      SVS_CK(h, cudaMemcpyAsync(nbr_strength, h->g.nbr_str, sizeof(int) * (size_t)nn, cudaMemcpyDeviceToHost, h->stream));
+    if (nbr_T && h->g.nbr_T) SVS_CK(h, cudaMemcpyAsync(nbr_T, h->g.nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyDeviceToHost, h->stream));
+    if (nbr_Lambda && h->g.nbr_Lam)
+      SVS_CK(h, cudaMemcpyAsync(nbr_Lambda, h->g.nbr_Lam, sizeof(double) * 36 * (size_t)nn, cudaMemcpyDeviceToHost, h->stream));
+  }
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  // what the graph does not hold reads as strength 0, the identity and Lambda = 0 (as svs_map_select_window pairs it)
+  for (int i = 0; i < nn; ++i) {
+    if (nbr_strength && !h->g.nbr_str) nbr_strength[i] = 0;
+    if (nbr_T && !h->g.nbr_T) for (int q = 0; q < 7; ++q) nbr_T[7 * (size_t)i + q] = q == 3 ? 1. : 0.;
+    if (nbr_Lambda && !h->g.nbr_Lam) memset(nbr_Lambda + 36 * (size_t)i, 0, sizeof(double) * 36);
+  }
   return SVS_OK;
 }
 
@@ -651,15 +883,17 @@ int svs_map_select_window(svs_map* h, int root, int inner_window_size, int doubl
   return SVS_OK;
 }
 
-int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new, const int* new_anchor,
-                         const double* new_xyz_anchor, const double* new_anchor_center, const int* new_anchor_level,
-                         const double* new_center, const int* new_level, int n_track, const int* track_point,
-                         const double* track_center, const int* track_level, int* vertex_index, int* first_new_point) {
+}  // extern "C"
+
+static int keyframe_check(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new, const int* new_anchor,
+                          const double* new_xyz_anchor, const double* new_anchor_center, const int* new_anchor_level,
+                          const double* new_center, const int* new_level, int n_track, const int* track_point,
+                          const double* track_center, const int* track_level) {
   if (!h || !h->d_map || !T_newkey_from_oldkey || n_new < 0 || n_track < 0 ||
       (n_new && (!new_anchor || !new_xyz_anchor || !new_anchor_center || !new_anchor_level || !new_center || !new_level)) ||
       (n_track && (!track_point || !track_center || !track_level)))
     return SVS_ERR_INVALID;
-  const int V = h->V, Np = h->Np, nnz = h->nnz;
+  const int V = h->V, Np = h->Np;
   if (oldkey < 0 || oldkey >= V) { h->err = "oldkey outside [0, V)"; return SVS_ERR_INVALID; }
   for (int q = 0; q < n_new; ++q)
     if (new_anchor[q] < 0 || new_anchor[q] >= V || new_anchor_level[q] < 0 || new_anchor_level[q] > 30 || new_level[q] < 0 || new_level[q] > 30) {
@@ -675,6 +909,15 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
         return SVS_ERR_INVALID;
       }
   }
+  return SVS_OK;
+}
+
+// the growth of svs_map_add_keyframe on checked arguments; the pose graph is left as it was
+static int keyframe_grow(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new, const int* new_anchor,
+                         const double* new_xyz_anchor, const double* new_anchor_center, const int* new_anchor_level,
+                         const double* new_center, const int* new_level, int n_track, const int* track_point,
+                         const double* track_center, const int* track_level) {
+  const int V = h->V, Np = h->Np, nnz = h->nnz;
   cudaSetDevice(h->device);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int V2 = V + 1, Np2 = Np + n_new, nnz2 = nnz + n_track + 2 * n_new;
@@ -722,12 +965,254 @@ int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_old
   cudaFree(h->d_map);
   h->d_map = B2; h->map_cap = lo.total + lo.total / 4;
   map_bind(h, B2, lo, V2, Np2, nnz2);
-  h->g = GraphDev{}; h->nnzN = 0;          // the pose graph changed with the new vertex: svs_map_set_graph again
   h->d_win_last = nullptr;                 // (a window assembled before the growth can no longer be absorbed)
+  return SVS_OK;
+}
+
+extern "C" int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new, const int* new_anchor,
+                                    const double* new_xyz_anchor, const double* new_anchor_center, const int* new_anchor_level,
+                                    const double* new_center, const int* new_level, int n_track, const int* track_point,
+                                    const double* track_center, const int* track_level, int* vertex_index,
+                                    int* first_new_point) {
+  int rc = keyframe_check(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
+                          new_center, new_level, n_track, track_point, track_center, track_level);
+  const int V = rc == SVS_OK ? h->V : 0, Np = rc == SVS_OK ? h->Np : 0;
+  if (rc == SVS_OK)
+    rc = keyframe_grow(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
+                       new_center, new_level, n_track, track_point, track_center, track_level);
+  if (rc != SVS_OK) return rc;
+  h->g = GraphDev{}; h->nnzN = 0;          // the pose graph changed with the new vertex: svs_map_set_graph again
   if (vertex_index) *vertex_index = V;
   if (first_new_point) *first_new_point = Np;
   return SVS_OK;
 }
+
+// addNewEdges' list insertion and setConstraint for n edges (device arrays v1, v2, strength on the map's stream):
+// the feature tables of the vertices they touch, computeConstraint(v1, v2) on `poses` (the map's, or a copy with one
+// vertex moved), then the new lists with their constraints.  The graph before the call has gV <= V lists; the lists of
+// vertices gV..V-1 start empty.
+static int grow_graph(svs_map* h, int gV, int n, const int* d_v1, const int* d_v2, const int* d_es, const double* d_poses) {
+  const int V = h->V, Np = h->Np, nn_old = h->nnzN, nn = nn_old + 2 * n;
+  const size_t nf = (size_t)std::max(h->nnz, 1), ni = (size_t)std::max(2 * n, 1);
+  cudaSetDevice(h->device);
+  size_t tmp_bytes = 0, b = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nf);
+  tmp_bytes = std::max(tmp_bytes, b);
+  cub::DeviceRadixSort::SortPairs(nullptr, b, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)ni);
+  tmp_bytes = std::max(tmp_bytes, b);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  const size_t o_touch = take(sizeof(int) * V), o_fcnt = take(sizeof(int) * V), o_fptr = take(sizeof(int) * ((size_t)V + 1));
+  const size_t o_fcur = take(sizeof(int) * V), o_ctl = take(sizeof(int) * 4);
+  const size_t o_fkey = take(8 * nf), o_fkey2 = take(8 * nf), o_fpt = take(sizeof(int) * nf);
+  const size_t o_T12 = take(sizeof(double) * 7 * ni), o_Lam = take(sizeof(double) * 36 * ni), o_cs = take(sizeof(int) * ni);
+  const size_t o_icnt = take(sizeof(int) * V), o_iptr = take(sizeof(int) * ((size_t)V + 1)), o_ncnt = take(sizeof(int) * V);
+  const size_t o_tgt = take(sizeof(int) * ni), o_tgt2 = take(sizeof(int) * ni), o_seq = take(sizeof(int) * ni);
+  const size_t o_seq2 = take(sizeof(int) * ni), o_tmp = take(tmp_bytes);
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->ge_cap, &h->d_ge));
+  const GraphLayout lo = graph_layout(V, nn);
+  SVS_CK(h, svs::grow(lo.total, &h->graph2_cap, &h->d_graph2));
+  char* W = h->d_ge;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
+  auto D = [&](size_t o) { return reinterpret_cast<double*>(W + o); };
+  const int bV = (V + 255) / 256;
+  for (size_t o : {o_touch, o_fcnt, o_fcur, o_icnt}) SVS_CK(h, cudaMemsetAsync(W + o, 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(W + o_ctl, 0, sizeof(int) * 4, h->stream));
+  if (n) {
+    k_touch<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(o_touch));
+    if (Np) k_feat_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, I(o_touch), I(o_fcnt));
+    k_scan<<<1, 1024, 0, h->stream>>>(I(o_fcnt), V, I(o_fptr));
+    k_max<<<bV, 256, 0, h->stream>>>(V, I(o_fcnt), I(o_ctl) + 1);
+    SVS_CK(h, cudaMemcpyAsync(I(o_ctl), I(o_fptr) + V, sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
+    int ctl[2] = {0, 0};
+    SVS_CK(h, cudaMemcpyAsync(ctl, I(o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
+    const int nfeat = ctl[0], stride = svs::constraint_scratch_stride(ctl[1]);
+    if (nfeat) {
+      k_feat_emit<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, I(o_touch), I(o_fptr), I(o_fcur), U(o_fkey));
+      size_t tb = tmp_bytes;
+      SVS_CK(h, cub::DeviceRadixSort::SortKeys(W + o_tmp, tb, U(o_fkey), U(o_fkey2), nfeat, 0, 64, h->stream));
+      k_feat_unpack<<<(nfeat + 255) / 256, 256, 0, h->stream>>>(nfeat, U(o_fkey2), I(o_fpt));
+    }
+    if (stride) {
+      SVS_CK(h, cudaStreamSynchronize(h->stream));
+      SVS_CK(h, svs::grow(sizeof(double) * (size_t)stride * n, &h->cs_cap, &h->d_cs));
+    }
+    svs::launch_compute_constraint(d_poses, I(o_fptr), I(o_fpt), h->m.anchor, h->m.xyz, n, d_v1, d_v2, D(o_T12), D(o_Lam), I(o_cs),
+                                   reinterpret_cast<double*>(h->d_cs), stride, h->stream);
+    k_ins_keys<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(o_tgt), I(o_seq), I(o_icnt));
+    size_t tb = tmp_bytes;   // a stable sort: inside one target the inserts stay in sequence order
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(W + o_tmp, tb, I(o_tgt), I(o_tgt2), I(o_seq), I(o_seq2), 2 * n, 0, 32, h->stream));
+  }
+  k_scan<<<1, 1024, 0, h->stream>>>(I(o_icnt), V, I(o_iptr));
+  char* B = h->d_graph2;
+  k_ins_count<<<bV, 256, 0, h->stream>>>(V, gV, h->g.nbr_ptr, I(o_icnt), I(o_ncnt));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(o_ncnt), V, reinterpret_cast<int*>(B + lo.o_ptr));
+  InsArgs a;
+  a.n = n; a.gV = gV; a.nn_old = nn_old; a.g = h->g; a.iptr = I(o_iptr); a.iseq = I(o_seq2);
+  a.v1 = d_v1; a.v2 = d_v2; a.es = d_es; a.T12 = D(o_T12); a.Lam = D(o_Lam);
+  a.nptr = reinterpret_cast<const int*>(B + lo.o_ptr);
+  a.id = reinterpret_cast<int*>(B + lo.o_id); a.str = reinterpret_cast<int*>(B + lo.o_str);
+  a.T = reinterpret_cast<double*>(B + lo.o_T); a.L = reinterpret_cast<double*>(B + lo.o_L);
+  if (nn_old) k_ins_move_old<<<(nn_old + 255) / 256, 256, 0, h->stream>>>(a);
+  if (n) k_ins_move_new<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(a, V);
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  std::swap(h->d_graph, h->d_graph2); std::swap(h->graph_cap, h->graph2_cap);
+  graph_bind(h, h->d_graph, lo, nn, true, true);
+  return SVS_OK;
+}
+
+static int needs_pose_graph(svs_map* h) {
+  if (!h->g.nbr_ptr || !h->g.nbr_str || !h->g.nbr_T) {
+    h->err = "the map has no pose graph with strengths and constraints (svs_map_set_pose_graph)";
+    return SVS_ERR_STATE;
+  }
+  return SVS_OK;
+}
+
+extern "C" int svs_map_add_keyframe_graph(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new,
+                                          const int* new_anchor, const double* new_xyz_anchor, const double* new_anchor_center,
+                                          const int* new_anchor_level, const double* new_center, const int* new_level,
+                                          int n_track, const int* track_point, const double* track_center,
+                                          const int* track_level, int covis_thr, int width, int height, int* vertex_index,
+                                          int* first_new_point, int* n_table, int* table, int* n_edges) {
+  svs::NvtxRange nvtx_("addKeyframe");
+  int rc = keyframe_check(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
+                          new_center, new_level, n_track, track_point, track_center, track_level);
+  if (rc != SVS_OK) return rc;
+  if (covis_thr < 1 || width <= 0 || height <= 0) { h->err = "covis_thr < 1 or an empty image"; return SVS_ERR_INVALID; }
+  if ((rc = needs_pose_graph(h)) != SVS_OK) return rc;
+  const int V = h->V, Np = h->Np;
+  const size_t nr = (size_t)std::max(h->nnz, 1);   // records: the tracked points are distinct, so at most nnz
+  cudaSetDevice(h->device);
+  size_t tmp_bytes = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
+                                  (unsigned char*)nullptr, (unsigned char*)nullptr, (int)nr);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  const size_t o_tp = take(sizeof(int) * n_track), o_tc = take(sizeof(double) * 3 * n_track), o_na = take(sizeof(int) * n_new);
+  const size_t o_tcnt = take(sizeof(int) * n_track), o_tptr = take(sizeof(int) * ((size_t)n_track + 1));
+  const size_t o_vcnt = take(sizeof(int) * V), o_vptr = take(sizeof(int) * ((size_t)V + 1)), o_new = take(sizeof(int) * V);
+  const size_t o_str = take(sizeof(int) * V), o_in = take(sizeof(int) * V), o_rptr = take(sizeof(int) * ((size_t)V + 1));
+  const size_t o_qual = take(sizeof(int) * V), o_eptr = take(sizeof(int) * ((size_t)V + 1)), o_rows = take(sizeof(int) * 2 * V);
+  const size_t o_v1 = take(sizeof(int) * V), o_v2 = take(sizeof(int) * V), o_es = take(sizeof(int) * V);
+  const size_t o_key = take(8 * nr), o_key2 = take(8 * nr), o_q = take(nr), o_q2 = take(nr), o_tmp = take(tmp_bytes);
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->gw_cap, &h->d_gw));
+  char* W = h->d_gw;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
+  auto Q = [&](size_t o) { return reinterpret_cast<unsigned char*>(W + o); };
+  if (n_track) {
+    SVS_CK(h, cudaMemcpyAsync(W + o_tp, track_point, sizeof(int) * n_track, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(W + o_tc, track_center, sizeof(double) * 3 * n_track, cudaMemcpyHostToDevice, h->stream));
+  }
+  if (n_new) SVS_CK(h, cudaMemcpyAsync(W + o_na, new_anchor, sizeof(int) * n_new, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(W + o_vcnt, 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(W + o_new, 0, sizeof(int) * V, h->stream));
+  // computeStrength on the map before the growth
+  int R = 0;
+  if (n_track) {
+    k_str_count<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, I(o_tp), I(o_tcnt));
+    k_scan<<<1, 1024, 0, h->stream>>>(I(o_tcnt), n_track, I(o_tptr));
+    SVS_CK(h, cudaMemcpyAsync(&R, I(o_tptr) + n_track, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaStreamSynchronize(h->stream));
+  }
+  if (R) {
+    const int half_w = (int)(width * 0.5), half_h = (int)(height * 0.5);   // int half_width = cam_.width()*0.5 (:480-481)
+    k_str_emit<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, I(o_tp), reinterpret_cast<const double*>(W + o_tc),
+                                                             (double)half_w, (double)half_h, I(o_tptr), U(o_key), Q(o_q), I(o_vcnt));
+    size_t tb = tmp_bytes;
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(W + o_tmp, tb, U(o_key), U(o_key2), Q(o_q), Q(o_q2), R, 0, 64, h->stream));
+  }
+  if (n_new) k_str_new<<<(n_new + 255) / 256, 256, 0, h->stream>>>(n_new, I(o_na), I(o_new));
+  const int bV = (V + 255) / 256;
+  k_scan<<<1, 1024, 0, h->stream>>>(I(o_vcnt), V, I(o_vptr));
+  k_str_closed<<<(int)((32 * (size_t)V + 255) / 256), 256, 0, h->stream>>>(V, n_track, std::max(1, covis_thr / 2), I(o_vptr), Q(o_q2),
+                                                                          I(o_new), I(o_str), I(o_in));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(o_in), V, I(o_rptr));
+  k_str_table<<<bV, 256, 0, h->stream>>>(V, oldkey, covis_thr, I(o_in), I(o_rptr), I(o_str), I(o_qual), I(o_rows));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(o_qual), V, I(o_eptr));
+  k_str_edges<<<bV, 256, 0, h->stream>>>(V, V, I(o_qual), I(o_eptr), I(o_str), I(o_v1), I(o_v2), I(o_es));
+  SVS_CK(h, cudaGetLastError());
+  int rows = 0, ne = 0, old_in = 0;
+  SVS_CK(h, cudaMemcpyAsync(&rows, I(o_rptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&ne, I(o_eptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&old_in, I(o_in) + oldkey, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  if (!old_in) { h->err = "oldkey is absent from the strength table (slam_graph.cpp:165 asserts)"; return SVS_ERR_INVALID; }
+  if (table && rows) SVS_CK(h, cudaMemcpyAsync(table, I(o_rows), sizeof(int) * 2 * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  // addNewPointsToMap + addNewObsToOldPoints, then addNewEdges(LOCAL) on the grown map
+  if ((rc = keyframe_grow(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
+                          new_center, new_level, n_track, track_point, track_center, track_level)) != SVS_OK)
+    return rc;
+  if ((rc = grow_graph(h, V, ne, I(o_v1), I(o_v2), I(o_es), h->m.pose)) != SVS_OK) {
+    h->g = GraphDev{}; h->nnzN = 0;   // the map has V + 1 vertices now: a graph of V lists must not stay behind
+    return rc;
+  }
+  if (vertex_index) *vertex_index = V;
+  if (first_new_point) *first_new_point = Np;
+  if (n_table) *n_table = rows;
+  if (n_edges) *n_edges = ne;
+  return SVS_OK;
+}
+
+extern "C" int svs_map_add_edges(svs_map* h, int n, const int* v1, const int* v2, const int* strength, int moved_vertex,
+                                 const double* T_moved_from_w) {
+  if (!h || !h->d_map || n < 0 || (n && (!v1 || !v2 || !strength))) return SVS_ERR_INVALID;
+  int rc = needs_pose_graph(h);
+  if (rc != SVS_OK) return rc;
+  const int V = h->V;
+  if (moved_vertex < -1 || moved_vertex >= V || (moved_vertex >= 0 && !T_moved_from_w)) {
+    h->err = "moved_vertex outside [-1, V) or its pose missing";
+    return SVS_ERR_INVALID;
+  }
+  std::vector<std::pair<int, int>> pairs(n);
+  for (int k = 0; k < n; ++k) {
+    if (v1[k] < 0 || v1[k] >= V || v2[k] < 0 || v2[k] >= V || v1[k] == v2[k]) {
+      h->err = "an edge names a vertex outside [0, V) or joins a vertex to itself";
+      return SVS_ERR_INVALID;
+    }
+    pairs[k] = {std::min(v1[k], v2[k]), std::max(v1[k], v2[k])};
+  }
+  std::sort(pairs.begin(), pairs.end());
+  if (std::adjacent_find(pairs.begin(), pairs.end()) != pairs.end()) { h->err = "an edge is listed twice"; return SVS_ERR_INVALID; }
+  if (n == 0) return SVS_OK;
+  cudaSetDevice(h->device);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  const size_t o_v1 = take(sizeof(int) * n), o_v2 = take(sizeof(int) * n), o_es = take(sizeof(int) * n), o_bad = take(sizeof(int));
+  const size_t o_pose = take(sizeof(double) * 7 * V);
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->gw_cap, &h->d_gw));
+  char* W = h->d_gw;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  SVS_CK(h, cudaMemcpyAsync(W + o_v1, v1, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(W + o_v2, v2, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(W + o_es, strength, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(W + o_bad, 0, sizeof(int), h->stream));
+  k_edge_exists<<<(n + 255) / 256, 256, 0, h->stream>>>(h->g, V, n, I(o_v1), I(o_v2), I(o_bad));
+  SVS_CK(h, cudaGetLastError());
+  int bad = 0;
+  SVS_CK(h, cudaMemcpyAsync(&bad, W + o_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  if (bad) { h->err = "an edge is already in the pose graph (insertEdge asserts, slam_graph.hpp:353)"; return SVS_ERR_INVALID; }
+  // registerKeyframes / addLoopClosure place the moved vertex at its new pose while the constraints are computed
+  const double* poses = h->m.pose;
+  if (moved_vertex >= 0) {
+    double* P = reinterpret_cast<double*>(W + o_pose);
+    SVS_CK(h, cudaMemcpyAsync(P, h->m.pose, sizeof(double) * 7 * V, cudaMemcpyDeviceToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(P + 7 * (size_t)moved_vertex, T_moved_from_w, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+    poses = P;
+  }
+  return grow_graph(h, V, n, I(o_v1), I(o_v2), I(o_es), poses);
+}
+
+extern "C" {
 
 // the assembled edge list of the last svs_ba_set_problem_from_map, for inspection
 int svs_map_last_edges(svs_map* h, int E, int* e_point, int* e_pose, int* e_anchor, double* e_obs, double* e_info) {

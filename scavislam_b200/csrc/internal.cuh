@@ -123,4 +123,14 @@ __attribute__((visibility("hidden"))) void launch_scan(const int* cnt, int n, in
 // the vertex already observes keeps its observation.  Forgets the last assembled window, keeps the pose graph.
 __attribute__((visibility("hidden"))) int map_add_observations(svs_map* h, int vertex, int n, const int* d_point,
                                                                const double* d_center, const int* d_level);
+// SlamGraph::computeConstraint (constraint.cu's k_compute_constraint) on npairs pairs of device arrays, enqueued on
+// `stream`: poses [.][7] and feat_ptr / feat_point (each frame's points, ascending) indexed by frame, point_anchor /
+// xyz indexed by point; outputs T_1_from_2 [npairs][7], Lambda [npairs][36], strength [npairs].  scratch holds
+// npairs rows of scratch_stride = constraint_scratch_stride(largest feature table) doubles (none when that is 0).
+__attribute__((visibility("hidden"))) int constraint_scratch_stride(int max_feat);
+__attribute__((visibility("hidden"))) void launch_compute_constraint(const double* poses, const int* feat_ptr, const int* feat_point,
+                                                                     const int* point_anchor, const double* xyz, int npairs,
+                                                                     const int* v1, const int* v2, double* T_1_from_2,
+                                                                     double* Lambda, int* strength, double* scratch,
+                                                                     int scratch_stride, cudaStream_t stream);
 }  // namespace svs
