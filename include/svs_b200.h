@@ -949,6 +949,62 @@ int svs_map_add_keyframe_graph(svs_map *h, int oldkey, const double *T_newkey_fr
                                int *vertex_index, int *first_new_point, int *n_table, int *table, int *n_edges);
 int svs_map_add_edges(svs_map *h, int n, const int *v1, const int *v2, const int *strength, int moved_vertex,
                       const double *T_moved_from_w);
+/* ------------------------------------------------------------------ prepareForOptimization on the device map
+ * SlamGraph::prepareForOptimization(root, loop) (slam_graph.cpp:290-310) on the device graph, so that one back-end step
+ * is a chain of device calls (svs_map_add_keyframe_graph -> svs_map_prepare_for_optimization ->
+ * svs_ba_set_problem_from_map -> svs_ba_optimize -> svs_map_absorb) and only counts and the window reach the host.
+ *
+ * State.  The map keeps the window of its last prepare (the next call's old_window, WindowTable in ascending vertex order)
+ *   and one Edge::is_marginalized_ flag per directed entry of the graph; both entries of an edge carry the same value.
+ *   svs_map_set_graph and svs_map_set_pose_graph mark every entry marginalised and clear the window (the reference's state
+ *   at its first prepare: addNewEdges and addLoopClosure end in setConstraint).  svs_map_add_keyframe_graph and
+ *   svs_map_add_edges keep both: the new vertex is outside the window, new entries are marginalised, copied entries keep
+ *   their flag.  svs_map_set and svs_map_add_keyframe drop the graph and the window with it.  svs_map_select_window reads
+ *   the graph and changes nothing.
+ *
+ * svs_map_prepare_for_optimization, in order:
+ *   1 The window of svs_map_select_window(root, inner_window_size, double_window_size).
+ *   2 reinitializePoses (:665-725): a FIFO walk from root over the lists (strongest first).  A popped entry is skipped
+ *     when its vertex was visited or is not in the NEW window.  A vertex with a parent is re-posed, T_me =
+ *     getRelativePose_1_from_2(me, parent) * T_parent with T_parent the parent's updated pose, when it is marked or was
+ *     not in the old window.  A vertex is marked when it is `loop` or its parent was; the mark passes to its children.
+ *     getRelativePose_1_from_2 is the stored constraint of a marginalised edge, else T_me * T_parent^-1 of the current
+ *     poses.  loop == root re-poses every other window vertex reachable from root; a loop outside the window, or -1,
+ *     marks nothing.
+ *   3 P < 2: *do_optimization = 0; the window and the poses of step 2 stay (the next call's old window is this one) and
+ *     steps 4 and 5 are skipped.
+ *   4 unmargPosesEnteringInnerW (:728-759): every edge whose two ends are INNER in the new window is unmarginalised.
+ *   5 margPosesLeftInnerWindow (:848-904): every edge whose two ends were INNER in the old window and are not both INNER
+ *     now gets computeConstraint(v1, v2) at the poses of step 2, stored as svs_map_add_edges stores it (v2's entry for
+ *     v1 holds T_1_from_2, v1's entry for v2 its inverse, both Lambda) and marked marginalised.  The reference's double
+ *     loop writes each such edge twice and the second write wins, so v1 = the larger and v2 = the smaller vertex index
+ *     (Lambda depends on the median depth in v1's frame).
+ *   Outputs: those of svs_map_select_window with its orders and capacity rules; c_T_ji / c_Lambda are read after step 5,
+ *   so they go into svs_ba_set_problem_from_map unchanged.  *do_optimization = (P >= 2).  After a successful call no
+ *   window waits for svs_map_absorb (its pose writes would overwrite step 2's).  One host synchronisation, for the counts.
+ *   Refusals, each leaving the map, the graph and the window state bit-identical:
+ *     SVS_ERR_INVALID: root outside [0, V), loop outside [-1, V), inner_window_size >= double_window_size, a null
+ *       output, or a capacity too small (*P, *L, *C then hold the sizes needed; every count is found before any change);
+ *     SVS_ERR_STATE: a map without a pose graph with strengths and constraints (as the growth calls).
+ *   A CUDA error once the state has started to change returns SVS_ERR_CUDA with the map left without a pose graph.
+ *   The lists must be symmetric (each edge has both directed entries), as every graph the growth calls build is.
+ *   DEVIATIONS:
+ *     anchor poses come from the map, as for svs_map_add_edges (the reference chains computeAbsolutePose for an anchor
+ *       outside the new window);
+ *     the vertex index stands in for the frame id: the orientation of step 5 and the std::map orders are orders of
+ *       vertex index, which agree with frame ids when vertices are numbered in creation order (svs_map_add_keyframe*);
+ *     both directions of a constraint are stored (the reference stores one and inverts it on read), so a re-pose through
+ *       a marginalised edge can differ from the reference in the last bits;
+ *     the reference asserts when copyContraintsToG2o reads an unmarginalised pair with an OUTER end (possible only after
+ *       a call that stopped at P < 2); here the stored constraint is passed.
+ * svs_map_get_window_state: window_type[V] (0 outside, 1 INNER, 2 OUTER: the last prepare's window) and
+ *   marginalized[nnzN] (in svs_map_get_graph's entry order); either may be NULL.  *nnzN is always set; SVS_ERR_INVALID
+ *   when marginalized is asked for and cap < nnzN; SVS_ERR_STATE when the map has no graph. */
+int svs_map_prepare_for_optimization(svs_map *h, int root, int loop, int inner_window_size, int double_window_size,
+                                     int *do_optimization, int cap_P, int *P, int *window_vertex, unsigned char *inner,
+                                     int cap_L, int *L, int *active_point, int cap_C, int *C, int *c_i, int *c_j,
+                                     double *c_T_ji, double *c_Lambda);
+int svs_map_get_window_state(svs_map *h, int cap, int *nnzN, unsigned char *window_type, unsigned char *marginalized);
 /* the edge list of the last assembly (any output may be NULL); E must equal *num_edges */
 int svs_map_last_edges(svs_map *h, int E, int *e_point, int *e_pose, int *e_anchor, double *e_obs, double *e_info);
 

@@ -752,6 +752,37 @@ class DeviceMap {
     nn_ += 2 * (int)v1.size();
     return true;
   }
+  // prepareForOptimization(root_id, loop_id) (slam_graph.cpp:290-310; svs_map_prepare_for_optimization): the window of
+  // computeDoubleWindow, reinitializePoses, unmargPosesEnteringInnerW and margPosesLeftInnerWindow on the device.  *w
+  // receives the window with its constraints read after the marginalisation.  Returns whether the window holds >= 2
+  // frames (the reference's return value); throws std::runtime_error on a refused call.
+  bool prepareForOptimization(int root_id, int loop_id, int inner_window_size, int double_window_size, DoubleWindow* w) {
+    if (!ok_) throw std::runtime_error("no CUDA device");
+    const int capC = nn_ > 0 ? nn_ : 1;
+    w->window_vertex.resize(V_); w->inner.resize(V_); w->active_point.resize(Np_ > 0 ? Np_ : 1);
+    w->c_i.resize(capC); w->c_j.resize(capC); w->c_T.resize(7 * (size_t)capC); w->c_Lambda.resize(36 * (size_t)capC);
+    int P = 0, L = 0, C = 0, do_opt = 0;
+    const int rc = svs_map_prepare_for_optimization(h_, root_id, loop_id, inner_window_size, double_window_size, &do_opt, V_, &P,
+                                                    w->window_vertex.data(), w->inner.data(), (int)w->active_point.size(), &L,
+                                                    w->active_point.data(), capC, &C, w->c_i.data(), w->c_j.data(), w->c_T.data(),
+                                                    w->c_Lambda.data());
+    if (rc != SVS_OK) throw std::runtime_error(std::string("svs_map_prepare_for_optimization: ") + last_error());
+    w->window_vertex.resize(P); w->inner.resize(P); w->active_point.resize(L);
+    w->c_i.resize(C); w->c_j.resize(C); w->c_T.resize(7 * (size_t)C); w->c_Lambda.resize(36 * (size_t)C);
+    return do_opt != 0;
+  }
+  // the window of the last prepare (window_type[V]: 0 outside, 1 INNER, 2 OUTER) and Edge::is_marginalized of every
+  // directed entry in poseGraph's order (svs_map_get_window_state); throws std::runtime_error on a refused call
+  void windowState(std::vector<unsigned char>* window_type, std::vector<unsigned char>* marginalized) {
+    if (!ok_) throw std::runtime_error("no CUDA device");
+    int nn = 0;
+    if (svs_map_get_window_state(h_, 0, &nn, nullptr, nullptr) != SVS_OK)
+      throw std::runtime_error(std::string("svs_map_get_window_state: ") + last_error());
+    window_type->resize(V_ > 0 ? V_ : 1); marginalized->resize(nn > 0 ? nn : 1);
+    if (svs_map_get_window_state(h_, nn, &nn, window_type->data(), marginalized->data()) != SVS_OK)
+      throw std::runtime_error(std::string("svs_map_get_window_state: ") + last_error());
+    window_type->resize(V_); marginalized->resize(nn);
+  }
   // Backend::globalLoopClosure (backend.cpp:830-1001) on this map; semantics: svs_globalLoopClosure.  The matcher holds
   // the loop keyframe as its current frame and the keyframe pyramids in the slots vertex_slot names.  Returns true when
   // the loop was verified and the map grew; *res (when given) holds the counts of every stage reached, *tracks the gated

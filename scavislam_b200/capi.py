@@ -237,6 +237,7 @@ EXPORTS = [
     "svs_map_create", "svs_map_destroy", "svs_map_last_error", "svs_map_set", "svs_map_update_poses",
     "svs_map_update_points", "svs_map_get", "svs_map_absorb", "svs_map_set_graph", "svs_map_select_window",
     "svs_map_add_keyframe", "svs_map_set_pose_graph", "svs_map_get_graph", "svs_map_add_keyframe_graph", "svs_map_add_edges",
+    "svs_map_prepare_for_optimization", "svs_map_get_window_state",
     "svs_ba_set_problem_from_map", "svs_map_last_edges",
     "svs_chol6_create", "svs_chol6_destroy", "svs_chol6_last_error", "svs_chol6_init", "svs_chol6_solve",
     "svs_chol6_solve_blocks", "svs_chol6_solve_pattern",
@@ -367,6 +368,9 @@ def lib():
     L.svs_map_add_keyframe_graph.argtypes = [vp, C.c_int, c_dp, C.c_int, c_ip, c_dp, c_dp, c_ip, c_dp, c_ip, C.c_int, c_ip, c_dp,
                                              c_ip, C.c_int, C.c_int, C.c_int, c_ip, c_ip, c_ip, c_ip, c_ip]
     L.svs_map_add_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, C.c_int, c_dp]
+    L.svs_map_prepare_for_optimization.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, c_ip, C.c_int, c_ip, c_ip, c_up, C.c_int,
+                                                   c_ip, c_ip, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp]
+    L.svs_map_get_window_state.argtypes = [vp, C.c_int, c_ip, c_up, c_up]
     L.svs_ba_set_problem_from_map.argtypes = [vp, vp, C.c_int, c_ip, c_up, C.c_int, c_ip, C.c_int, c_ip, c_ip, c_dp, c_dp,
                                               C.POINTER(SvsCam), c_ip]
     L.svs_map_last_edges.argtypes = [vp, C.c_int, c_ip, c_ip, c_ip, c_dp, c_dp]
@@ -1502,6 +1506,31 @@ class DeviceMap(_Handle):
         T = None if T_moved_from_w is None else np.ascontiguousarray(T_moved_from_w, np.float64).reshape(7)
         self._ck(lib().svs_map_add_edges(self._h, len(a), _ip(a), _ip(b), _ip(s), int(moved_vertex), None if T is None else _dp(T)))
         self._nn = getattr(self, "_nn", 0) + 2 * len(a)
+
+    def prepare_for_optimization(self, root, loop, inner_window_size, double_window_size):
+        """SlamGraph::prepareForOptimization(root, loop) on the device: the window of select_window, reinitializePoses,
+        unmargPosesEnteringInnerW and margPosesLeftInnerWindow.  Returns select_window's dict, its constraints read after
+        the marginalisation, plus do_optimization (P >= 2)."""
+        capP, capL, capC = self.V, max(self.Np, 1), max(getattr(self, "_nn", 0), 1)
+        win, inner, act = np.zeros(capP, np.int32), np.zeros(capP, np.uint8), np.zeros(capL, np.int32)
+        ci, cj, cT, cL = np.zeros(capC, np.int32), np.zeros(capC, np.int32), np.zeros((capC, 7)), np.zeros((capC, 36))
+        P, L, Cn, do = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        self._ck(lib().svs_map_prepare_for_optimization(self._h, int(root), int(loop), int(inner_window_size), int(double_window_size),
+                                                        C.byref(do), capP, C.byref(P), _ip(win), inner.ctypes.data_as(c_up), capL,
+                                                        C.byref(L), _ip(act), capC, C.byref(Cn), _ip(ci), _ip(cj), _dp(cT), _dp(cL)))
+        P, L, Cn = P.value, L.value, Cn.value
+        return dict(window_vertex=win[:P].copy(), inner=inner[:P].copy(), active_point=act[:L].copy(), c_i=ci[:Cn].copy(),
+                    c_j=cj[:Cn].copy(), c_T=cT[:Cn].copy(), c_Lambda=cL[:Cn].copy(), do_optimization=bool(do.value))
+
+    def window_state(self):
+        """(window_type [V] uint8: 0 outside, 1 INNER, 2 OUTER -- the last prepare's window; marginalized [nnzN] uint8:
+        Edge::is_marginalized of each directed entry in get_graph's order)."""
+        nn = C.c_int()
+        self._ck(lib().svs_map_get_window_state(self._h, 0, C.byref(nn), None, None))
+        n = nn.value
+        wt, mg = np.zeros(max(self.V, 1), np.uint8), np.zeros(max(n, 1), np.uint8)
+        self._ck(lib().svs_map_get_window_state(self._h, n, C.byref(nn), wt.ctypes.data_as(c_up), mg.ctypes.data_as(c_up)))
+        return wt[:self.V].copy(), mg[:n].copy()
 
     def set_problem(self, ba, window_vertex, active_point, cam, fixed=None, c_i=(), c_j=(), c_T=None, c_Lambda=None):
         """Assembles the window on the device and loads it into `ba` (a BundleAdjuster).  Returns E."""

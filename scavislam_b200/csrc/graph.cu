@@ -145,6 +145,7 @@ struct GraphDev {
   const int* nbr_str;       // [nnzN] the strength key of neighbor_ids_ordered_by_strength (or nullptr)
   const double* nbr_T;      // [nnzN][7]  T_nbr_from_me of the directed entry (or nullptr)
   const double* nbr_Lam;    // [nnzN][36]
+  const unsigned char* nbr_mrg;   // [nnzN] Edge::is_marginalized_ of the entry's edge (both entries carry it)
 };
 
 // computeInitialDoubleWin (slam_graph.cpp:556-598).  The queue discipline IS the algorithm (a vertex joins when it
@@ -420,7 +421,7 @@ struct InsArgs {
   const int *v1, *v2, *es;        // the edges
   const double *T12, *Lam;        // their constraints: T_1_from_2, Lambda
   const int* nptr;                // the new lists
-  int *id, *str; double *T, *L;
+  int *id, *str; double *T, *L; unsigned char* mrg;
 };
 __global__ void k_ins_move_old(InsArgs a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -430,7 +431,7 @@ __global__ void k_ins_move_old(InsArgs a) {
   const int v = lo, s = a.g.nbr_str[i];
   int at = a.nptr[v] + (i - a.g.nbr_ptr[v]);
   for (int j = a.iptr[v]; j < a.iptr[v + 1]; ++j) at += a.es[a.iseq[j] >> 1] >= s;
-  a.id[at] = a.g.nbr_id[i]; a.str[at] = s;
+  a.id[at] = a.g.nbr_id[i]; a.str[at] = s; a.mrg[at] = a.g.nbr_mrg[i];
   for (int q = 0; q < 7; ++q) a.T[7 * (size_t)at + q] = a.g.nbr_T[7 * (size_t)i + q];
   for (int q = 0; q < 36; ++q) a.L[36 * (size_t)at + q] = a.g.nbr_Lam[36 * (size_t)i + q];
 }
@@ -449,12 +450,97 @@ __global__ void k_ins_move_new(InsArgs a, int V) {
     at += s2 > s || (s2 == s && a.iseq[r] > sq);
   }
   // setConstraint(v1, v2, T_1_from_2, Lambda, Lambda): v2's entry for v1 holds T_1_from_2, v1's entry its inverse
-  a.id[at] = (sq & 1) ? a.v1[k] : a.v2[k]; a.str[at] = s;
+  a.id[at] = (sq & 1) ? a.v1[k] : a.v2[k]; a.str[at] = s; a.mrg[at] = 1;
   double Ti[7];
   const double* T12 = a.T12 + 7 * (size_t)k;
   if (!(sq & 1)) svs::se3_inv(T12, Ti);
   for (int q = 0; q < 7; ++q) a.T[7 * (size_t)at + q] = (sq & 1) ? T12[q] : Ti[q];
   for (int q = 0; q < 36; ++q) a.L[36 * (size_t)at + q] = a.Lam[36 * (size_t)k + q];
+}
+
+// ------------------------------------------------------------------ prepareForOptimization (slam_graph.cpp:290-310)
+// reinitializePoses (:665-725).  The FIFO queue decides every vertex's parent, so one thread walks it as k_bfs does; a
+// node carries its parent, the parent's entry for it (T_me_from_parent when the edge is marginalised) and the mark.
+// Both skips happen at pop time.  The parent's pose is final once the parent has been popped.
+struct ReinitNode { int v, parent, entry, mark; };
+__global__ void k_reinit(GraphDev g, int root, int loop, const int* __restrict__ new_t, const int* __restrict__ old_t,
+                         double* __restrict__ pose, int* __restrict__ seen, ReinitNode* __restrict__ queue, int qcap) {
+  if (blockIdx.x || threadIdx.x) return;
+  int head = 0, tail = 0;
+  queue[tail++] = ReinitNode{root, -1, -1, 0};
+  while (head < tail) {
+    const ReinitNode n = queue[head++];
+    if (seen[n.v] || !new_t[n.v]) continue;      // "Avoid cycles!", then "Skip is it is not in double window"
+    seen[n.v] = 1;
+    const int mark = n.mark || n.v == loop;
+    if (n.parent >= 0 && (mark || !old_t[n.v])) {
+      // T_me = getRelativePose_1_from_2(me, parent) * T_parent: the stored constraint of a marginalised edge, else
+      // T_me * T_parent^-1 from the current poses
+      double Tp[7], R[7], Pi[7], Tm[7];
+      for (int q = 0; q < 7; ++q) { Tp[q] = pose[7 * (size_t)n.parent + q]; Tm[q] = pose[7 * (size_t)n.v + q]; }
+      if (g.nbr_mrg[n.entry]) {
+        for (int q = 0; q < 7; ++q) R[q] = g.nbr_T[7 * (size_t)n.entry + q];
+      } else {
+        svs::se3_inv(Tp, Pi);
+        svs::se3_mul(Tm, Pi, R);
+      }
+      svs::se3_mul(R, Tp, Tm);
+      for (int q = 0; q < 7; ++q) pose[7 * (size_t)n.v + q] = Tm[q];
+    }
+    for (int i = g.nbr_ptr[n.v]; i < g.nbr_ptr[n.v + 1] && tail < qcap; ++i) queue[tail++] = ReinitNode{g.nbr_id[i], n.v, i, mark};
+  }
+}
+
+// margPosesLeftInnerWindow's pairs (:848-904): edges whose two ends were INNER in the old window and are not both INNER
+// now, one row per edge from the entry of its larger end (v1 = max, v2 = min: the reference's second write wins);
+// the vertices they touch get their feature tables
+__device__ __forceinline__ bool leaves_inner(const int* old_t, const int* new_t, int a, int b) {
+  return a > b && old_t[a] == 1 && old_t[b] == 1 && !(new_t[a] == 1 && new_t[b] == 1);
+}
+__global__ void k_marg_count(int V, GraphDev g, const int* __restrict__ old_t, const int* __restrict__ new_t, int* __restrict__ cnt,
+                             int* __restrict__ touched) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= V) return;
+  int c = 0;
+  for (int i = g.nbr_ptr[a]; i < g.nbr_ptr[a + 1]; ++i) {
+    const int b = g.nbr_id[i];
+    if (leaves_inner(old_t, new_t, a, b)) { ++c; touched[b] = 1; }
+  }
+  cnt[a] = c;
+  if (c) touched[a] = 1;
+}
+__global__ void k_marg_emit(int V, GraphDev g, const int* __restrict__ old_t, const int* __restrict__ new_t, const int* __restrict__ ptr,
+                            int* __restrict__ v1, int* __restrict__ v2) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= V) return;
+  int at = ptr[a];
+  for (int i = g.nbr_ptr[a]; i < g.nbr_ptr[a + 1]; ++i)
+    if (leaves_inner(old_t, new_t, a, g.nbr_id[i])) { v1[at] = a; v2[at] = g.nbr_id[i]; ++at; }
+}
+// unmargPosesEnteringInnerW (:728-759): an edge between two INNER frames of the new window is unmarginalised
+__global__ void k_unmarg(int V, GraphDev g, const int* __restrict__ new_t, unsigned char* __restrict__ mrg) {
+  const int a = blockIdx.x * blockDim.x + threadIdx.x;
+  if (a >= V || new_t[a] != 1) return;
+  for (int i = g.nbr_ptr[a]; i < g.nbr_ptr[a + 1]; ++i)
+    if (new_t[g.nbr_id[i]] == 1) mrg[i] = 0;
+}
+// setConstraint(v1, v2, T_1_from_2, Lambda, Lambda) on both entries of pair k, as k_ins_move_new stores a new edge
+__global__ void k_marg_store(int n, GraphDev g, const int* __restrict__ v1, const int* __restrict__ v2, const double* __restrict__ T12,
+                             const double* __restrict__ Lam, double* __restrict__ T, double* __restrict__ L, unsigned char* __restrict__ mrg) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  double Ti[7];
+  svs::se3_inv(T12 + 7 * (size_t)k, Ti);
+  for (int side = 0; side < 2; ++side) {
+    const int me = side ? v1[k] : v2[k], nb = side ? v2[k] : v1[k];
+    const double* t = side ? Ti : T12 + 7 * (size_t)k;
+    for (int i = g.nbr_ptr[me]; i < g.nbr_ptr[me + 1]; ++i) {
+      if (g.nbr_id[i] != nb) continue;
+      for (int q = 0; q < 7; ++q) T[7 * (size_t)i + q] = t[q];
+      for (int q = 0; q < 36; ++q) L[36 * (size_t)i + q] = Lam[36 * (size_t)k + q];
+      mrg[i] = 1;
+    }
+  }
 }
 
 }  // namespace
@@ -478,7 +564,10 @@ struct svs_map : svs::Handle {
   char* d_gw = nullptr; size_t gw_cap = 0;           // work of the growth calls: strengths and staged edge lists
   char* d_ge = nullptr; size_t ge_cap = 0;           // ... feature tables, constraints and list insertion
   char* d_cs = nullptr; size_t cs_cap = 0;           // ... median scratch of the constraint kernel
-  char* d_sel = nullptr; size_t sel_cap = 0;   // work buffers of svs_map_select_window
+  char* d_sel = nullptr; size_t sel_cap = 0;   // work buffers of svs_map_select_window / svs_map_prepare_for_optimization
+  // the window of the last svs_map_prepare_for_optimization (0 / 1 INNER / 2 OUTER) for vertices [0, wtV); vertices
+  // from wtV on (added since) are outside it.  wtV = 0: no window yet
+  int* d_wt = nullptr; size_t wt_cap = 0; int wtV = 0;
 };
 
 static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
@@ -524,7 +613,7 @@ void svs_map_destroy(svs_map* h) {
   if (!h) return;
   svs::begin_close(h);
   cudaFree(h->d_map); cudaFree(h->d_work); cudaFree(h->d_upd); cudaFree(h->d_graph); cudaFree(h->d_sel);
-  cudaFree(h->d_graph2); cudaFree(h->d_gw); cudaFree(h->d_ge); cudaFree(h->d_cs);
+  cudaFree(h->d_graph2); cudaFree(h->d_gw); cudaFree(h->d_ge); cudaFree(h->d_cs); cudaFree(h->d_wt);
   delete h;
 }
 
@@ -566,7 +655,7 @@ int svs_map_set(svs_map* h, int V, const double* T_me_from_world, int Np, const 
   }
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   map_bind(h, B, lo, V, Np, nnz);
-  h->g = GraphDev{}; h->nnzN = 0;   // a new map: its pose graph comes with svs_map_set_graph
+  h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // a new map: its pose graph comes with svs_map_set_graph
   return SVS_OK;
 }
 
@@ -726,7 +815,7 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
 
 // ------------------------------------------------------------------ pose graph, window selection, growth
 
-struct GraphLayout { size_t o_ptr, o_id, o_str, o_T, o_L, total; };
+struct GraphLayout { size_t o_ptr, o_id, o_str, o_T, o_L, o_M, total; };
 static GraphLayout graph_layout(int V, int nn) {
   GraphLayout lo{};
   size_t off = 0;
@@ -735,6 +824,7 @@ static GraphLayout graph_layout(int V, int nn) {
   lo.o_str = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
   lo.o_T = off; off += al256(sizeof(double) * 7 * (size_t)std::max(nn, 1));
   lo.o_L = off; off += al256(sizeof(double) * 36 * (size_t)std::max(nn, 1));
+  lo.o_M = off; off += al256((size_t)std::max(nn, 1));
   lo.total = off;
   return lo;
 }
@@ -743,6 +833,7 @@ static void graph_bind(svs_map* h, char* B, const GraphLayout& lo, int nn, bool 
   h->g.nbr_str = strength ? reinterpret_cast<const int*>(B + lo.o_str) : nullptr;
   h->g.nbr_T = constraints ? reinterpret_cast<const double*>(B + lo.o_T) : nullptr;
   h->g.nbr_Lam = constraints ? reinterpret_cast<const double*>(B + lo.o_L) : nullptr;
+  h->g.nbr_mrg = reinterpret_cast<const unsigned char*>(B + lo.o_M);
   h->nnzN = nn;
 }
 
@@ -775,8 +866,11 @@ static int upload_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const
       SVS_CK(h, cudaMemcpyAsync(B + lo.o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     }
   }
+  // the reference's state at its first prepareForOptimization: addNewEdges and addLoopClosure end in setConstraint
+  SVS_CK(h, cudaMemsetAsync(B + lo.o_M, 1, (size_t)std::max(nn, 1), h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   graph_bind(h, B, lo, nn, pose_graph, pose_graph || nbr_T != nullptr);
+  h->wtV = 0;
   return SVS_OK;
 }
 
@@ -816,66 +910,69 @@ int svs_map_get_graph(svs_map* h, int cap, int* nnzN, int* nbr_ptr, int* nbr_id,
   return SVS_OK;
 }
 
-int svs_map_select_window(svs_map* h, int root, int inner_window_size, int double_window_size, int cap_P, int* P_out,
-                          int* window_vertex, unsigned char* inner, int cap_L, int* L_out, int* active_point, int cap_C,
-                          int* C_out, int* c_i, int* c_j, double* c_T, double* c_Lambda) {
-  if (!h || !h->d_map || !P_out || !window_vertex || !L_out || (cap_L && !active_point) || cap_P <= 0 || cap_L < 0 || cap_C < 0)
-    return SVS_ERR_INVALID;
-  if (!h->g.nbr_ptr) { h->err = "svs_map_set_graph has not been called for this map"; return SVS_ERR_STATE; }
+}  // extern "C"
+
+// ------------------------------------------------------------------ window selection (svs_map_select_window and prepare)
+struct SelWork { size_t o_type, o_ext, o_wtype, o_flag, o_ptrV, o_win, o_pos, o_act, o_ptrP, o_actl, o_q, o_cc, o_cp, o_ci, o_cj, o_cT, o_cL; };
+template <class Take>
+static SelWork sel_take(Take take, int V, int Np, int nn) {
+  SelWork s;
+  s.o_type = take(sizeof(int) * V); s.o_ext = take(sizeof(int) * V); s.o_wtype = take(sizeof(int) * V);
+  s.o_flag = take(sizeof(int) * V); s.o_ptrV = take(sizeof(int) * ((size_t)V + 1)); s.o_win = take(sizeof(int) * V);
+  s.o_pos = take(sizeof(int) * V); s.o_act = take(sizeof(int) * (size_t)std::max(Np, 1));
+  s.o_ptrP = take(sizeof(int) * ((size_t)Np + 1)); s.o_actl = take(sizeof(int) * (size_t)std::max(Np, 1));
+  s.o_q = take(sizeof(int) * ((size_t)nn + 1)); s.o_cc = take(sizeof(int) * V); s.o_cp = take(sizeof(int) * ((size_t)V + 1));
+  s.o_ci = take(sizeof(int) * (size_t)std::max(nn, 1)); s.o_cj = take(sizeof(int) * (size_t)std::max(nn, 1));
+  s.o_cT = take(sizeof(double) * 7 * (size_t)std::max(nn, 1)); s.o_cL = take(sizeof(double) * 36 * (size_t)std::max(nn, 1));
+  return s;
+}
+
+// computeInitialDoubleWin + computeActivePointsAndExtendOuterWindow and the pair count of copyContraintsToG2o, enqueued
+// on the map's stream; the counts P, L, C go to counts[0..2] once the stream is synchronised.  The window types (0 / 1
+// INNER / 2 OUTER) are left in W + s.o_wtype.
+static int sel_enqueue(svs_map* h, char* W, const SelWork& s, int root, int inner, int dbl, int* counts) {
   const int V = h->V, Np = h->Np, nn = h->nnzN;
-  if (root < 0 || root >= V || inner_window_size < 0 || inner_window_size >= double_window_size) {   // assert at slam_graph.cpp:563
-    h->err = "root outside [0, V) or inner_window_size >= double_window_size";
-    return SVS_ERR_INVALID;
-  }
-  cudaSetDevice(h->device);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_type = take(sizeof(int) * V), o_ext = take(sizeof(int) * V), o_wtype = take(sizeof(int) * V);
-  const size_t o_flag = take(sizeof(int) * V), o_ptrV = take(sizeof(int) * ((size_t)V + 1)), o_win = take(sizeof(int) * V);
-  const size_t o_pos = take(sizeof(int) * V), o_act = take(sizeof(int) * (size_t)std::max(Np, 1));
-  const size_t o_ptrP = take(sizeof(int) * ((size_t)Np + 1)), o_actl = take(sizeof(int) * (size_t)std::max(Np, 1));
-  const size_t o_q = take(sizeof(int) * ((size_t)nn + 1)), o_cc = take(sizeof(int) * V), o_cp = take(sizeof(int) * ((size_t)V + 1));
-  const size_t o_ci = take(sizeof(int) * (size_t)std::max(nn, 1)), o_cj = take(sizeof(int) * (size_t)std::max(nn, 1));
-  const size_t o_cT = take(sizeof(double) * 7 * (size_t)std::max(nn, 1)), o_cL = take(sizeof(double) * 36 * (size_t)std::max(nn, 1));
-  SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
-  char* W = h->d_sel;
   auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  SVS_CK(h, cudaMemsetAsync(I(o_type), 0, sizeof(int) * V, h->stream));
-  SVS_CK(h, cudaMemsetAsync(I(o_ext), 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(I(s.o_type), 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(I(s.o_ext), 0, sizeof(int) * V, h->stream));
   const int bV = (V + 255) / 256, bP = (std::max(Np, 1) + 255) / 256;
-  k_bfs<<<1, 32, 0, h->stream>>>(V, h->g, root, inner_window_size, double_window_size, I(o_type), I(o_q), nn + 1);
-  if (Np) k_active<<<bP, 256, 0, h->stream>>>(h->m, h->g, I(o_type), I(o_ext), I(o_act));
-  k_window_flags<<<bV, 256, 0, h->stream>>>(V, I(o_type), I(o_ext), I(o_wtype), I(o_flag));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_flag), V, I(o_ptrV));
-  k_compact<<<bV, 256, 0, h->stream>>>(V, I(o_flag), I(o_ptrV), I(o_win), I(o_pos));
+  k_bfs<<<1, 32, 0, h->stream>>>(V, h->g, root, inner, dbl, I(s.o_type), I(s.o_q), nn + 1);
+  if (Np) k_active<<<bP, 256, 0, h->stream>>>(h->m, h->g, I(s.o_type), I(s.o_ext), I(s.o_act));
+  k_window_flags<<<bV, 256, 0, h->stream>>>(V, I(s.o_type), I(s.o_ext), I(s.o_wtype), I(s.o_flag));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_flag), V, I(s.o_ptrV));
+  k_compact<<<bV, 256, 0, h->stream>>>(V, I(s.o_flag), I(s.o_ptrV), I(s.o_win), I(s.o_pos));
   if (Np) {
-    k_scan<<<1, 1024, 0, h->stream>>>(I(o_act), Np, I(o_ptrP));
-    k_compact<<<bP, 256, 0, h->stream>>>(Np, I(o_act), I(o_ptrP), I(o_actl), nullptr);
+    k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_act), Np, I(s.o_ptrP));
+    k_compact<<<bP, 256, 0, h->stream>>>(Np, I(s.o_act), I(s.o_ptrP), I(s.o_actl), nullptr);
   }
-  k_pair_count<<<bV, 256, 0, h->stream>>>(V, h->g, I(o_wtype), I(o_cc));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_cc), V, I(o_cp));
-  k_pair_emit<<<bV, 256, 0, h->stream>>>(V, h->g, I(o_wtype), I(o_pos), I(o_cp), I(o_ci), I(o_cj),
-                                        reinterpret_cast<double*>(W + o_cT), reinterpret_cast<double*>(W + o_cL));
+  k_pair_count<<<bV, 256, 0, h->stream>>>(V, h->g, I(s.o_wtype), I(s.o_cc));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_cc), V, I(s.o_cp));
   SVS_CK(h, cudaGetLastError());
-  int P = 0, L = 0, C = 0;
-  SVS_CK(h, cudaMemcpyAsync(&P, I(o_ptrV) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (Np) SVS_CK(h, cudaMemcpyAsync(&L, I(o_ptrP) + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(&C, I(o_cp) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaStreamSynchronize(h->stream));
-  *P_out = P; *L_out = L;
-  if (C_out) *C_out = C;
-  if (P > cap_P || L > cap_L || (c_i && C > cap_C)) { h->err = "window, active points or constraints exceed the caller's capacity"; return SVS_ERR_INVALID; }
-  SVS_CK(h, cudaMemcpyAsync(window_vertex, I(o_win), sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
-  if (L) SVS_CK(h, cudaMemcpyAsync(active_point, I(o_actl), sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
+  counts[1] = 0;
+  SVS_CK(h, cudaMemcpyAsync(counts, I(s.o_ptrV) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (Np) SVS_CK(h, cudaMemcpyAsync(counts + 1, I(s.o_ptrP) + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts + 2, I(s.o_cp) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  return SVS_OK;
+}
+
+// the window's outputs once the counts fit: the pairs with the graph's constraints as they are now, then the copies
+static int sel_emit(svs_map* h, char* W, const SelWork& s, int P, int L, int C, int* window_vertex, unsigned char* inner,
+                    int* active_point, int* c_i, int* c_j, double* c_T, double* c_Lambda) {
+  const int V = h->V;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  k_pair_emit<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, I(s.o_wtype), I(s.o_pos), I(s.o_cp), I(s.o_ci), I(s.o_cj),
+                                                      reinterpret_cast<double*>(W + s.o_cT), reinterpret_cast<double*>(W + s.o_cL));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(window_vertex, I(s.o_win), sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(active_point, I(s.o_actl), sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
   h->h_winpos.resize(V);
-  SVS_CK(h, cudaMemcpyAsync(h->h_winpos.data(), I(o_wtype), sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_winpos.data(), I(s.o_wtype), sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
   if (c_i && C) {
     if (!c_j || !c_T || !c_Lambda) return SVS_ERR_INVALID;
-    SVS_CK(h, cudaMemcpyAsync(c_i, I(o_ci), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_j, I(o_cj), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_T, W + o_cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_Lambda, W + o_cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_i, I(s.o_ci), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_j, I(s.o_cj), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_T, W + s.o_cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_Lambda, W + s.o_cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
   }
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (inner)
@@ -883,7 +980,36 @@ int svs_map_select_window(svs_map* h, int root, int inner_window_size, int doubl
   return SVS_OK;
 }
 
-}  // extern "C"
+static bool sel_args_ok(int cap_P, int* P_out, int* window_vertex, int cap_L, int* L_out, int* active_point, int cap_C) {
+  return P_out && window_vertex && L_out && (!cap_L || active_point) && cap_P > 0 && cap_L >= 0 && cap_C >= 0;
+}
+
+extern "C" int svs_map_select_window(svs_map* h, int root, int inner_window_size, int double_window_size, int cap_P, int* P_out,
+                                     int* window_vertex, unsigned char* inner, int cap_L, int* L_out, int* active_point, int cap_C,
+                                     int* C_out, int* c_i, int* c_j, double* c_T, double* c_Lambda) {
+  if (!h || !h->d_map || !sel_args_ok(cap_P, P_out, window_vertex, cap_L, L_out, active_point, cap_C)) return SVS_ERR_INVALID;
+  if (!h->g.nbr_ptr) { h->err = "svs_map_set_graph has not been called for this map"; return SVS_ERR_STATE; }
+  const int V = h->V;
+  if (root < 0 || root >= V || inner_window_size < 0 || inner_window_size >= double_window_size) {   // assert at slam_graph.cpp:563
+    h->err = "root outside [0, V) or inner_window_size >= double_window_size";
+    return SVS_ERR_INVALID;
+  }
+  cudaSetDevice(h->device);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  const SelWork s = sel_take(take, V, h->Np, h->nnzN);
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
+  int counts[3] = {0, 0, 0};
+  if (int rc = sel_enqueue(h, h->d_sel, s, root, inner_window_size, double_window_size, counts)) return rc;
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  const int P = counts[0], L = counts[1], C = counts[2];
+  *P_out = P; *L_out = L;
+  if (C_out) *C_out = C;
+  if (P > cap_P || L > cap_L || (c_i && C > cap_C)) { h->err = "window, active points or constraints exceed the caller's capacity"; return SVS_ERR_INVALID; }
+  return sel_emit(h, h->d_sel, s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
+}
+
 
 static int keyframe_check(svs_map* h, int oldkey, const double* T_newkey_from_oldkey, int n_new, const int* new_anchor,
                           const double* new_xyz_anchor, const double* new_anchor_center, const int* new_anchor_level,
@@ -981,10 +1107,53 @@ extern "C" int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newk
     rc = keyframe_grow(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
                        new_center, new_level, n_track, track_point, track_center, track_level);
   if (rc != SVS_OK) return rc;
-  h->g = GraphDev{}; h->nnzN = 0;          // the pose graph changed with the new vertex: svs_map_set_graph again
+  h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // the pose graph changed with the new vertex: svs_map_set_graph again
   if (vertex_index) *vertex_index = V;
   if (first_new_point) *first_new_point = Np;
   return SVS_OK;
+}
+
+// The feature tables (points in ascending id) of the vertices flagged in `touched`, for computeConstraint.  Clear,
+// flag, count (nfeat and the largest table go to ctl[0], ctl[1]), then -- once the caller has read ctl on the host --
+// build: emit one key (vertex, point) per observation, sort with CUB, unpack into point.
+struct FeatWork { size_t o_touch, o_fcnt, o_fptr, o_fcur, o_ctl, o_fkey, o_fkey2, o_fpt; };
+template <class Take>
+static FeatWork feat_take(Take take, int V, size_t nf) {
+  FeatWork f;
+  f.o_touch = take(sizeof(int) * V); f.o_fcnt = take(sizeof(int) * V); f.o_fptr = take(sizeof(int) * ((size_t)V + 1));
+  f.o_fcur = take(sizeof(int) * V); f.o_ctl = take(sizeof(int) * 4);
+  f.o_fkey = take(8 * nf); f.o_fkey2 = take(8 * nf); f.o_fpt = take(sizeof(int) * nf);
+  return f;
+}
+static size_t feat_sort_bytes(size_t nf) {
+  size_t b = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nf);
+  return b;
+}
+static cudaError_t feat_clear(svs_map* h, char* W, const FeatWork& f) {
+  cudaError_t e = cudaSuccess;
+  for (size_t o : {f.o_touch, f.o_fcnt, f.o_fcur})
+    if (e == cudaSuccess) e = cudaMemsetAsync(W + o, 0, sizeof(int) * h->V, h->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(W + f.o_ctl, 0, sizeof(int) * 4, h->stream);
+  return e;
+}
+static cudaError_t feat_count(svs_map* h, char* W, const FeatWork& f) {
+  const int V = h->V, Np = h->Np;
+  int* touched = reinterpret_cast<int*>(W + f.o_touch); int* fcnt = reinterpret_cast<int*>(W + f.o_fcnt);
+  int* fptr = reinterpret_cast<int*>(W + f.o_fptr); int* ctl = reinterpret_cast<int*>(W + f.o_ctl);
+  if (Np) k_feat_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, touched, fcnt);
+  k_scan<<<1, 1024, 0, h->stream>>>(fcnt, V, fptr);
+  k_max<<<(V + 255) / 256, 256, 0, h->stream>>>(V, fcnt, ctl + 1);
+  return cudaMemcpyAsync(ctl, fptr + V, sizeof(int), cudaMemcpyDeviceToDevice, h->stream);
+}
+static cudaError_t feat_build(svs_map* h, char* W, const FeatWork& f, int nfeat, void* tmp, size_t tmp_bytes) {
+  if (!nfeat) return cudaSuccess;
+  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
+  k_feat_emit<<<(h->Np + 255) / 256, 256, 0, h->stream>>>(h->m, reinterpret_cast<int*>(W + f.o_touch), reinterpret_cast<int*>(W + f.o_fptr),
+                                                          reinterpret_cast<int*>(W + f.o_fcur), U(f.o_fkey));
+  cudaError_t e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, U(f.o_fkey), U(f.o_fkey2), nfeat, 0, 64, h->stream);
+  k_feat_unpack<<<(nfeat + 255) / 256, 256, 0, h->stream>>>(nfeat, U(f.o_fkey2), reinterpret_cast<int*>(W + f.o_fpt));
+  return e;
 }
 
 // addNewEdges' list insertion and setConstraint for n edges (device arrays v1, v2, strength on the map's stream):
@@ -992,19 +1161,15 @@ extern "C" int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newk
 // vertex moved), then the new lists with their constraints.  The graph before the call has gV <= V lists; the lists of
 // vertices gV..V-1 start empty.
 static int grow_graph(svs_map* h, int gV, int n, const int* d_v1, const int* d_v2, const int* d_es, const double* d_poses) {
-  const int V = h->V, Np = h->Np, nn_old = h->nnzN, nn = nn_old + 2 * n;
+  const int V = h->V, nn_old = h->nnzN, nn = nn_old + 2 * n;
   const size_t nf = (size_t)std::max(h->nnz, 1), ni = (size_t)std::max(2 * n, 1);
   cudaSetDevice(h->device);
-  size_t tmp_bytes = 0, b = 0;
-  cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nf);
-  tmp_bytes = std::max(tmp_bytes, b);
+  size_t tmp_bytes = feat_sort_bytes(nf), b = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)ni);
   tmp_bytes = std::max(tmp_bytes, b);
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_touch = take(sizeof(int) * V), o_fcnt = take(sizeof(int) * V), o_fptr = take(sizeof(int) * ((size_t)V + 1));
-  const size_t o_fcur = take(sizeof(int) * V), o_ctl = take(sizeof(int) * 4);
-  const size_t o_fkey = take(8 * nf), o_fkey2 = take(8 * nf), o_fpt = take(sizeof(int) * nf);
+  const FeatWork f = feat_take(take, V, nf);
   const size_t o_T12 = take(sizeof(double) * 7 * ni), o_Lam = take(sizeof(double) * 36 * ni), o_cs = take(sizeof(int) * ni);
   const size_t o_icnt = take(sizeof(int) * V), o_iptr = take(sizeof(int) * ((size_t)V + 1)), o_ncnt = take(sizeof(int) * V);
   const size_t o_tgt = take(sizeof(int) * ni), o_tgt2 = take(sizeof(int) * ni), o_seq = take(sizeof(int) * ni);
@@ -1015,32 +1180,23 @@ static int grow_graph(svs_map* h, int gV, int n, const int* d_v1, const int* d_v
   SVS_CK(h, svs::grow(lo.total, &h->graph2_cap, &h->d_graph2));
   char* W = h->d_ge;
   auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
   auto D = [&](size_t o) { return reinterpret_cast<double*>(W + o); };
   const int bV = (V + 255) / 256;
-  for (size_t o : {o_touch, o_fcnt, o_fcur, o_icnt}) SVS_CK(h, cudaMemsetAsync(W + o, 0, sizeof(int) * V, h->stream));
-  SVS_CK(h, cudaMemsetAsync(W + o_ctl, 0, sizeof(int) * 4, h->stream));
+  SVS_CK(h, feat_clear(h, W, f));
+  SVS_CK(h, cudaMemsetAsync(W + o_icnt, 0, sizeof(int) * V, h->stream));
   if (n) {
-    k_touch<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(o_touch));
-    if (Np) k_feat_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, I(o_touch), I(o_fcnt));
-    k_scan<<<1, 1024, 0, h->stream>>>(I(o_fcnt), V, I(o_fptr));
-    k_max<<<bV, 256, 0, h->stream>>>(V, I(o_fcnt), I(o_ctl) + 1);
-    SVS_CK(h, cudaMemcpyAsync(I(o_ctl), I(o_fptr) + V, sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
+    k_touch<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(f.o_touch));
+    SVS_CK(h, feat_count(h, W, f));
     int ctl[2] = {0, 0};
-    SVS_CK(h, cudaMemcpyAsync(ctl, I(o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(ctl, I(f.o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
     SVS_CK(h, cudaStreamSynchronize(h->stream));
     const int nfeat = ctl[0], stride = svs::constraint_scratch_stride(ctl[1]);
-    if (nfeat) {
-      k_feat_emit<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, I(o_touch), I(o_fptr), I(o_fcur), U(o_fkey));
-      size_t tb = tmp_bytes;
-      SVS_CK(h, cub::DeviceRadixSort::SortKeys(W + o_tmp, tb, U(o_fkey), U(o_fkey2), nfeat, 0, 64, h->stream));
-      k_feat_unpack<<<(nfeat + 255) / 256, 256, 0, h->stream>>>(nfeat, U(o_fkey2), I(o_fpt));
-    }
+    SVS_CK(h, feat_build(h, W, f, nfeat, W + o_tmp, tmp_bytes));
     if (stride) {
       SVS_CK(h, cudaStreamSynchronize(h->stream));
       SVS_CK(h, svs::grow(sizeof(double) * (size_t)stride * n, &h->cs_cap, &h->d_cs));
     }
-    svs::launch_compute_constraint(d_poses, I(o_fptr), I(o_fpt), h->m.anchor, h->m.xyz, n, d_v1, d_v2, D(o_T12), D(o_Lam), I(o_cs),
+    svs::launch_compute_constraint(d_poses, I(f.o_fptr), I(f.o_fpt), h->m.anchor, h->m.xyz, n, d_v1, d_v2, D(o_T12), D(o_Lam), I(o_cs),
                                    reinterpret_cast<double*>(h->d_cs), stride, h->stream);
     k_ins_keys<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(o_tgt), I(o_seq), I(o_icnt));
     size_t tb = tmp_bytes;   // a stable sort: inside one target the inserts stay in sequence order
@@ -1056,6 +1212,7 @@ static int grow_graph(svs_map* h, int gV, int n, const int* d_v1, const int* d_v
   a.nptr = reinterpret_cast<const int*>(B + lo.o_ptr);
   a.id = reinterpret_cast<int*>(B + lo.o_id); a.str = reinterpret_cast<int*>(B + lo.o_str);
   a.T = reinterpret_cast<double*>(B + lo.o_T); a.L = reinterpret_cast<double*>(B + lo.o_L);
+  a.mrg = reinterpret_cast<unsigned char*>(B + lo.o_M);
   if (nn_old) k_ins_move_old<<<(nn_old + 255) / 256, 256, 0, h->stream>>>(a);
   if (n) k_ins_move_new<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(a, V);
   SVS_CK(h, cudaGetLastError());
@@ -1151,7 +1308,7 @@ extern "C" int svs_map_add_keyframe_graph(svs_map* h, int oldkey, const double* 
                           new_center, new_level, n_track, track_point, track_center, track_level)) != SVS_OK)
     return rc;
   if ((rc = grow_graph(h, V, ne, I(o_v1), I(o_v2), I(o_es), h->m.pose)) != SVS_OK) {
-    h->g = GraphDev{}; h->nnzN = 0;   // the map has V + 1 vertices now: a graph of V lists must not stay behind
+    h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // the map has V + 1 vertices now: a graph of V lists must not stay behind
     return rc;
   }
   if (vertex_index) *vertex_index = V;
@@ -1210,6 +1367,123 @@ extern "C" int svs_map_add_edges(svs_map* h, int n, const int* v1, const int* v2
     poses = P;
   }
   return grow_graph(h, V, n, I(o_v1), I(o_v2), I(o_es), poses);
+}
+
+// ------------------------------------------------------------------ prepareForOptimization
+struct PrepWork { SelWork s; FeatWork f; size_t o_old, o_seen, o_q, o_mcnt, o_mptr, o_v1, o_v2, o_T12, o_Lam, o_cs, o_tmp; };
+
+// steps 2, 4 and 5 once the counts have fitted: from here on the map changes
+static int prepare_apply(svs_map* h, const PrepWork& w, int root, int loop, int P, int nM, int nfeat, int max_feat) {
+  const int V = h->V, nn = h->nnzN;
+  char* W = h->d_sel;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  auto D = [&](size_t o) { return reinterpret_cast<double*>(W + o); };
+  const int* new_t = I(w.s.o_wtype);
+  h->d_win_last = nullptr;   // absorbing the previous window would overwrite the reinitialised poses
+  SVS_CK(h, cudaMemsetAsync(I(w.o_seen), 0, sizeof(int) * V, h->stream));
+  k_reinit<<<1, 32, 0, h->stream>>>(h->g, root, loop, new_t, I(w.o_old), const_cast<double*>(h->m.pose), I(w.o_seen),
+                                    reinterpret_cast<ReinitNode*>(W + w.o_q), nn + 1);
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(sizeof(int) * (size_t)V, &h->wt_cap, &h->d_wt));
+  SVS_CK(h, cudaMemcpyAsync(h->d_wt, new_t, sizeof(int) * (size_t)V, cudaMemcpyDeviceToDevice, h->stream));
+  h->wtV = V;
+  if (P >= 2) {
+    const GraphLayout lo = graph_layout(V, nn);
+    unsigned char* mrg = reinterpret_cast<unsigned char*>(h->d_graph + lo.o_M);
+    const int bV = (V + 255) / 256;
+    k_unmarg<<<bV, 256, 0, h->stream>>>(V, h->g, new_t, mrg);
+    if (nM) {
+      k_marg_emit<<<bV, 256, 0, h->stream>>>(V, h->g, I(w.o_old), new_t, I(w.o_mptr), I(w.o_v1), I(w.o_v2));
+      SVS_CK(h, feat_build(h, W, w.f, nfeat, W + w.o_tmp, feat_sort_bytes((size_t)std::max(h->nnz, 1))));
+      const int stride = svs::constraint_scratch_stride(max_feat);
+      if (stride) {
+        SVS_CK(h, cudaStreamSynchronize(h->stream));
+        SVS_CK(h, svs::grow(sizeof(double) * (size_t)stride * nM, &h->cs_cap, &h->d_cs));
+      }
+      // computeConstraint(v1 = max, v2 = min) at the reinitialised poses
+      svs::launch_compute_constraint(h->m.pose, I(w.f.o_fptr), I(w.f.o_fpt), h->m.anchor, h->m.xyz, nM, I(w.o_v1), I(w.o_v2),
+                                     D(w.o_T12), D(w.o_Lam), I(w.o_cs), reinterpret_cast<double*>(h->d_cs), stride, h->stream);
+      k_marg_store<<<(nM + 255) / 256, 256, 0, h->stream>>>(nM, h->g, I(w.o_v1), I(w.o_v2), D(w.o_T12), D(w.o_Lam),
+                                                            reinterpret_cast<double*>(h->d_graph + lo.o_T),
+                                                            reinterpret_cast<double*>(h->d_graph + lo.o_L), mrg);
+    }
+  }
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  return SVS_OK;
+}
+
+extern "C" int svs_map_prepare_for_optimization(svs_map* h, int root, int loop, int inner_window_size, int double_window_size,
+                                                int* do_optimization, int cap_P, int* P_out, int* window_vertex,
+                                                unsigned char* inner, int cap_L, int* L_out, int* active_point, int cap_C,
+                                                int* C_out, int* c_i, int* c_j, double* c_T, double* c_Lambda) {
+  svs::NvtxRange nvtx_("prepareForOptimization");
+  if (!h || !h->d_map || !do_optimization || !sel_args_ok(cap_P, P_out, window_vertex, cap_L, L_out, active_point, cap_C))
+    return SVS_ERR_INVALID;
+  int rc = needs_pose_graph(h);
+  if (rc != SVS_OK) return rc;
+  const int V = h->V, nn = h->nnzN;
+  if (root < 0 || root >= V || loop < -1 || loop >= V || inner_window_size < 0 || inner_window_size >= double_window_size) {
+    h->err = "root outside [0, V), loop outside [-1, V) or inner_window_size >= double_window_size";
+    return SVS_ERR_INVALID;
+  }
+  cudaSetDevice(h->device);
+  const size_t nf = (size_t)std::max(h->nnz, 1), ne = (size_t)std::max(nn, 1);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  PrepWork w;
+  w.s = sel_take(take, V, h->Np, nn);
+  w.f = feat_take(take, V, nf);
+  w.o_old = take(sizeof(int) * V); w.o_seen = take(sizeof(int) * V); w.o_q = take(sizeof(ReinitNode) * ((size_t)nn + 1));
+  w.o_mcnt = take(sizeof(int) * V); w.o_mptr = take(sizeof(int) * ((size_t)V + 1));
+  w.o_v1 = take(sizeof(int) * ne); w.o_v2 = take(sizeof(int) * ne);
+  w.o_T12 = take(sizeof(double) * 7 * ne); w.o_Lam = take(sizeof(double) * 36 * ne); w.o_cs = take(sizeof(int) * ne);
+  w.o_tmp = take(feat_sort_bytes(nf));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
+  char* W = h->d_sel;
+  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  // every count the call needs, before anything changes: window, active points, pairs, marginalised edges, features
+  SVS_CK(h, cudaMemsetAsync(I(w.o_old), 0, sizeof(int) * V, h->stream));   // vertices from wtV on are outside the old window
+  if (h->wtV) SVS_CK(h, cudaMemcpyAsync(I(w.o_old), h->d_wt, sizeof(int) * (size_t)h->wtV, cudaMemcpyDeviceToDevice, h->stream));
+  int counts[6] = {0, 0, 0, 0, 0, 0};
+  if ((rc = sel_enqueue(h, W, w.s, root, inner_window_size, double_window_size, counts)) != SVS_OK) return rc;
+  SVS_CK(h, feat_clear(h, W, w.f));
+  k_marg_count<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, I(w.o_old), I(w.s.o_wtype), I(w.o_mcnt), I(w.f.o_touch));
+  k_scan<<<1, 1024, 0, h->stream>>>(I(w.o_mcnt), V, I(w.o_mptr));
+  SVS_CK(h, feat_count(h, W, w.f));
+  SVS_CK(h, cudaGetLastError());
+  SVS_CK(h, cudaMemcpyAsync(counts + 3, I(w.o_mptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts + 4, I(w.f.o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  const int P = counts[0], L = counts[1], C = counts[2];
+  *P_out = P; *L_out = L;
+  if (C_out) *C_out = C;
+  *do_optimization = P >= 2;
+  if (P > cap_P || L > cap_L || (c_i && C > cap_C)) { h->err = "window, active points or constraints exceed the caller's capacity"; return SVS_ERR_INVALID; }
+  if ((rc = prepare_apply(h, w, root, loop, P, counts[3], counts[4], counts[5])) != SVS_OK) {
+    h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // a graph half marginalised must not stay behind
+    return rc;
+  }
+  return sel_emit(h, W, w.s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
+}
+
+extern "C" int svs_map_get_window_state(svs_map* h, int cap, int* nnzN, unsigned char* window_type, unsigned char* marginalized) {
+  if (!h || !h->d_map || !nnzN) return SVS_ERR_INVALID;
+  if (!h->g.nbr_ptr) { h->err = "the map has no pose graph"; return SVS_ERR_STATE; }
+  const int V = h->V, nn = h->nnzN;
+  *nnzN = nn;
+  if (marginalized && cap < nn) { h->err = "nnzN exceeds the caller's capacity"; return SVS_ERR_INVALID; }
+  cudaSetDevice(h->device);
+  std::vector<int> wt(h->wtV);
+  if (window_type && h->wtV)
+    SVS_CK(h, cudaMemcpyAsync(wt.data(), h->d_wt, sizeof(int) * (size_t)h->wtV, cudaMemcpyDeviceToHost, h->stream));
+  if (marginalized && nn) SVS_CK(h, cudaMemcpyAsync(marginalized, h->g.nbr_mrg, (size_t)nn, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaStreamSynchronize(h->stream));
+  if (window_type)
+    for (int v = 0; v < V; ++v) window_type[v] = (unsigned char)(v < h->wtV ? wt[v] : 0);
+  return SVS_OK;
 }
 
 extern "C" {
