@@ -98,9 +98,8 @@ struct svs_ba : svs::Handle {
   int cur_known = -1;   // host mirror of LmCtl::cur (index of the accepted state buffers), -1 = ask the device
   BaDev d{};
   // one device arena + one pinned staging arena, grown on demand and reused across set_problem calls
-  char* arena = nullptr; size_t arena_cap = 0, arena_off = 0;
+  char* arena = nullptr; size_t arena_cap = 0;
   char* stage = nullptr; size_t stage_cap = 0;
-  bool measuring = false;
   LmCtl* h_ctl = nullptr;  // pinned
   double* d_pose0 = nullptr;
   double* d_psi0 = nullptr;
@@ -163,42 +162,29 @@ struct CudaErr {
   const char* what;
 };
 
-constexpr size_t kAlign = 256;
-
 template <typename T>
-int dev_alloc(svs_ba* h, T** p, size_t n) {
-  const size_t bytes = ((std::max<size_t>(n, 1) * sizeof(T) + kAlign - 1) / kAlign) * kAlign;
-  if (!h->measuring) *p = reinterpret_cast<T*>(h->arena + h->arena_off);
-  h->arena_off += bytes;
-  return SVS_OK;
-}
+void dev_alloc(Bump& m, T** p, size_t n) { *p = m.take<T>(n); }
 
-// Uploads are laid out at the front of the arena, mirrored in the pinned staging buffer, and
-// shipped with a single H2D copy (finish_upload).
+// Uploads are laid out at the front of the arena, mirrored at the same offset in the pinned staging buffer, and
+// shipped with a single H2D copy (finish_problem).  src == nullptr: only the place is taken.
 template <typename T>
-int dev_upload(svs_ba* h, const T** p, const T* src, size_t n) {
-  const size_t off = h->arena_off;
-  T* q = nullptr;
-  dev_alloc(h, &q, n);
-  if (!h->measuring) {
-    if (n) {
-      const size_t bytes = n * sizeof(T);
-      if (bytes >= (1u << 20)) {   // multi-MB arrays (observations, weights): split the copy over a few threads
-        const int parts = 4;
-        h->pool.parallel_for(parts, [&](int q) {
-          const size_t b0 = bytes * q / parts, b1 = bytes * (q + 1) / parts;
-          memcpy(h->stage + off + b0, reinterpret_cast<const char*>(src) + b0, b1 - b0);
-        });
-      } else {
-        memcpy(h->stage + off, src, bytes);
-      }
-    }
-    *p = q;
+void dev_upload(svs_ba* h, Bump& m, const T** p, const T* src, size_t n) {
+  const size_t off = m.off;
+  *p = m.take<T>(n);
+  if (!m.base || !src || !n) return;
+  const size_t bytes = n * sizeof(T);
+  if (bytes >= (1u << 20)) {   // multi-MB arrays (observations, weights): split the copy over a few threads
+    const int parts = 4;
+    h->pool.parallel_for(parts, [&](int q) {
+      const size_t b0 = bytes * q / parts, b1 = bytes * (q + 1) / parts;
+      memcpy(h->stage + off + b0, reinterpret_cast<const char*>(src) + b0, b1 - b0);
+    });
+  } else {
+    memcpy(h->stage + off, src, bytes);
   }
-  return SVS_OK;
 }
 template <typename T>
-int dev_upload(svs_ba* h, const T** p, const std::vector<T>& v) { return dev_upload(h, p, v.data(), v.size()); }
+void dev_upload(svs_ba* h, Bump& m, const T** p, const std::vector<T>& v) { dev_upload(h, m, p, v.data(), v.size()); }
 
 // process-wide, so that no two set-ups on any two handles share a serial (a destroyed handle's address can come back)
 unsigned long long next_serial() {
@@ -549,47 +535,42 @@ struct LaySrc {
   const double* c_T = nullptr; const double* c_Lam = nullptr; const double* pose0 = nullptr; const double* psi0 = nullptr;
 };
 
-// Device image of the problem in h->d (sizes set by the caller): the constant arrays (the uploaded ones mirrored in the
-// staging buffer) followed by the work buffers.  With h->measuring only h->arena_off advances.
-static void lay(svs_ba* h, const Symbolic& sy, const LaySrc& s, const double** d_pose0, const double** d_psi0) {
+// Device image of the problem in h->d (sizes set by the caller), laid out on m: the constant arrays (the uploaded ones
+// mirrored in the staging buffer) followed by the work buffers.  Both passes set the marks off_* and upload_bytes.
+static void lay(svs_ba* h, Bump& m, const Symbolic& sy, const LaySrc& s, const double** d_pose0, const double** d_psi0) {
   BaDev& d = h->d;
   const int P = d.P, L = d.L, C = d.C, ne = d.E, ns = d.nslots;
-  h->arena_off = 0;
-  auto put = [&](auto& field, auto src, size_t n) {
-    if (src) dev_upload(h, &field, src, n);
-    else dev_alloc(h, &field, n);
-  };
+  auto put = [&](auto& field, auto src, size_t n) { dev_upload(h, m, &field, src, n); };
   put(d.fixed, s.fixed, P); put(d.lm_eptr, s.lm_eptr, (size_t)L + 1); put(d.lm_sptr, s.lm_sptr, (size_t)L + 1);
   put(d.lm_anchor, s.lm_anchor, L); put(d.lm_self, s.lm_self, L); put(d.lm_user, s.lm_user, L);
   put(d.e_pose, s.e_pose, ne); put(d.edge_src, s.edge_src, ne);
   put(d.task_lm, s.task_lm, d.ntasks); put(d.task_cnt, s.task_cnt, d.ntasks); put(d.gen_lm, s.gen_lm, d.ngen);
   put(d.long_lm, s.long_lm, d.nlong);
-  h->off_sym = h->arena_off;
-#define UP(field, vec) dev_upload(h, &d.field, vec)
+  h->off_sym = m.off;
+#define UP(field, vec) dev_upload(h, m, &d.field, vec)
   UP(tbl, sy.tbl); UP(perm, sy.perm); UP(pos, sy.pos); UP(col_ptr, sy.col_ptr); UP(row_idx, sy.row_idx);
   UP(upd_ptr, sy.upd_ptr); UP(upd_dst, sy.upd_dst); UP(upd_ab, sy.upd_ab); UP(urg_dst, sy.urg_dst);
   UP(branch_ptr, sy.branch_ptr); UP(rptr, sy.rptr); UP(rowpos, sy.rowpos); UP(rcol, sy.rcol);
 #undef UP
-  h->off_sym_end = h->arena_off;
+  h->off_sym_end = m.off;
   put(d.col_need, s.col_need, P);
   put(d.c_i, s.c_i, C); put(d.c_j, s.c_j, C);
-  h->off_num = h->off_cT = h->arena_off;   // the numbers (everything a same-structure call re-sends) lie last
+  h->off_num = h->off_cT = m.off;   // the numbers (everything a same-structure call re-sends) lie last
   put(d.c_T, s.c_T, 7 * (size_t)C);
-  h->off_cLam = h->arena_off;
+  h->off_cLam = m.off;
   put(d.c_Lam, s.c_Lam, 36 * (size_t)C);
-  h->off_pose0 = h->arena_off;
+  h->off_pose0 = m.off;
   put(*d_pose0, s.pose0, 7 * (size_t)P);
-  h->off_psi0 = h->arena_off;
+  h->off_psi0 = m.off;
   put(*d_psi0, s.psi0, 3 * (size_t)L);
-  h->upload_bytes = h->arena_off;
-#define AL(field, n) dev_alloc(h, &d.field, (size_t)(n))
+  h->upload_bytes = m.off;
+#define AL(field, n) dev_alloc(m, &d.field, (size_t)(n))
   for (int b = 0; b < 2; ++b) { AL(pose[b], 7 * (size_t)P); AL(Rt[b], 12 * (size_t)P); AL(psi[b], 3 * (size_t)L); }
   AL(e_obs_w, 3 * (size_t)ne); AL(e_w_w, 3 * (size_t)ne);
   AL(W, 18 * (size_t)ns); AL(Dbl, 12 * (size_t)L); AL(chi_l, L); AL(chi_new_l, L); AL(scale_l, L);
   {   // reduced system S | bp | bc | totals in ONE buffer: a sharded window sums it with a single all-reduce
-    double* sys = nullptr;
-    dev_alloc(h, &sys, 36 * (size_t)sy.nblk + 12 * (size_t)P + 4);
-    if (!h->measuring) { d.S = sys; d.bp = sys + 36 * (size_t)sy.nblk; d.bc = d.bp + 6 * (size_t)P; d.totals = d.bc + 6 * (size_t)P; }
+    double* sys = m.take<double>(36 * (size_t)sy.nblk + 12 * (size_t)P + 4);
+    if (sys) { d.S = sys; d.bp = sys + 36 * (size_t)sy.nblk; d.bc = d.bp + 6 * (size_t)P; d.totals = d.bc + 6 * (size_t)P; }
     h->sys_count = 36 * (size_t)sy.nblk + 12 * (size_t)P;
   }
   AL(x, 6 * (size_t)P); AL(Nrow, 36 * (size_t)std::max(sy.nblk - P, 1));
@@ -603,15 +584,24 @@ static void lay(svs_ba* h, const Symbolic& sy, const LaySrc& s, const double** d
 static int lay_arena(svs_ba* h, const Symbolic& sy, const LaySrc& s) {
   const double* d_pose0c = nullptr;
   const double* d_psi0c = nullptr;
-  h->measuring = true;
-  lay(h, sy, s, &d_pose0c, &d_psi0c);
-  h->measuring = false;
-  SVS_CK(h, grow(h->arena_off, &h->arena_cap, &h->arena));
+  Bump m{nullptr};
+  lay(h, m, sy, s, &d_pose0c, &d_psi0c);
+  SVS_CK(h, grow(m.off, &h->arena_cap, &h->arena));
   SVS_CK(h, grow<char>(h->upload_bytes, &h->stage_cap, nullptr, &h->stage));
-  lay(h, sy, s, &d_pose0c, &d_psi0c);
+  m = Bump{h->arena};
+  lay(h, m, sy, s, &d_pose0c, &d_psi0c);
   h->d_pose0 = const_cast<double*>(d_pose0c);
   h->d_psi0 = const_cast<double*>(d_psi0c);
   return SVS_OK;
+}
+
+// The index arrays of the last device set-up, which the next one compares with on the device (d_keep)
+struct Keep { int *e_point, *e_pose, *e_anchor, *c_i, *c_j; unsigned char* fixed; };
+static Keep keep_carve(Bump& m, int P, int E, int C) {
+  Keep k;
+  k.e_point = m.take<int>(E); k.e_pose = m.take<int>(E); k.e_anchor = m.take<int>(E);
+  k.c_i = m.take<int>(C); k.c_j = m.take<int>(C); k.fixed = m.take<unsigned char>(P);
+  return k;
 }
 
 // The rest of a new structure, shared by both set-ups: state pointers, solver widths, counts and the structure key.
@@ -1066,9 +1056,10 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   // the same structure as the problem on the device, if the index arrays say so (compared on the device)
   in.compare = h->has_problem && h->k_on_device && P == h->k_P && L == h->k_L && E == h->k_E && C == h->k_C &&
                h->flags == h->k_flags && h->extra_pairs == h->k_extra;
-  const int* keep = reinterpret_cast<const int*>(h->d_keep);
-  in.k_epoint = keep; in.k_epose = keep + E; in.k_eanchor = keep + 2 * (size_t)E; in.k_ci = keep + 3 * (size_t)E;
-  in.k_cj = keep + 3 * (size_t)E + C; in.k_fixed = reinterpret_cast<const unsigned char*>(keep + 3 * (size_t)E + 2 * (size_t)C);
+  Bump km{h->d_keep};
+  const Keep old = keep_carve(km, P, E, C);
+  in.k_epoint = old.e_point; in.k_epose = old.e_pose; in.k_eanchor = old.e_anchor; in.k_ci = old.c_i; in.k_cj = old.c_j;
+  in.k_fixed = old.fixed;
   StructOut so{};
   SVS_CK(h, grow(launch_structure(in, nullptr, &so, st), &h->scr_cap, &h->d_scr));
   launch_structure(in, h->d_scr, &so, st);
@@ -1119,9 +1110,11 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   if (int rc = lay_arena(h, sy, LaySrc{})) return rc;   // every array but the symbolic ones comes from the device
   SVS_CK(h, cudaMemcpyAsync(h->arena + h->off_sym, h->stage + h->off_sym, h->off_sym_end - h->off_sym, cudaMemcpyHostToDevice, st));
   // the device's results into the arena, and this structure's index arrays into the copy the next call compares with
-  const size_t keep_bytes = 4 * (3 * (size_t)E + 2 * (size_t)C) + P;
-  SVS_CK(h, grow(keep_bytes, &h->keep_cap, &h->d_keep));
-  int* kp = reinterpret_cast<int*>(h->d_keep);
+  km = Bump{nullptr};
+  keep_carve(km, P, E, C);
+  SVS_CK(h, grow(km.off, &h->keep_cap, &h->d_keep));
+  km = Bump{h->d_keep};
+  const Keep kp = keep_carve(km, P, E, C);
   CopyList cl;
   auto I = [](const int* p) { return const_cast<int*>(p); };
   cl.add(so.fixed, const_cast<unsigned char*>(d.fixed), P);
@@ -1134,9 +1127,8 @@ static int set_problem_dev(svs_ba* h, int P, const double* T_qt, const unsigned 
   cl.add(c_i, I(d.c_i), 4 * (size_t)C); cl.add(c_j, I(d.c_j), 4 * (size_t)C);
   cl.add(c_T, const_cast<double*>(d.c_T), 56 * (size_t)C); cl.add(c_Lambda, const_cast<double*>(d.c_Lam), 288 * (size_t)C);
   cl.add(T_qt, h->d_pose0, 56 * (size_t)P); cl.add(so.psi, h->d_psi0, 24 * (size_t)L);
-  cl.add(e_point, kp, 4 * (size_t)E); cl.add(e_pose, kp + E, 4 * (size_t)E); cl.add(e_anchor, kp + 2 * (size_t)E, 4 * (size_t)E);
-  cl.add(c_i, kp + 3 * (size_t)E, 4 * (size_t)C); cl.add(c_j, kp + 3 * (size_t)E + C, 4 * (size_t)C);
-  cl.add(so.fixed, kp + 3 * (size_t)E + 2 * (size_t)C, P);
+  cl.add(e_point, kp.e_point, 4 * (size_t)E); cl.add(e_pose, kp.e_pose, 4 * (size_t)E); cl.add(e_anchor, kp.e_anchor, 4 * (size_t)E);
+  cl.add(c_i, kp.c_i, 4 * (size_t)C); cl.add(c_j, kp.c_j, 4 * (size_t)C); cl.add(so.fixed, kp.fixed, P);
   if (!d_obs_info) { cl.add(e_obs, h->d_raw, 24 * (size_t)E); cl.add(e_info, h->d_raw + 3 * (size_t)E, 24 * (size_t)E); }
   launch_copies(cl, st);
   SVS_CK(h, cudaMemsetAsync(I(d.col_need), 0, sizeof(int) * (size_t)std::max(P, 1), st));

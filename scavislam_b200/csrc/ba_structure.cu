@@ -18,6 +18,7 @@
 #include "ba_rules.cuh"
 #include "ba_structure.cuh"
 #include "ba_types.cuh"
+#include "handle.cuh"
 
 namespace svs {
 namespace {
@@ -271,16 +272,6 @@ __global__ void k_copies(CopyList c) {
   for (size_t i = done + tid; i < j.bytes; i += stride) d[i] = s[i];
 }
 
-// bump allocation in the scratch (256-byte aligned); measuring when base == nullptr
-struct Bump {
-  char* base; size_t off = 0;
-  template <typename T> T* take(size_t n) {
-    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
-    off += ((std::max<size_t>(n, 1) * sizeof(T) + 255) / 256) * 256;
-    return p;
-  }
-};
-
 }  // namespace
 
 size_t launch_structure(const StructIn& in, void* scratch, StructOut* out, cudaStream_t st) {
@@ -331,7 +322,7 @@ size_t launch_structure(const StructIn& in, void* scratch, StructOut* out, cudaS
   const int pbits = bits_for(std::max(P - 1, 0)), lbits = bits_for(std::max(L - 1, 0)), bbits = bits_for(P);
   const int ebits = std::min(64, lbits + 1 + pbits);
   thrust::counting_iterator<int> count0(0);
-  // CUB's temporary storage: the largest of the calls below (sized in the measuring pass)
+  // CUB's temporary storage: the largest of the calls below (sized in the sizing pass)
   size_t tmp = 0;
   auto need = [&](size_t b) { tmp = std::max(tmp, b); };
   {

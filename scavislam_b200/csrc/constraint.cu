@@ -173,46 +173,40 @@ int svs_computeConstraint_batch(svs_constraints* h, int P, const double* T_me_fr
   cudaSetDevice(h->device);
   const int scratch_stride = svs::constraint_scratch_stride(max_feat);
   // one arena: inputs, outputs, scratch
-  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
-  size_t off = 0;
-  const size_t o_pose = off; off += al(sizeof(double) * 7 * (size_t)P);
-  const size_t o_fptr = off; off += al(sizeof(int) * ((size_t)P + 1));
-  const size_t o_fpt = off; off += al(sizeof(int) * (size_t)std::max(nfeat, 1));
-  const size_t o_anch = off; off += al(sizeof(int) * (size_t)std::max(L, 1));
-  const size_t o_xyz = off; off += al(sizeof(double) * 3 * (size_t)std::max(L, 1));
-  const size_t o_v1 = off; off += al(sizeof(int) * (size_t)npairs);
-  const size_t o_v2 = off; off += al(sizeof(int) * (size_t)npairs);
-  const size_t o_T = off; off += al(sizeof(double) * 7 * (size_t)npairs);
-  const size_t o_L = off; off += al(sizeof(double) * 36 * (size_t)npairs);
-  const size_t o_n = off; off += al(sizeof(int) * (size_t)npairs);
-  const size_t o_s = off; off += al(sizeof(double) * (size_t)scratch_stride * (size_t)npairs);
-  if (off > h->cap_bytes) {
+  struct {
+    double *pose, *xyz, *T12, *Lam, *scr;
+    int *fptr, *fpt, *anch, *v1, *v2, *n;
+  } b;
+  auto carve = [&](svs::Bump m) {
+    b.pose = m.take<double>(7 * (size_t)P); b.fptr = m.take<int>((size_t)P + 1); b.fpt = m.take<int>(nfeat);
+    b.anch = m.take<int>(L); b.xyz = m.take<double>(3 * (size_t)L);
+    b.v1 = m.take<int>(npairs); b.v2 = m.take<int>(npairs); b.T12 = m.take<double>(7 * (size_t)npairs);
+    b.Lam = m.take<double>(36 * (size_t)npairs); b.n = m.take<int>(npairs);
+    b.scr = m.take<double>((size_t)scratch_stride * npairs);
+    return m.off;
+  };
+  const size_t bytes = carve(svs::Bump{nullptr});
+  if (bytes > h->cap_bytes) {
     SVS_CK(h, cudaStreamSynchronize(h->stream));
-    SVS_CK(h, svs::grow(off, &h->cap_bytes, &h->d_buf));
+    SVS_CK(h, svs::grow(bytes, &h->cap_bytes, &h->d_buf));
   }
-  char* B = h->d_buf;
-  SVS_CK(h, cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)P, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(B + o_fptr, feat_ptr, sizeof(int) * ((size_t)P + 1), cudaMemcpyHostToDevice, h->stream));
-  if (nfeat) SVS_CK(h, cudaMemcpyAsync(B + o_fpt, feat_point, sizeof(int) * (size_t)nfeat, cudaMemcpyHostToDevice, h->stream));
+  carve(svs::Bump{h->d_buf});
+  SVS_CK(h, cudaMemcpyAsync(b.pose, T_me_from_world, sizeof(double) * 7 * (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(b.fptr, feat_ptr, sizeof(int) * ((size_t)P + 1), cudaMemcpyHostToDevice, h->stream));
+  if (nfeat) SVS_CK(h, cudaMemcpyAsync(b.fpt, feat_point, sizeof(int) * (size_t)nfeat, cudaMemcpyHostToDevice, h->stream));
   if (L) {
-    SVS_CK(h, cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(b.anch, point_anchor, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(b.xyz, xyz_anchor, sizeof(double) * 3 * (size_t)L, cudaMemcpyHostToDevice, h->stream));
   }
-  SVS_CK(h, cudaMemcpyAsync(B + o_v1, v1, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(B + o_v2, v2, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
-  double* T12 = reinterpret_cast<double*>(B + o_T);
-  double* Lm = reinterpret_cast<double*>(B + o_L);
-  int* n = reinterpret_cast<int*>(B + o_n);
-  svs::launch_compute_constraint(reinterpret_cast<const double*>(B + o_pose), reinterpret_cast<const int*>(B + o_fptr),
-                                 reinterpret_cast<const int*>(B + o_fpt), reinterpret_cast<const int*>(B + o_anch),
-                                 reinterpret_cast<const double*>(B + o_xyz), npairs, reinterpret_cast<const int*>(B + o_v1),
-                                 reinterpret_cast<const int*>(B + o_v2), T12, Lm, n, reinterpret_cast<double*>(B + o_s),
+  SVS_CK(h, cudaMemcpyAsync(b.v1, v1, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(b.v2, v2, sizeof(int) * (size_t)npairs, cudaMemcpyHostToDevice, h->stream));
+  svs::launch_compute_constraint(b.pose, b.fptr, b.fpt, b.anch, b.xyz, npairs, b.v1, b.v2, b.T12, b.Lam, b.n, b.scr,
                                  scratch_stride, h->stream);
   SVS_CK(h, cudaGetLastError());
-  SVS_CK(h, cudaMemcpyAsync(T_1_from_2, T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(Lambda, Lm, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(T_1_from_2, b.T12, sizeof(double) * 7 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(Lambda, b.Lam, sizeof(double) * 36 * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
   if (visibility_strength)
-    SVS_CK(h, cudaMemcpyAsync(visibility_strength, n, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(visibility_strength, b.n, sizeof(int) * (size_t)npairs, cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   return SVS_OK;
 }

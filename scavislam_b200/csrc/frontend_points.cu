@@ -590,22 +590,17 @@ int svs_addMorePoints(svs_matcher* m, int fresh, const double T_newkey_from_cur[
     q.stride_cell = (size_t)ncell + 1;
     q.stride_item = (size_t)c.max_kp + c.max_pts;
     const size_t L = (size_t)c.nlevels;
-    const size_t bytes = L * (2 * q.stride_kp * 8 + 8 * q.stride_kp * 4 + 2 * q.stride_cell * 4 + q.stride_item * 4) + 14 * 256;
-    SVS_CK(c.base, cudaMalloc(&s->d_scratch, bytes));
-    char* p = static_cast<char*>(s->d_scratch);
-    auto take = [&](size_t b) { char* r = p; p += (b + 255) / 256 * 256; return r; };
-    q.key = reinterpret_cast<unsigned long long*>(take(L * q.stride_kp * 8));
-    q.nh = reinterpret_cast<unsigned long long*>(take(L * q.stride_kp * 8));
-    q.path = reinterpret_cast<unsigned*>(take(L * q.stride_kp * 4));
-    q.spos = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.edepth = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.order = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.rank = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.status = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.outk = reinterpret_cast<int*>(take(L * q.stride_kp * 4));
-    q.cell_ptr = reinterpret_cast<int*>(take(L * q.stride_cell * 4));
-    q.cell_cur = reinterpret_cast<int*>(take(L * q.stride_cell * 4));
-    q.cell_item = reinterpret_cast<int*>(take(L * q.stride_item * 4));
+    auto carve = [&](svs::Bump m) {
+      q.key = m.take<unsigned long long>(L * q.stride_kp); q.nh = m.take<unsigned long long>(L * q.stride_kp);
+      q.path = m.take<unsigned>(L * q.stride_kp);
+      q.spos = m.take<int>(L * q.stride_kp); q.edepth = m.take<int>(L * q.stride_kp); q.order = m.take<int>(L * q.stride_kp);
+      q.rank = m.take<int>(L * q.stride_kp); q.status = m.take<int>(L * q.stride_kp); q.outk = m.take<int>(L * q.stride_kp);
+      q.cell_ptr = m.take<int>(L * q.stride_cell); q.cell_cur = m.take<int>(L * q.stride_cell);
+      q.cell_item = m.take<int>(L * q.stride_item);
+      return m.off;
+    };
+    SVS_CK(c.base, cudaMalloc(&s->d_scratch, carve(svs::Bump{nullptr})));
+    carve(svs::Bump{static_cast<char*>(s->d_scratch)});
   }
   SVS_CK(c.base, svs::grow((size_t)bound, &s->pts_cap, &s->d_out_pts));
   SVS_CK(c.base, svs::grow((size_t)bound, &s->rows_cap, &s->d_out_rows));

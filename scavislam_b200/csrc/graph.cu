@@ -543,12 +543,29 @@ __global__ void k_marg_store(int n, GraphDev g, const int* __restrict__ v1, cons
   }
 }
 
+// the map's tables and the pose graph's lists, each carved from one device buffer; the handle keeps them writable
+struct MapTables { double* pose; int* anchor; double* xyz; int* vis_ptr; int* vis_pose; double* center; int* level; };
+MapTables map_carve(svs::Bump& m, int V, int Np, int nnz) {
+  MapTables t;
+  t.pose = m.take<double>(7 * (size_t)V); t.anchor = m.take<int>(Np); t.xyz = m.take<double>(3 * (size_t)Np);
+  t.vis_ptr = m.take<int>((size_t)Np + 1); t.vis_pose = m.take<int>(nnz); t.center = m.take<double>(3 * (size_t)nnz);
+  t.level = m.take<int>(nnz);
+  return t;
+}
+struct GraphTables { int *ptr, *id, *str; double *T, *Lam; unsigned char* mrg; };
+GraphTables graph_carve(svs::Bump& m, int V, int nn) {
+  GraphTables t;
+  t.ptr = m.take<int>((size_t)V + 1); t.id = m.take<int>(nn); t.str = m.take<int>(nn); t.T = m.take<double>(7 * (size_t)nn);
+  t.Lam = m.take<double>(36 * (size_t)nn); t.mrg = m.take<unsigned char>(nn);
+  return t;
+}
+
 }  // namespace
 
 struct svs_map : svs::Handle {
   int V = 0, Np = 0, nnz = 0;
   char* d_map = nullptr; size_t map_cap = 0;
-  MapDev m{};
+  MapTables t{}; MapDev m{};   // m: t as the kernels read it
   char* d_work = nullptr; size_t work_cap = 0;
   std::vector<int> h_winpos;
   const double* d_oi_last = nullptr;   // [E][3] observations, [E][3] weights of the last assembly
@@ -559,7 +576,7 @@ struct svs_map : svs::Handle {
   const int* d_win_last = nullptr; const int* d_act_last = nullptr; int last_P = 0, last_L = 0;
   unsigned long long last_serial = 0;
   char* d_upd = nullptr; size_t upd_cap = 0;   // staging of svs_map_update_*
-  char* d_graph = nullptr; size_t graph_cap = 0; GraphDev g{}; int nnzN = 0;   // svs_map_set_graph
+  char* d_graph = nullptr; size_t graph_cap = 0; GraphTables gt{}; GraphDev g{}; int nnzN = 0;   // svs_map_set_graph
   char* d_graph2 = nullptr; size_t graph2_cap = 0;   // the next graph while the growth calls build it (then swapped)
   char* d_gw = nullptr; size_t gw_cap = 0;           // work of the growth calls: strengths and staged edge lists
   char* d_ge = nullptr; size_t ge_cap = 0;           // ... feature tables, constraints and list insertion
@@ -570,29 +587,10 @@ struct svs_map : svs::Handle {
   int* d_wt = nullptr; size_t wt_cap = 0; int wtV = 0;
 };
 
-static size_t al256(size_t x) { return (x + 255) / 256 * 256; }
-
-struct MapLayout { size_t o_pose, o_anch, o_xyz, o_vptr, o_vpose, o_cen, o_lvl, total; };
-static MapLayout map_layout(int V, int Np, int nnz) {
-  MapLayout lo{};
-  size_t off = 0;
-  lo.o_pose = off; off += al256(sizeof(double) * 7 * (size_t)V);
-  lo.o_anch = off; off += al256(sizeof(int) * (size_t)std::max(Np, 1));
-  lo.o_xyz = off; off += al256(sizeof(double) * 3 * (size_t)std::max(Np, 1));
-  lo.o_vptr = off; off += al256(sizeof(int) * ((size_t)Np + 1));
-  lo.o_vpose = off; off += al256(sizeof(int) * (size_t)std::max(nnz, 1));
-  lo.o_cen = off; off += al256(sizeof(double) * 3 * (size_t)std::max(nnz, 1));
-  lo.o_lvl = off; off += al256(sizeof(int) * (size_t)std::max(nnz, 1));
-  lo.total = off;
-  return lo;
-}
-static void map_bind(svs_map* h, char* B, const MapLayout& lo, int V, int Np, int nnz) {
+static void map_bind(svs_map* h, const MapTables& t, int V, int Np, int nnz) {
   h->V = V; h->Np = Np; h->nnz = nnz;
-  h->m.V = V; h->m.Np = Np;
-  h->m.pose = reinterpret_cast<const double*>(B + lo.o_pose); h->m.anchor = reinterpret_cast<const int*>(B + lo.o_anch);
-  h->m.xyz = reinterpret_cast<const double*>(B + lo.o_xyz); h->m.vis_ptr = reinterpret_cast<const int*>(B + lo.o_vptr);
-  h->m.vis_pose = reinterpret_cast<const int*>(B + lo.o_vpose); h->m.center = reinterpret_cast<const double*>(B + lo.o_cen);
-  h->m.level = reinterpret_cast<const int*>(B + lo.o_lvl);
+  h->t = t;
+  h->m = MapDev{V, Np, t.pose, t.anchor, t.xyz, t.vis_ptr, t.vis_pose, t.center, t.level};
 }
 
 extern "C" {
@@ -634,27 +632,26 @@ int svs_map_set(svs_map* h, int V, const double* T_me_from_world, int Np, const 
       return SVS_ERR_INVALID;
     }
   cudaSetDevice(h->device);
-  const MapLayout lo = map_layout(V, Np, nnz);
-  const size_t off = lo.total;
-  const size_t o_pose = lo.o_pose, o_anch = lo.o_anch, o_xyz = lo.o_xyz, o_vptr = lo.o_vptr, o_vpose = lo.o_vpose, o_cen = lo.o_cen,
-               o_lvl = lo.o_lvl;
+  svs::Bump m{nullptr};
+  map_carve(m, V, Np, nnz);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   h->d_win_last = nullptr;   // a window assembled from the previous map names its rows, not this map's
-  SVS_CK(h, svs::grow(off, &h->map_cap, &h->d_map));
-  char* B = h->d_map;
-  SVS_CK(h, cudaMemcpyAsync(B + o_pose, T_me_from_world, sizeof(double) * 7 * (size_t)V, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, svs::grow(m.off, &h->map_cap, &h->d_map));
+  m = svs::Bump{h->d_map};
+  const MapTables t = map_carve(m, V, Np, nnz);
+  SVS_CK(h, cudaMemcpyAsync(t.pose, T_me_from_world, sizeof(double) * 7 * (size_t)V, cudaMemcpyHostToDevice, h->stream));
   if (Np) {
-    SVS_CK(h, cudaMemcpyAsync(B + o_anch, point_anchor, sizeof(int) * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(B + o_xyz, xyz_anchor, sizeof(double) * 3 * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(B + o_vptr, vis_ptr, sizeof(int) * ((size_t)Np + 1), cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.anchor, point_anchor, sizeof(int) * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.xyz, xyz_anchor, sizeof(double) * 3 * (size_t)Np, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.vis_ptr, vis_ptr, sizeof(int) * ((size_t)Np + 1), cudaMemcpyHostToDevice, h->stream));
   }
   if (nnz) {
-    SVS_CK(h, cudaMemcpyAsync(B + o_vpose, vis_pose, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(B + o_cen, feat_center, sizeof(double) * 3 * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(B + o_lvl, feat_level, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.vis_pose, vis_pose, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.center, feat_center, sizeof(double) * 3 * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.level, feat_level, sizeof(int) * (size_t)nnz, cudaMemcpyHostToDevice, h->stream));
   }
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  map_bind(h, B, lo, V, Np, nnz);
+  map_bind(h, t, V, Np, nnz);
   h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // a new map: its pose graph comes with svs_map_set_graph
   return SVS_OK;
 }
@@ -666,15 +663,17 @@ static int map_scatter(svs_map* h, double* table, int rows_in_table, int n, cons
     if (index[i] < 0 || index[i] >= rows_in_table) { h->err = std::string(what) + " index out of range"; return SVS_ERR_INVALID; }
   if (n == 0) return SVS_OK;
   cudaSetDevice(h->device);
-  const size_t ib = al256(sizeof(int) * (size_t)n), rb = sizeof(double) * (size_t)n * width;
-  if (ib + rb > h->upd_cap) {
+  int* d_index = nullptr; double* d_rows = nullptr;
+  auto carve = [&](svs::Bump m) { d_index = m.take<int>(n); d_rows = m.take<double>((size_t)n * width); return m.off; };
+  const size_t bytes = carve(svs::Bump{nullptr});
+  if (bytes > h->upd_cap) {
     SVS_CK(h, cudaStreamSynchronize(h->stream));
-    SVS_CK(h, svs::grow(ib + rb, &h->upd_cap, &h->d_upd));
+    SVS_CK(h, svs::grow(bytes, &h->upd_cap, &h->d_upd));
   }
-  SVS_CK(h, cudaMemcpyAsync(h->d_upd, index, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(h->d_upd + ib, rows, rb, cudaMemcpyHostToDevice, h->stream));
-  k_scatter_rows<<<(n * width + 255) / 256, 256, 0, h->stream>>>(table, reinterpret_cast<const int*>(h->d_upd),
-                                                                 reinterpret_cast<const double*>(h->d_upd + ib), n, width);
+  carve(svs::Bump{h->d_upd});
+  SVS_CK(h, cudaMemcpyAsync(d_index, index, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d_rows, rows, sizeof(double) * (size_t)n * width, cudaMemcpyHostToDevice, h->stream));
+  k_scatter_rows<<<(n * width + 255) / 256, 256, 0, h->stream>>>(table, d_index, d_rows, n, width);
   SVS_CK(h, cudaGetLastError());
   SVS_CK(h, cudaStreamSynchronize(h->stream));   // the caller's arrays may go away
   return SVS_OK;
@@ -682,12 +681,12 @@ static int map_scatter(svs_map* h, double* table, int rows_in_table, int n, cons
 
 int svs_map_update_poses(svs_map* h, int n, const int* vertex, const double* T_me_from_world) {
   if (!h || n < 0 || (n && (!vertex || !T_me_from_world)) || !h->d_map) return SVS_ERR_INVALID;
-  return map_scatter(h, const_cast<double*>(h->m.pose), h->V, n, vertex, T_me_from_world, 7, "vertex");
+  return map_scatter(h, h->t.pose, h->V, n, vertex, T_me_from_world, 7, "vertex");
 }
 
 int svs_map_update_points(svs_map* h, int n, const int* point, const double* xyz_anchor) {
   if (!h || n < 0 || (n && (!point || !xyz_anchor)) || !h->d_map) return SVS_ERR_INVALID;
-  return map_scatter(h, const_cast<double*>(h->m.xyz), h->Np, n, point, xyz_anchor, 3, "point");
+  return map_scatter(h, h->t.xyz, h->Np, n, point, xyz_anchor, 3, "point");
 }
 
 int svs_map_get(svs_map* h, double* T_me_from_world, double* xyz_anchor) {
@@ -715,7 +714,7 @@ int svs_map_absorb(svs_map* h, svs_ba* ba) {
   cudaSetDevice(h->device);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int n = std::max(7 * P, L);
-  k_absorb<<<(n + 255) / 256, 256, 0, st>>>(const_cast<double*>(h->m.pose), const_cast<double*>(h->m.xyz), pose[0], pose[1], psi[0], psi[1],
+  k_absorb<<<(n + 255) / 256, 256, 0, st>>>(h->t.pose, h->t.xyz, pose[0], pose[1], psi[0], psi[1],
                                             lm_user, cur, h->d_win_last, h->d_act_last, P, L);
   SVS_CK(h, cudaGetLastError());
   SVS_CK(h, cudaStreamSynchronize(st));
@@ -740,74 +739,60 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
   for (int l = 0; l < L; ++l)
     if (active_point[l] < 0 || active_point[l] >= h->Np) { h->err = "active point outside [0, Np)"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  // work arena: win_pos, window, active, cnt, ptr, bad | poses, psi | edges (sized for every observation of the map)
-  size_t off = 0;
-  const size_t o_wp = off; off += al256(sizeof(int) * (size_t)h->V);
-  const size_t o_win = off; off += al256(sizeof(int) * (size_t)P);
-  const size_t o_act = off; off += al256(sizeof(int) * (size_t)std::max(L, 1));
-  const size_t o_cnt = off; off += al256(sizeof(int) * (size_t)std::max(L, 1));
-  const size_t o_ptr = off; off += al256(sizeof(int) * ((size_t)L + 1));
-  const size_t o_bad = off; off += 256;
-  const size_t o_pose = off; off += al256(sizeof(double) * 7 * (size_t)P);
-  const size_t o_psi = off; off += al256(sizeof(double) * 3 * (size_t)std::max(L, 1));
-  const size_t emax = (size_t)std::max(h->nnz, 1);
-  const size_t o_ep = off; off += al256(sizeof(int) * emax);
-  const size_t o_es = off; off += al256(sizeof(int) * emax);
-  const size_t o_ea = off; off += al256(sizeof(int) * emax);
-  const size_t o_oi = off; off += al256(sizeof(double) * 6 * emax);
-  // the caller's fixed flags and pose-pose constraints (host arrays) go up next to the window
-  const size_t o_fx = off; off += al256((size_t)P);
-  const size_t o_ci = off; off += al256(sizeof(int) * (size_t)C);
-  const size_t o_cj = off; off += al256(sizeof(int) * (size_t)C);
-  const size_t o_cT = off; off += al256(sizeof(double) * 7 * (size_t)C);
-  const size_t o_cL = off; off += al256(sizeof(double) * 36 * (size_t)C);
+  // work arena: win_pos, window, active, cnt, ptr, bad | poses, psi | edges (sized for every observation of the map) |
+  // the caller's fixed flags and pose-pose constraints (host arrays), next to the window
+  struct {
+    int *wp, *win, *act, *cnt, *ptr, *bad, *ep, *es, *ea, *ci, *cj; double *pose, *psi, *oi, *cT, *cL; unsigned char* fx;
+  } w;
+  auto carve = [&](svs::Bump m) {
+    w.wp = m.take<int>(h->V); w.win = m.take<int>(P); w.act = m.take<int>(L); w.cnt = m.take<int>(L);
+    w.ptr = m.take<int>((size_t)L + 1); w.bad = m.take<int>(1);
+    w.pose = m.take<double>(7 * (size_t)P); w.psi = m.take<double>(3 * (size_t)L);
+    w.ep = m.take<int>(h->nnz); w.es = m.take<int>(h->nnz); w.ea = m.take<int>(h->nnz); w.oi = m.take<double>(6 * (size_t)h->nnz);
+    w.fx = m.take<unsigned char>(P); w.ci = m.take<int>(C); w.cj = m.take<int>(C);
+    w.cT = m.take<double>(7 * (size_t)C); w.cL = m.take<double>(36 * (size_t)C);
+    return m.off;
+  };
+  const size_t bytes = carve(svs::Bump{nullptr});
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  if (off > h->work_cap) {
+  if (bytes > h->work_cap) {
     h->last_E = 0; h->d_oi_last = nullptr; h->d_ep_last = h->d_es_last = h->d_ea_last = nullptr;   // they lay in the old arena
-    SVS_CK(h, svs::grow(off, &h->work_cap, &h->d_work));
+    SVS_CK(h, svs::grow(bytes, &h->work_cap, &h->d_work));
   }
-  char* W = h->d_work;
-  int* d_wp = reinterpret_cast<int*>(W + o_wp); int* d_win = reinterpret_cast<int*>(W + o_win);
-  int* d_act = reinterpret_cast<int*>(W + o_act); int* d_cnt = reinterpret_cast<int*>(W + o_cnt);
-  int* d_ptr = reinterpret_cast<int*>(W + o_ptr); int* d_bad = reinterpret_cast<int*>(W + o_bad);
-  double* d_pose = reinterpret_cast<double*>(W + o_pose); double* d_psi = reinterpret_cast<double*>(W + o_psi);
-  int* d_ep = reinterpret_cast<int*>(W + o_ep); int* d_es = reinterpret_cast<int*>(W + o_es); int* d_ea = reinterpret_cast<int*>(W + o_ea);
-  double* d_oi = reinterpret_cast<double*>(W + o_oi);
-  SVS_CK(h, cudaMemcpyAsync(d_wp, h->h_winpos.data(), sizeof(int) * (size_t)h->V, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(d_win, window_vertex, sizeof(int) * (size_t)P, cudaMemcpyHostToDevice, h->stream));
-  if (L) SVS_CK(h, cudaMemcpyAsync(d_act, active_point, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream));
-  if (fixed) SVS_CK(h, cudaMemcpyAsync(W + o_fx, fixed, (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  carve(svs::Bump{h->d_work});
+  SVS_CK(h, cudaMemcpyAsync(w.wp, h->h_winpos.data(), sizeof(int) * (size_t)h->V, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(w.win, window_vertex, sizeof(int) * (size_t)P, cudaMemcpyHostToDevice, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(w.act, active_point, sizeof(int) * (size_t)L, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(w.bad, 0, sizeof(int), h->stream));
+  if (fixed) SVS_CK(h, cudaMemcpyAsync(w.fx, fixed, (size_t)P, cudaMemcpyHostToDevice, h->stream));
   if (C) {
-    SVS_CK(h, cudaMemcpyAsync(W + o_ci, c_i, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(W + o_cj, c_j, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(W + o_cT, c_T, sizeof(double) * 7 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(W + o_cL, c_Lambda, sizeof(double) * 36 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.ci, c_i, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.cj, c_j, sizeof(int) * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.cT, c_T, sizeof(double) * 7 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.cL, c_Lambda, sizeof(double) * 36 * (size_t)C, cudaMemcpyHostToDevice, h->stream));
   }
   int E = 0, bad = 0;
   if (L) {
-    k_count<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, d_wp, d_act, L, d_cnt, d_bad);
-    k_scan<<<1, 1024, 0, h->stream>>>(d_cnt, L, d_ptr);
-    SVS_CK(h, cudaMemcpyAsync(&E, d_ptr + L, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    k_count<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, w.wp, w.act, L, w.cnt, w.bad);
+    k_scan<<<1, 1024, 0, h->stream>>>(w.cnt, L, w.ptr);
+    SVS_CK(h, cudaMemcpyAsync(&E, w.ptr + L, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(&bad, w.bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     SVS_CK(h, cudaStreamSynchronize(h->stream));
     if (bad) { h->err = "an active point is anchored in a frame outside the window"; return SVS_ERR_INVALID; }
     // obs_info = [E][3] observations followed by [E][3] weights: the emit kernel needs E for the second half
-    k_emit<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, d_wp, d_act, L, d_ptr, E, d_ep, d_es, d_ea, d_oi, d_psi);
+    k_emit<<<(L + 255) / 256, 256, 0, h->stream>>>(h->m, w.wp, w.act, L, w.ptr, E, w.ep, w.es, w.ea, w.oi, w.psi);
   }
-  k_gather_poses<<<(7 * P + 255) / 256, 256, 0, h->stream>>>(h->m, d_win, P, d_pose);
+  k_gather_poses<<<(7 * P + 255) / 256, 256, 0, h->stream>>>(h->m, w.win, P, w.pose);
   SVS_CK(h, cudaGetLastError());
   SVS_CK(h, cudaStreamSynchronize(h->stream));   // the BA handle reads the window on its own stream
   if (num_edges) *num_edges = E;
-  h->d_oi_last = d_oi; h->last_E = E;
-  h->d_ep_last = d_ep; h->d_es_last = d_es; h->d_ea_last = d_ea;
+  h->d_oi_last = w.oi; h->last_E = E;
+  h->d_ep_last = w.ep; h->d_es_last = w.es; h->d_ea_last = w.ea;
   // the window goes to the BA handle device to device: its structure is analysed there (svs_ba_set_problem_device)
-  const int rc = svs::ba_set_problem_device_obs(ba, P, d_pose, fixed ? reinterpret_cast<const unsigned char*>(W + o_fx) : nullptr, L,
-                                                 d_psi, E, d_ep, d_es, d_ea, d_oi, C, reinterpret_cast<const int*>(W + o_ci),
-                                                 reinterpret_cast<const int*>(W + o_cj), reinterpret_cast<const double*>(W + o_cT),
-                                                 reinterpret_cast<const double*>(W + o_cL), cam);
+  const int rc = svs::ba_set_problem_device_obs(ba, P, w.pose, fixed ? w.fx : nullptr, L, w.psi, E, w.ep, w.es,
+                                                 w.ea, w.oi, C, w.ci, w.cj, w.cT, w.cL, cam);
   if (rc != SVS_OK) { h->err = std::string("svs_ba_set_problem: ") + svs_last_error(ba); return rc; }
-  h->d_win_last = d_win; h->d_act_last = d_act; h->last_P = P; h->last_L = L;
+  h->d_win_last = w.win; h->d_act_last = w.act; h->last_P = P; h->last_L = L;
   h->last_serial = svs::ba_problem_serial(ba);
   return SVS_OK;
 }
@@ -815,25 +800,9 @@ int svs_ba_set_problem_from_map(svs_ba* ba, svs_map* h, int P, const int* window
 
 // ------------------------------------------------------------------ pose graph, window selection, growth
 
-struct GraphLayout { size_t o_ptr, o_id, o_str, o_T, o_L, o_M, total; };
-static GraphLayout graph_layout(int V, int nn) {
-  GraphLayout lo{};
-  size_t off = 0;
-  lo.o_ptr = off; off += al256(sizeof(int) * ((size_t)V + 1));
-  lo.o_id = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
-  lo.o_str = off; off += al256(sizeof(int) * (size_t)std::max(nn, 1));
-  lo.o_T = off; off += al256(sizeof(double) * 7 * (size_t)std::max(nn, 1));
-  lo.o_L = off; off += al256(sizeof(double) * 36 * (size_t)std::max(nn, 1));
-  lo.o_M = off; off += al256((size_t)std::max(nn, 1));
-  lo.total = off;
-  return lo;
-}
-static void graph_bind(svs_map* h, char* B, const GraphLayout& lo, int nn, bool strength, bool constraints) {
-  h->g.nbr_ptr = reinterpret_cast<const int*>(B + lo.o_ptr); h->g.nbr_id = reinterpret_cast<const int*>(B + lo.o_id);
-  h->g.nbr_str = strength ? reinterpret_cast<const int*>(B + lo.o_str) : nullptr;
-  h->g.nbr_T = constraints ? reinterpret_cast<const double*>(B + lo.o_T) : nullptr;
-  h->g.nbr_Lam = constraints ? reinterpret_cast<const double*>(B + lo.o_L) : nullptr;
-  h->g.nbr_mrg = reinterpret_cast<const unsigned char*>(B + lo.o_M);
+static void graph_bind(svs_map* h, const GraphTables& t, int nn, bool strength, bool constraints) {
+  h->gt = t;
+  h->g = GraphDev{t.ptr, t.id, strength ? t.str : nullptr, constraints ? t.T : nullptr, constraints ? t.Lam : nullptr, t.mrg};
   h->nnzN = nn;
 }
 
@@ -853,23 +822,25 @@ static int upload_graph(svs_map* h, const int* nbr_ptr, const int* nbr_id, const
       for (int i = nbr_ptr[v] + 1; i < nbr_ptr[v + 1]; ++i)
         if (nbr_strength[i] > nbr_strength[i - 1]) { h->err = "a neighbour list is not ordered strongest first"; return SVS_ERR_INVALID; }
   cudaSetDevice(h->device);
-  const GraphLayout lo = graph_layout(V, nn);
+  svs::Bump m{nullptr};
+  graph_carve(m, V, nn);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(lo.total, &h->graph_cap, &h->d_graph));
-  char* B = h->d_graph;
-  SVS_CK(h, cudaMemcpyAsync(B + lo.o_ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, svs::grow(m.off, &h->graph_cap, &h->d_graph));
+  m = svs::Bump{h->d_graph};
+  const GraphTables t = graph_carve(m, V, nn);
+  SVS_CK(h, cudaMemcpyAsync(t.ptr, nbr_ptr, sizeof(int) * ((size_t)V + 1), cudaMemcpyHostToDevice, h->stream));
   if (nn) {
-    SVS_CK(h, cudaMemcpyAsync(B + lo.o_id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
-    if (pose_graph) SVS_CK(h, cudaMemcpyAsync(B + lo.o_str, nbr_strength, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(t.id, nbr_id, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+    if (pose_graph) SVS_CK(h, cudaMemcpyAsync(t.str, nbr_strength, sizeof(int) * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     if (nbr_T) {
-      SVS_CK(h, cudaMemcpyAsync(B + lo.o_T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
-      SVS_CK(h, cudaMemcpyAsync(B + lo.o_L, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(t.T, nbr_T, sizeof(double) * 7 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
+      SVS_CK(h, cudaMemcpyAsync(t.Lam, nbr_Lambda, sizeof(double) * 36 * (size_t)nn, cudaMemcpyHostToDevice, h->stream));
     }
   }
   // the reference's state at its first prepareForOptimization: addNewEdges and addLoopClosure end in setConstraint
-  SVS_CK(h, cudaMemsetAsync(B + lo.o_M, 1, (size_t)std::max(nn, 1), h->stream));
+  SVS_CK(h, cudaMemsetAsync(t.mrg, 1, (size_t)std::max(nn, 1), h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  graph_bind(h, B, lo, nn, pose_graph, pose_graph || nbr_T != nullptr);
+  graph_bind(h, t, nn, pose_graph, pose_graph || nbr_T != nullptr);
   h->wtV = 0;
   return SVS_OK;
 }
@@ -913,66 +884,60 @@ int svs_map_get_graph(svs_map* h, int cap, int* nnzN, int* nbr_ptr, int* nbr_id,
 }  // extern "C"
 
 // ------------------------------------------------------------------ window selection (svs_map_select_window and prepare)
-struct SelWork { size_t o_type, o_ext, o_wtype, o_flag, o_ptrV, o_win, o_pos, o_act, o_ptrP, o_actl, o_q, o_cc, o_cp, o_ci, o_cj, o_cT, o_cL; };
-template <class Take>
-static SelWork sel_take(Take take, int V, int Np, int nn) {
+struct SelWork { int *type, *ext, *wtype, *flag, *ptrV, *win, *pos, *act, *ptrP, *actl, *q, *cc, *cp, *ci, *cj; double *cT, *cL; };
+static SelWork sel_carve(svs::Bump& m, int V, int Np, int nn) {
   SelWork s;
-  s.o_type = take(sizeof(int) * V); s.o_ext = take(sizeof(int) * V); s.o_wtype = take(sizeof(int) * V);
-  s.o_flag = take(sizeof(int) * V); s.o_ptrV = take(sizeof(int) * ((size_t)V + 1)); s.o_win = take(sizeof(int) * V);
-  s.o_pos = take(sizeof(int) * V); s.o_act = take(sizeof(int) * (size_t)std::max(Np, 1));
-  s.o_ptrP = take(sizeof(int) * ((size_t)Np + 1)); s.o_actl = take(sizeof(int) * (size_t)std::max(Np, 1));
-  s.o_q = take(sizeof(int) * ((size_t)nn + 1)); s.o_cc = take(sizeof(int) * V); s.o_cp = take(sizeof(int) * ((size_t)V + 1));
-  s.o_ci = take(sizeof(int) * (size_t)std::max(nn, 1)); s.o_cj = take(sizeof(int) * (size_t)std::max(nn, 1));
-  s.o_cT = take(sizeof(double) * 7 * (size_t)std::max(nn, 1)); s.o_cL = take(sizeof(double) * 36 * (size_t)std::max(nn, 1));
+  s.type = m.take<int>(V); s.ext = m.take<int>(V); s.wtype = m.take<int>(V); s.flag = m.take<int>(V);
+  s.ptrV = m.take<int>((size_t)V + 1); s.win = m.take<int>(V); s.pos = m.take<int>(V); s.act = m.take<int>(Np);
+  s.ptrP = m.take<int>((size_t)Np + 1); s.actl = m.take<int>(Np); s.q = m.take<int>((size_t)nn + 1); s.cc = m.take<int>(V);
+  s.cp = m.take<int>((size_t)V + 1); s.ci = m.take<int>(nn); s.cj = m.take<int>(nn); s.cT = m.take<double>(7 * (size_t)nn);
+  s.cL = m.take<double>(36 * (size_t)nn);
   return s;
 }
 
 // computeInitialDoubleWin + computeActivePointsAndExtendOuterWindow and the pair count of copyContraintsToG2o, enqueued
 // on the map's stream; the counts P, L, C go to counts[0..2] once the stream is synchronised.  The window types (0 / 1
-// INNER / 2 OUTER) are left in W + s.o_wtype.
-static int sel_enqueue(svs_map* h, char* W, const SelWork& s, int root, int inner, int dbl, int* counts) {
+// INNER / 2 OUTER) are left in s.wtype.
+static int sel_enqueue(svs_map* h, const SelWork& s, int root, int inner, int dbl, int* counts) {
   const int V = h->V, Np = h->Np, nn = h->nnzN;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  SVS_CK(h, cudaMemsetAsync(I(s.o_type), 0, sizeof(int) * V, h->stream));
-  SVS_CK(h, cudaMemsetAsync(I(s.o_ext), 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(s.type, 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(s.ext, 0, sizeof(int) * V, h->stream));
   const int bV = (V + 255) / 256, bP = (std::max(Np, 1) + 255) / 256;
-  k_bfs<<<1, 32, 0, h->stream>>>(V, h->g, root, inner, dbl, I(s.o_type), I(s.o_q), nn + 1);
-  if (Np) k_active<<<bP, 256, 0, h->stream>>>(h->m, h->g, I(s.o_type), I(s.o_ext), I(s.o_act));
-  k_window_flags<<<bV, 256, 0, h->stream>>>(V, I(s.o_type), I(s.o_ext), I(s.o_wtype), I(s.o_flag));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_flag), V, I(s.o_ptrV));
-  k_compact<<<bV, 256, 0, h->stream>>>(V, I(s.o_flag), I(s.o_ptrV), I(s.o_win), I(s.o_pos));
+  k_bfs<<<1, 32, 0, h->stream>>>(V, h->g, root, inner, dbl, s.type, s.q, nn + 1);
+  if (Np) k_active<<<bP, 256, 0, h->stream>>>(h->m, h->g, s.type, s.ext, s.act);
+  k_window_flags<<<bV, 256, 0, h->stream>>>(V, s.type, s.ext, s.wtype, s.flag);
+  k_scan<<<1, 1024, 0, h->stream>>>(s.flag, V, s.ptrV);
+  k_compact<<<bV, 256, 0, h->stream>>>(V, s.flag, s.ptrV, s.win, s.pos);
   if (Np) {
-    k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_act), Np, I(s.o_ptrP));
-    k_compact<<<bP, 256, 0, h->stream>>>(Np, I(s.o_act), I(s.o_ptrP), I(s.o_actl), nullptr);
+    k_scan<<<1, 1024, 0, h->stream>>>(s.act, Np, s.ptrP);
+    k_compact<<<bP, 256, 0, h->stream>>>(Np, s.act, s.ptrP, s.actl, nullptr);
   }
-  k_pair_count<<<bV, 256, 0, h->stream>>>(V, h->g, I(s.o_wtype), I(s.o_cc));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(s.o_cc), V, I(s.o_cp));
+  k_pair_count<<<bV, 256, 0, h->stream>>>(V, h->g, s.wtype, s.cc);
+  k_scan<<<1, 1024, 0, h->stream>>>(s.cc, V, s.cp);
   SVS_CK(h, cudaGetLastError());
   counts[1] = 0;
-  SVS_CK(h, cudaMemcpyAsync(counts, I(s.o_ptrV) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  if (Np) SVS_CK(h, cudaMemcpyAsync(counts + 1, I(s.o_ptrP) + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(counts + 2, I(s.o_cp) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts, s.ptrV + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (Np) SVS_CK(h, cudaMemcpyAsync(counts + 1, s.ptrP + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts + 2, s.cp + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   return SVS_OK;
 }
 
 // the window's outputs once the counts fit: the pairs with the graph's constraints as they are now, then the copies
-static int sel_emit(svs_map* h, char* W, const SelWork& s, int P, int L, int C, int* window_vertex, unsigned char* inner,
+static int sel_emit(svs_map* h, const SelWork& s, int P, int L, int C, int* window_vertex, unsigned char* inner,
                     int* active_point, int* c_i, int* c_j, double* c_T, double* c_Lambda) {
   const int V = h->V;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  k_pair_emit<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, I(s.o_wtype), I(s.o_pos), I(s.o_cp), I(s.o_ci), I(s.o_cj),
-                                                      reinterpret_cast<double*>(W + s.o_cT), reinterpret_cast<double*>(W + s.o_cL));
+  k_pair_emit<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, s.wtype, s.pos, s.cp, s.ci, s.cj, s.cT, s.cL);
   SVS_CK(h, cudaGetLastError());
-  SVS_CK(h, cudaMemcpyAsync(window_vertex, I(s.o_win), sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
-  if (L) SVS_CK(h, cudaMemcpyAsync(active_point, I(s.o_actl), sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(window_vertex, s.win, sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, h->stream));
+  if (L) SVS_CK(h, cudaMemcpyAsync(active_point, s.actl, sizeof(int) * (size_t)L, cudaMemcpyDeviceToHost, h->stream));
   h->h_winpos.resize(V);
-  SVS_CK(h, cudaMemcpyAsync(h->h_winpos.data(), I(s.o_wtype), sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(h->h_winpos.data(), s.wtype, sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, h->stream));
   if (c_i && C) {
     if (!c_j || !c_T || !c_Lambda) return SVS_ERR_INVALID;
-    SVS_CK(h, cudaMemcpyAsync(c_i, I(s.o_ci), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_j, I(s.o_cj), sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_T, W + s.o_cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(c_Lambda, W + s.o_cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_i, s.ci, sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_j, s.cj, sizeof(int) * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_T, s.cT, sizeof(double) * 7 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(c_Lambda, s.cL, sizeof(double) * 36 * (size_t)C, cudaMemcpyDeviceToHost, h->stream));
   }
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (inner)
@@ -995,19 +960,20 @@ extern "C" int svs_map_select_window(svs_map* h, int root, int inner_window_size
     return SVS_ERR_INVALID;
   }
   cudaSetDevice(h->device);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const SelWork s = sel_take(take, V, h->Np, h->nnzN);
+  svs::Bump m{nullptr};
+  sel_carve(m, V, h->Np, h->nnzN);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
+  SVS_CK(h, svs::grow(m.off, &h->sel_cap, &h->d_sel));
+  m = svs::Bump{h->d_sel};
+  const SelWork s = sel_carve(m, V, h->Np, h->nnzN);
   int counts[3] = {0, 0, 0};
-  if (int rc = sel_enqueue(h, h->d_sel, s, root, inner_window_size, double_window_size, counts)) return rc;
+  if (int rc = sel_enqueue(h, s, root, inner_window_size, double_window_size, counts)) return rc;
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int P = counts[0], L = counts[1], C = counts[2];
   *P_out = P; *L_out = L;
   if (C_out) *C_out = C;
   if (P > cap_P || L > cap_L || (c_i && C > cap_C)) { h->err = "window, active points or constraints exceed the caller's capacity"; return SVS_ERR_INVALID; }
-  return sel_emit(h, h->d_sel, s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
+  return sel_emit(h, s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
 }
 
 
@@ -1047,50 +1013,63 @@ static int keyframe_grow(svs_map* h, int oldkey, const double* T_newkey_from_old
   cudaSetDevice(h->device);
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int V2 = V + 1, Np2 = Np + n_new, nnz2 = nnz + n_track + 2 * n_new;
-  const MapLayout lo = map_layout(V2, Np2, nnz2);
+  svs::Bump mz{nullptr};
+  map_carve(mz, V2, Np2, nnz2);
+  const size_t cap = mz.off + mz.off / 4;
   char* B2 = nullptr;
-  SVS_CK(h, cudaMalloc(&B2, lo.total + lo.total / 4));
-  // staging: everything the kernels read from the caller, in one pinned-less copy (keyframe rate, a few 10 KB)
-  std::vector<char> st;
-  auto push = [&](const void* src, size_t bytes) { const size_t o = st.size(); st.resize(o + al256(bytes)); if (bytes) memcpy(st.data() + o, src, bytes); return o; };
-  const size_t s_T = push(T_newkey_from_oldkey, sizeof(double) * 7);
-  const size_t s_na = push(new_anchor, sizeof(int) * (size_t)n_new), s_nx = push(new_xyz_anchor, sizeof(double) * 3 * (size_t)n_new);
-  const size_t s_nac = push(new_anchor_center, sizeof(double) * 3 * (size_t)n_new), s_nal = push(new_anchor_level, sizeof(int) * (size_t)n_new);
-  const size_t s_nc = push(new_center, sizeof(double) * 3 * (size_t)n_new), s_nl = push(new_level, sizeof(int) * (size_t)n_new);
-  const size_t s_tp = push(track_point, sizeof(int) * (size_t)n_track), s_tc = push(track_center, sizeof(double) * 3 * (size_t)n_track);
-  const size_t s_tl = push(track_level, sizeof(int) * (size_t)n_track);
-  const size_t s_add = st.size(); st.resize(s_add + al256(sizeof(int) * (size_t)Np2));
-  const size_t s_cnt = st.size(); st.resize(s_cnt + al256(sizeof(int) * (size_t)Np2));
+  SVS_CK(h, cudaMalloc(&B2, cap));
+  svs::Bump mb{B2};
+  const MapTables t = map_carve(mb, V2, Np2, nnz2);
+  // staging: everything the kernels read from the caller, carved alike in a host vector and the device buffer so that
+  // one pinned-less copy (keyframe rate, a few 10 KB) moves the prefix [0, up); add and cnt are the kernels' own
+  struct Stage { double *T, *nx, *nac, *nc, *tc; int *na, *nal, *nl, *tp, *tl, *add, *cnt; size_t up, end; };
+  auto carve = [&](char* base) {
+    svs::Bump m{base};
+    Stage g;
+    g.T = m.take<double>(7); g.na = m.take<int>(n_new); g.nx = m.take<double>(3 * (size_t)n_new);
+    g.nac = m.take<double>(3 * (size_t)n_new); g.nal = m.take<int>(n_new); g.nc = m.take<double>(3 * (size_t)n_new);
+    g.nl = m.take<int>(n_new); g.tp = m.take<int>(n_track); g.tc = m.take<double>(3 * (size_t)n_track);
+    g.tl = m.take<int>(n_track);
+    g.up = m.off;
+    g.add = m.take<int>(Np2); g.cnt = m.take<int>(Np2);
+    g.end = m.off;
+    return g;
+  };
+  std::vector<char> st(carve(nullptr).end);
+  const Stage hs = carve(st.data());
+  auto put = [](void* dst, const void* src, size_t bytes) { if (bytes) memcpy(dst, src, bytes); };
+  put(hs.T, T_newkey_from_oldkey, sizeof(double) * 7);
+  put(hs.na, new_anchor, sizeof(int) * (size_t)n_new); put(hs.nx, new_xyz_anchor, sizeof(double) * 3 * (size_t)n_new);
+  put(hs.nac, new_anchor_center, sizeof(double) * 3 * (size_t)n_new); put(hs.nal, new_anchor_level, sizeof(int) * (size_t)n_new);
+  put(hs.nc, new_center, sizeof(double) * 3 * (size_t)n_new); put(hs.nl, new_level, sizeof(int) * (size_t)n_new);
+  put(hs.tp, track_point, sizeof(int) * (size_t)n_track); put(hs.tc, track_center, sizeof(double) * 3 * (size_t)n_track);
+  put(hs.tl, track_level, sizeof(int) * (size_t)n_track);
   if (svs::grow(st.size(), &h->upd_cap, &h->d_upd) != cudaSuccess) { cudaFree(B2); h->err = "cudaMalloc"; return SVS_ERR_CUDA; }
-  char* U = h->d_upd;
-  cudaError_t e = cudaMemcpyAsync(U, st.data(), s_add, cudaMemcpyHostToDevice, h->stream);
-  auto D = [&](size_t o) { return reinterpret_cast<double*>(U + o); };
-  auto Ii = [&](size_t o) { return reinterpret_cast<int*>(U + o); };
-  if (e == cudaSuccess) e = cudaMemsetAsync(U + s_add, 0xff, sizeof(int) * (size_t)Np2, h->stream);
+  const Stage u = carve(h->d_upd);
+  cudaError_t e = cudaMemcpyAsync(h->d_upd, st.data(), u.up, cudaMemcpyHostToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(u.add, 0xff, sizeof(int) * (size_t)Np2, h->stream);
   // vertices
-  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_pose, h->m.pose, sizeof(double) * 7 * (size_t)V, cudaMemcpyDeviceToDevice, h->stream);
-  k_new_pose<<<1, 32, 0, h->stream>>>(h->m.pose, oldkey, D(s_T), reinterpret_cast<double*>(B2 + lo.o_pose) + 7 * (size_t)V);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t.pose, h->m.pose, sizeof(double) * 7 * (size_t)V, cudaMemcpyDeviceToDevice, h->stream);
+  k_new_pose<<<1, 32, 0, h->stream>>>(h->m.pose, oldkey, u.T, t.pose + 7 * (size_t)V);
   // points
-  if (Np && e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_anch, h->m.anchor, sizeof(int) * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
-  if (Np && e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_xyz, h->m.xyz, sizeof(double) * 3 * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
-  if (n_new && e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_anch + sizeof(int) * (size_t)Np, U + s_na, sizeof(int) * (size_t)n_new, cudaMemcpyDeviceToDevice, h->stream);
-  if (n_new && e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_xyz + sizeof(double) * 3 * (size_t)Np, U + s_nx, sizeof(double) * 3 * (size_t)n_new, cudaMemcpyDeviceToDevice, h->stream);
+  if (Np && e == cudaSuccess) e = cudaMemcpyAsync(t.anchor, h->m.anchor, sizeof(int) * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
+  if (Np && e == cudaSuccess) e = cudaMemcpyAsync(t.xyz, h->m.xyz, sizeof(double) * 3 * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
+  if (n_new && e == cudaSuccess) e = cudaMemcpyAsync(t.anchor + Np, u.na, sizeof(int) * (size_t)n_new, cudaMemcpyDeviceToDevice, h->stream);
+  if (n_new && e == cudaSuccess) e = cudaMemcpyAsync(t.xyz + 3 * (size_t)Np, u.nx, sizeof(double) * 3 * (size_t)n_new, cudaMemcpyDeviceToDevice, h->stream);
   // observations
   if (Np2) {
-    if (n_track) k_mark_tracks<<<(n_track + 255) / 256, 256, 0, h->stream>>>(n_track, Ii(s_tp), Ii(s_add));
-    k_grow_count<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, Ii(s_add), Ii(s_cnt));
-    k_scan<<<1, 1024, 0, h->stream>>>(Ii(s_cnt), Np2, reinterpret_cast<int*>(B2 + lo.o_vptr));
-    k_grow_move<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, Ii(s_add), reinterpret_cast<const int*>(B2 + lo.o_vptr), D(s_tc),
-                                                        Ii(s_tl), Ii(s_na), D(s_nac), Ii(s_nal), D(s_nc), Ii(s_nl),
-                                                        reinterpret_cast<int*>(B2 + lo.o_vpose), reinterpret_cast<double*>(B2 + lo.o_cen),
-                                                        reinterpret_cast<int*>(B2 + lo.o_lvl));
+    if (n_track) k_mark_tracks<<<(n_track + 255) / 256, 256, 0, h->stream>>>(n_track, u.tp, u.add);
+    k_grow_count<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, u.add, u.cnt);
+    k_scan<<<1, 1024, 0, h->stream>>>(u.cnt, Np2, t.vis_ptr);
+    k_grow_move<<<(Np2 + 255) / 256, 256, 0, h->stream>>>(h->m, Np2, V, u.add, t.vis_ptr, u.tc, u.tl, u.na, u.nac, u.nal, u.nc,
+                                                        u.nl, t.vis_pose, t.center, t.level);
   }
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e != cudaSuccess) { cudaFree(B2); h->err = std::string("svs_map_add_keyframe: ") + cudaGetErrorString(e); return SVS_ERR_CUDA; }
   cudaFree(h->d_map);
-  h->d_map = B2; h->map_cap = lo.total + lo.total / 4;
-  map_bind(h, B2, lo, V2, Np2, nnz2);
+  h->d_map = B2; h->map_cap = cap;
+  map_bind(h, t, V2, Np2, nnz2);
   h->d_win_last = nullptr;                 // (a window assembled before the growth can no longer be absorbed)
   return SVS_OK;
 }
@@ -1116,13 +1095,12 @@ extern "C" int svs_map_add_keyframe(svs_map* h, int oldkey, const double* T_newk
 // The feature tables (points in ascending id) of the vertices flagged in `touched`, for computeConstraint.  Clear,
 // flag, count (nfeat and the largest table go to ctl[0], ctl[1]), then -- once the caller has read ctl on the host --
 // build: emit one key (vertex, point) per observation, sort with CUB, unpack into point.
-struct FeatWork { size_t o_touch, o_fcnt, o_fptr, o_fcur, o_ctl, o_fkey, o_fkey2, o_fpt; };
-template <class Take>
-static FeatWork feat_take(Take take, int V, size_t nf) {
+struct FeatWork { int *touch, *fcnt, *fptr, *fcur, *ctl, *fpt; unsigned long long *fkey, *fkey2; };
+static FeatWork feat_carve(svs::Bump& m, int V, size_t nf) {
   FeatWork f;
-  f.o_touch = take(sizeof(int) * V); f.o_fcnt = take(sizeof(int) * V); f.o_fptr = take(sizeof(int) * ((size_t)V + 1));
-  f.o_fcur = take(sizeof(int) * V); f.o_ctl = take(sizeof(int) * 4);
-  f.o_fkey = take(8 * nf); f.o_fkey2 = take(8 * nf); f.o_fpt = take(sizeof(int) * nf);
+  f.touch = m.take<int>(V); f.fcnt = m.take<int>(V); f.fptr = m.take<int>((size_t)V + 1); f.fcur = m.take<int>(V);
+  f.ctl = m.take<int>(4); f.fkey = m.take<unsigned long long>(nf); f.fkey2 = m.take<unsigned long long>(nf);
+  f.fpt = m.take<int>(nf);
   return f;
 }
 static size_t feat_sort_bytes(size_t nf) {
@@ -1130,29 +1108,25 @@ static size_t feat_sort_bytes(size_t nf) {
   cub::DeviceRadixSort::SortKeys(nullptr, b, (unsigned long long*)nullptr, (unsigned long long*)nullptr, (int)nf);
   return b;
 }
-static cudaError_t feat_clear(svs_map* h, char* W, const FeatWork& f) {
+static cudaError_t feat_clear(svs_map* h, const FeatWork& f) {
   cudaError_t e = cudaSuccess;
-  for (size_t o : {f.o_touch, f.o_fcnt, f.o_fcur})
-    if (e == cudaSuccess) e = cudaMemsetAsync(W + o, 0, sizeof(int) * h->V, h->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(W + f.o_ctl, 0, sizeof(int) * 4, h->stream);
+  for (int* p : {f.touch, f.fcnt, f.fcur})
+    if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, sizeof(int) * h->V, h->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(f.ctl, 0, sizeof(int) * 4, h->stream);
   return e;
 }
-static cudaError_t feat_count(svs_map* h, char* W, const FeatWork& f) {
+static cudaError_t feat_count(svs_map* h, const FeatWork& f) {
   const int V = h->V, Np = h->Np;
-  int* touched = reinterpret_cast<int*>(W + f.o_touch); int* fcnt = reinterpret_cast<int*>(W + f.o_fcnt);
-  int* fptr = reinterpret_cast<int*>(W + f.o_fptr); int* ctl = reinterpret_cast<int*>(W + f.o_ctl);
-  if (Np) k_feat_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, touched, fcnt);
-  k_scan<<<1, 1024, 0, h->stream>>>(fcnt, V, fptr);
-  k_max<<<(V + 255) / 256, 256, 0, h->stream>>>(V, fcnt, ctl + 1);
-  return cudaMemcpyAsync(ctl, fptr + V, sizeof(int), cudaMemcpyDeviceToDevice, h->stream);
+  if (Np) k_feat_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, f.touch, f.fcnt);
+  k_scan<<<1, 1024, 0, h->stream>>>(f.fcnt, V, f.fptr);
+  k_max<<<(V + 255) / 256, 256, 0, h->stream>>>(V, f.fcnt, f.ctl + 1);
+  return cudaMemcpyAsync(f.ctl, f.fptr + V, sizeof(int), cudaMemcpyDeviceToDevice, h->stream);
 }
-static cudaError_t feat_build(svs_map* h, char* W, const FeatWork& f, int nfeat, void* tmp, size_t tmp_bytes) {
+static cudaError_t feat_build(svs_map* h, const FeatWork& f, int nfeat, void* tmp, size_t tmp_bytes) {
   if (!nfeat) return cudaSuccess;
-  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
-  k_feat_emit<<<(h->Np + 255) / 256, 256, 0, h->stream>>>(h->m, reinterpret_cast<int*>(W + f.o_touch), reinterpret_cast<int*>(W + f.o_fptr),
-                                                          reinterpret_cast<int*>(W + f.o_fcur), U(f.o_fkey));
-  cudaError_t e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, U(f.o_fkey), U(f.o_fkey2), nfeat, 0, 64, h->stream);
-  k_feat_unpack<<<(nfeat + 255) / 256, 256, 0, h->stream>>>(nfeat, U(f.o_fkey2), reinterpret_cast<int*>(W + f.o_fpt));
+  k_feat_emit<<<(h->Np + 255) / 256, 256, 0, h->stream>>>(h->m, f.touch, f.fptr, f.fcur, f.fkey);
+  cudaError_t e = cub::DeviceRadixSort::SortKeys(tmp, tmp_bytes, f.fkey, f.fkey2, nfeat, 0, 64, h->stream);
+  k_feat_unpack<<<(nfeat + 255) / 256, 256, 0, h->stream>>>(nfeat, f.fkey2, f.fpt);
   return e;
 }
 
@@ -1167,58 +1141,58 @@ static int grow_graph(svs_map* h, int gV, int n, const int* d_v1, const int* d_v
   size_t tmp_bytes = feat_sort_bytes(nf), b = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int*)nullptr, (int)ni);
   tmp_bytes = std::max(tmp_bytes, b);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const FeatWork f = feat_take(take, V, nf);
-  const size_t o_T12 = take(sizeof(double) * 7 * ni), o_Lam = take(sizeof(double) * 36 * ni), o_cs = take(sizeof(int) * ni);
-  const size_t o_icnt = take(sizeof(int) * V), o_iptr = take(sizeof(int) * ((size_t)V + 1)), o_ncnt = take(sizeof(int) * V);
-  const size_t o_tgt = take(sizeof(int) * ni), o_tgt2 = take(sizeof(int) * ni), o_seq = take(sizeof(int) * ni);
-  const size_t o_seq2 = take(sizeof(int) * ni), o_tmp = take(tmp_bytes);
+  FeatWork f;
+  struct { double *T12, *Lam; int *cs, *icnt, *iptr, *ncnt, *tgt, *tgt2, *seq, *seq2; char* tmp; } w;
+  auto carve = [&](svs::Bump m) {
+    f = feat_carve(m, V, nf);
+    w.T12 = m.take<double>(7 * ni); w.Lam = m.take<double>(36 * ni); w.cs = m.take<int>(ni);
+    w.icnt = m.take<int>(V); w.iptr = m.take<int>((size_t)V + 1); w.ncnt = m.take<int>(V);
+    w.tgt = m.take<int>(ni); w.tgt2 = m.take<int>(ni); w.seq = m.take<int>(ni); w.seq2 = m.take<int>(ni);
+    w.tmp = m.take<char>(tmp_bytes);
+    return m.off;
+  };
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->ge_cap, &h->d_ge));
-  const GraphLayout lo = graph_layout(V, nn);
-  SVS_CK(h, svs::grow(lo.total, &h->graph2_cap, &h->d_graph2));
-  char* W = h->d_ge;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  auto D = [&](size_t o) { return reinterpret_cast<double*>(W + o); };
+  SVS_CK(h, svs::grow(carve(svs::Bump{nullptr}), &h->ge_cap, &h->d_ge));
+  carve(svs::Bump{h->d_ge});
+  svs::Bump m{nullptr};
+  graph_carve(m, V, nn);
+  SVS_CK(h, svs::grow(m.off, &h->graph2_cap, &h->d_graph2));
+  m = svs::Bump{h->d_graph2};
+  const GraphTables t = graph_carve(m, V, nn);
   const int bV = (V + 255) / 256;
-  SVS_CK(h, feat_clear(h, W, f));
-  SVS_CK(h, cudaMemsetAsync(W + o_icnt, 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, feat_clear(h, f));
+  SVS_CK(h, cudaMemsetAsync(w.icnt, 0, sizeof(int) * V, h->stream));
   if (n) {
-    k_touch<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(f.o_touch));
-    SVS_CK(h, feat_count(h, W, f));
+    k_touch<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, f.touch);
+    SVS_CK(h, feat_count(h, f));
     int ctl[2] = {0, 0};
-    SVS_CK(h, cudaMemcpyAsync(ctl, I(f.o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(ctl, f.ctl, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
     SVS_CK(h, cudaStreamSynchronize(h->stream));
     const int nfeat = ctl[0], stride = svs::constraint_scratch_stride(ctl[1]);
-    SVS_CK(h, feat_build(h, W, f, nfeat, W + o_tmp, tmp_bytes));
+    SVS_CK(h, feat_build(h, f, nfeat, w.tmp, tmp_bytes));
     if (stride) {
       SVS_CK(h, cudaStreamSynchronize(h->stream));
       SVS_CK(h, svs::grow(sizeof(double) * (size_t)stride * n, &h->cs_cap, &h->d_cs));
     }
-    svs::launch_compute_constraint(d_poses, I(f.o_fptr), I(f.o_fpt), h->m.anchor, h->m.xyz, n, d_v1, d_v2, D(o_T12), D(o_Lam), I(o_cs),
+    svs::launch_compute_constraint(d_poses, f.fptr, f.fpt, h->m.anchor, h->m.xyz, n, d_v1, d_v2, w.T12, w.Lam, w.cs,
                                    reinterpret_cast<double*>(h->d_cs), stride, h->stream);
-    k_ins_keys<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, I(o_tgt), I(o_seq), I(o_icnt));
+    k_ins_keys<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(n, d_v1, d_v2, w.tgt, w.seq, w.icnt);
     size_t tb = tmp_bytes;   // a stable sort: inside one target the inserts stay in sequence order
-    SVS_CK(h, cub::DeviceRadixSort::SortPairs(W + o_tmp, tb, I(o_tgt), I(o_tgt2), I(o_seq), I(o_seq2), 2 * n, 0, 32, h->stream));
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.tgt, w.tgt2, w.seq, w.seq2, 2 * n, 0, 32, h->stream));
   }
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_icnt), V, I(o_iptr));
-  char* B = h->d_graph2;
-  k_ins_count<<<bV, 256, 0, h->stream>>>(V, gV, h->g.nbr_ptr, I(o_icnt), I(o_ncnt));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_ncnt), V, reinterpret_cast<int*>(B + lo.o_ptr));
+  k_scan<<<1, 1024, 0, h->stream>>>(w.icnt, V, w.iptr);
+  k_ins_count<<<bV, 256, 0, h->stream>>>(V, gV, h->g.nbr_ptr, w.icnt, w.ncnt);
+  k_scan<<<1, 1024, 0, h->stream>>>(w.ncnt, V, t.ptr);
   InsArgs a;
-  a.n = n; a.gV = gV; a.nn_old = nn_old; a.g = h->g; a.iptr = I(o_iptr); a.iseq = I(o_seq2);
-  a.v1 = d_v1; a.v2 = d_v2; a.es = d_es; a.T12 = D(o_T12); a.Lam = D(o_Lam);
-  a.nptr = reinterpret_cast<const int*>(B + lo.o_ptr);
-  a.id = reinterpret_cast<int*>(B + lo.o_id); a.str = reinterpret_cast<int*>(B + lo.o_str);
-  a.T = reinterpret_cast<double*>(B + lo.o_T); a.L = reinterpret_cast<double*>(B + lo.o_L);
-  a.mrg = reinterpret_cast<unsigned char*>(B + lo.o_M);
+  a.n = n; a.gV = gV; a.nn_old = nn_old; a.g = h->g; a.iptr = w.iptr; a.iseq = w.seq2;
+  a.v1 = d_v1; a.v2 = d_v2; a.es = d_es; a.T12 = w.T12; a.Lam = w.Lam;
+  a.nptr = t.ptr; a.id = t.id; a.str = t.str; a.T = t.T; a.L = t.Lam; a.mrg = t.mrg;
   if (nn_old) k_ins_move_old<<<(nn_old + 255) / 256, 256, 0, h->stream>>>(a);
   if (n) k_ins_move_new<<<(2 * n + 255) / 256, 256, 0, h->stream>>>(a, V);
   SVS_CK(h, cudaGetLastError());
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   std::swap(h->d_graph, h->d_graph2); std::swap(h->graph_cap, h->graph2_cap);
-  graph_bind(h, h->d_graph, lo, nn, true, true);
+  graph_bind(h, t, nn, true, true);
   return SVS_OK;
 }
 
@@ -1248,66 +1222,69 @@ extern "C" int svs_map_add_keyframe_graph(svs_map* h, int oldkey, const double* 
   size_t tmp_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, (unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                   (unsigned char*)nullptr, (unsigned char*)nullptr, (int)nr);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_tp = take(sizeof(int) * n_track), o_tc = take(sizeof(double) * 3 * n_track), o_na = take(sizeof(int) * n_new);
-  const size_t o_tcnt = take(sizeof(int) * n_track), o_tptr = take(sizeof(int) * ((size_t)n_track + 1));
-  const size_t o_vcnt = take(sizeof(int) * V), o_vptr = take(sizeof(int) * ((size_t)V + 1)), o_new = take(sizeof(int) * V);
-  const size_t o_str = take(sizeof(int) * V), o_in = take(sizeof(int) * V), o_rptr = take(sizeof(int) * ((size_t)V + 1));
-  const size_t o_qual = take(sizeof(int) * V), o_eptr = take(sizeof(int) * ((size_t)V + 1)), o_rows = take(sizeof(int) * 2 * V);
-  const size_t o_v1 = take(sizeof(int) * V), o_v2 = take(sizeof(int) * V), o_es = take(sizeof(int) * V);
-  const size_t o_key = take(8 * nr), o_key2 = take(8 * nr), o_q = take(nr), o_q2 = take(nr), o_tmp = take(tmp_bytes);
+  struct {
+    int *tp, *na, *tcnt, *tptr, *vcnt, *vptr, *nw, *str, *in, *rptr, *qual, *eptr, *rows, *v1, *v2, *es;
+    double* tc; unsigned long long *key, *key2; unsigned char *q, *q2; char* tmp;
+  } w;
+  auto carve = [&](svs::Bump m) {
+    w.tp = m.take<int>(n_track); w.tc = m.take<double>(3 * (size_t)n_track); w.na = m.take<int>(n_new);
+    w.tcnt = m.take<int>(n_track); w.tptr = m.take<int>((size_t)n_track + 1);
+    w.vcnt = m.take<int>(V); w.vptr = m.take<int>((size_t)V + 1); w.nw = m.take<int>(V);
+    w.str = m.take<int>(V); w.in = m.take<int>(V); w.rptr = m.take<int>((size_t)V + 1);
+    w.qual = m.take<int>(V); w.eptr = m.take<int>((size_t)V + 1); w.rows = m.take<int>(2 * (size_t)V);
+    w.v1 = m.take<int>(V); w.v2 = m.take<int>(V); w.es = m.take<int>(V);
+    w.key = m.take<unsigned long long>(nr); w.key2 = m.take<unsigned long long>(nr);
+    w.q = m.take<unsigned char>(nr); w.q2 = m.take<unsigned char>(nr); w.tmp = m.take<char>(tmp_bytes);
+    return m.off;
+  };
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->gw_cap, &h->d_gw));
-  char* W = h->d_gw;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  auto U = [&](size_t o) { return reinterpret_cast<unsigned long long*>(W + o); };
-  auto Q = [&](size_t o) { return reinterpret_cast<unsigned char*>(W + o); };
+  SVS_CK(h, svs::grow(carve(svs::Bump{nullptr}), &h->gw_cap, &h->d_gw));
+  carve(svs::Bump{h->d_gw});
   if (n_track) {
-    SVS_CK(h, cudaMemcpyAsync(W + o_tp, track_point, sizeof(int) * n_track, cudaMemcpyHostToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(W + o_tc, track_center, sizeof(double) * 3 * n_track, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.tp, track_point, sizeof(int) * n_track, cudaMemcpyHostToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(w.tc, track_center, sizeof(double) * 3 * n_track, cudaMemcpyHostToDevice, h->stream));
   }
-  if (n_new) SVS_CK(h, cudaMemcpyAsync(W + o_na, new_anchor, sizeof(int) * n_new, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemsetAsync(W + o_vcnt, 0, sizeof(int) * V, h->stream));
-  SVS_CK(h, cudaMemsetAsync(W + o_new, 0, sizeof(int) * V, h->stream));
+  if (n_new) SVS_CK(h, cudaMemcpyAsync(w.na, new_anchor, sizeof(int) * n_new, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(w.vcnt, 0, sizeof(int) * V, h->stream));
+  SVS_CK(h, cudaMemsetAsync(w.nw, 0, sizeof(int) * V, h->stream));
   // computeStrength on the map before the growth
   int R = 0;
   if (n_track) {
-    k_str_count<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, I(o_tp), I(o_tcnt));
-    k_scan<<<1, 1024, 0, h->stream>>>(I(o_tcnt), n_track, I(o_tptr));
-    SVS_CK(h, cudaMemcpyAsync(&R, I(o_tptr) + n_track, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    k_str_count<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, w.tp, w.tcnt);
+    k_scan<<<1, 1024, 0, h->stream>>>(w.tcnt, n_track, w.tptr);
+    SVS_CK(h, cudaMemcpyAsync(&R, w.tptr + n_track, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     SVS_CK(h, cudaStreamSynchronize(h->stream));
   }
   if (R) {
     const int half_w = (int)(width * 0.5), half_h = (int)(height * 0.5);   // int half_width = cam_.width()*0.5 (:480-481)
-    k_str_emit<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, I(o_tp), reinterpret_cast<const double*>(W + o_tc),
-                                                             (double)half_w, (double)half_h, I(o_tptr), U(o_key), Q(o_q), I(o_vcnt));
+    k_str_emit<<<(n_track + 255) / 256, 256, 0, h->stream>>>(h->m, n_track, w.tp, w.tc, (double)half_w, (double)half_h, w.tptr,
+                                                             w.key, w.q, w.vcnt);
     size_t tb = tmp_bytes;
-    SVS_CK(h, cub::DeviceRadixSort::SortPairs(W + o_tmp, tb, U(o_key), U(o_key2), Q(o_q), Q(o_q2), R, 0, 64, h->stream));
+    SVS_CK(h, cub::DeviceRadixSort::SortPairs(w.tmp, tb, w.key, w.key2, w.q, w.q2, R, 0, 64, h->stream));
   }
-  if (n_new) k_str_new<<<(n_new + 255) / 256, 256, 0, h->stream>>>(n_new, I(o_na), I(o_new));
+  if (n_new) k_str_new<<<(n_new + 255) / 256, 256, 0, h->stream>>>(n_new, w.na, w.nw);
   const int bV = (V + 255) / 256;
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_vcnt), V, I(o_vptr));
-  k_str_closed<<<(int)((32 * (size_t)V + 255) / 256), 256, 0, h->stream>>>(V, n_track, std::max(1, covis_thr / 2), I(o_vptr), Q(o_q2),
-                                                                          I(o_new), I(o_str), I(o_in));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_in), V, I(o_rptr));
-  k_str_table<<<bV, 256, 0, h->stream>>>(V, oldkey, covis_thr, I(o_in), I(o_rptr), I(o_str), I(o_qual), I(o_rows));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(o_qual), V, I(o_eptr));
-  k_str_edges<<<bV, 256, 0, h->stream>>>(V, V, I(o_qual), I(o_eptr), I(o_str), I(o_v1), I(o_v2), I(o_es));
+  k_scan<<<1, 1024, 0, h->stream>>>(w.vcnt, V, w.vptr);
+  k_str_closed<<<(int)((32 * (size_t)V + 255) / 256), 256, 0, h->stream>>>(V, n_track, std::max(1, covis_thr / 2), w.vptr, w.q2,
+                                                                          w.nw, w.str, w.in);
+  k_scan<<<1, 1024, 0, h->stream>>>(w.in, V, w.rptr);
+  k_str_table<<<bV, 256, 0, h->stream>>>(V, oldkey, covis_thr, w.in, w.rptr, w.str, w.qual, w.rows);
+  k_scan<<<1, 1024, 0, h->stream>>>(w.qual, V, w.eptr);
+  k_str_edges<<<bV, 256, 0, h->stream>>>(V, V, w.qual, w.eptr, w.str, w.v1, w.v2, w.es);
   SVS_CK(h, cudaGetLastError());
   int rows = 0, ne = 0, old_in = 0;
-  SVS_CK(h, cudaMemcpyAsync(&rows, I(o_rptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(&ne, I(o_eptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(&old_in, I(o_in) + oldkey, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&rows, w.rptr + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&ne, w.eptr + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&old_in, w.in + oldkey, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (!old_in) { h->err = "oldkey is absent from the strength table (slam_graph.cpp:165 asserts)"; return SVS_ERR_INVALID; }
-  if (table && rows) SVS_CK(h, cudaMemcpyAsync(table, I(o_rows), sizeof(int) * 2 * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
+  if (table && rows) SVS_CK(h, cudaMemcpyAsync(table, w.rows, sizeof(int) * 2 * (size_t)rows, cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   // addNewPointsToMap + addNewObsToOldPoints, then addNewEdges(LOCAL) on the grown map
   if ((rc = keyframe_grow(h, oldkey, T_newkey_from_oldkey, n_new, new_anchor, new_xyz_anchor, new_anchor_center, new_anchor_level,
                           new_center, new_level, n_track, track_point, track_center, track_level)) != SVS_OK)
     return rc;
-  if ((rc = grow_graph(h, V, ne, I(o_v1), I(o_v2), I(o_es), h->m.pose)) != SVS_OK) {
+  if ((rc = grow_graph(h, V, ne, w.v1, w.v2, w.es, h->m.pose)) != SVS_OK) {
     h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // the map has V + 1 vertices now: a graph of V lists must not stay behind
     return rc;
   }
@@ -1340,73 +1317,67 @@ extern "C" int svs_map_add_edges(svs_map* h, int n, const int* v1, const int* v2
   if (std::adjacent_find(pairs.begin(), pairs.end()) != pairs.end()) { h->err = "an edge is listed twice"; return SVS_ERR_INVALID; }
   if (n == 0) return SVS_OK;
   cudaSetDevice(h->device);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_v1 = take(sizeof(int) * n), o_v2 = take(sizeof(int) * n), o_es = take(sizeof(int) * n), o_bad = take(sizeof(int));
-  const size_t o_pose = take(sizeof(double) * 7 * V);
+  int *d_v1 = nullptr, *d_v2 = nullptr, *d_es = nullptr, *d_bad = nullptr; double* d_pose = nullptr;
+  auto carve = [&](svs::Bump m) {
+    d_v1 = m.take<int>(n); d_v2 = m.take<int>(n); d_es = m.take<int>(n); d_bad = m.take<int>(1); d_pose = m.take<double>(7 * (size_t)V);
+    return m.off;
+  };
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->gw_cap, &h->d_gw));
-  char* W = h->d_gw;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  SVS_CK(h, cudaMemcpyAsync(W + o_v1, v1, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(W + o_v2, v2, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(W + o_es, strength, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-  SVS_CK(h, cudaMemsetAsync(W + o_bad, 0, sizeof(int), h->stream));
-  k_edge_exists<<<(n + 255) / 256, 256, 0, h->stream>>>(h->g, V, n, I(o_v1), I(o_v2), I(o_bad));
+  SVS_CK(h, svs::grow(carve(svs::Bump{nullptr}), &h->gw_cap, &h->d_gw));
+  carve(svs::Bump{h->d_gw});
+  SVS_CK(h, cudaMemcpyAsync(d_v1, v1, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d_v2, v2, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(d_es, strength, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(d_bad, 0, sizeof(int), h->stream));
+  k_edge_exists<<<(n + 255) / 256, 256, 0, h->stream>>>(h->g, V, n, d_v1, d_v2, d_bad);
   SVS_CK(h, cudaGetLastError());
   int bad = 0;
-  SVS_CK(h, cudaMemcpyAsync(&bad, W + o_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   if (bad) { h->err = "an edge is already in the pose graph (insertEdge asserts, slam_graph.hpp:353)"; return SVS_ERR_INVALID; }
   // registerKeyframes / addLoopClosure place the moved vertex at its new pose while the constraints are computed
   const double* poses = h->m.pose;
   if (moved_vertex >= 0) {
-    double* P = reinterpret_cast<double*>(W + o_pose);
-    SVS_CK(h, cudaMemcpyAsync(P, h->m.pose, sizeof(double) * 7 * V, cudaMemcpyDeviceToDevice, h->stream));
-    SVS_CK(h, cudaMemcpyAsync(P + 7 * (size_t)moved_vertex, T_moved_from_w, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
-    poses = P;
+    SVS_CK(h, cudaMemcpyAsync(d_pose, h->m.pose, sizeof(double) * 7 * V, cudaMemcpyDeviceToDevice, h->stream));
+    SVS_CK(h, cudaMemcpyAsync(d_pose + 7 * (size_t)moved_vertex, T_moved_from_w, sizeof(double) * 7, cudaMemcpyHostToDevice, h->stream));
+    poses = d_pose;
   }
-  return grow_graph(h, V, n, I(o_v1), I(o_v2), I(o_es), poses);
+  return grow_graph(h, V, n, d_v1, d_v2, d_es, poses);
 }
 
 // ------------------------------------------------------------------ prepareForOptimization
-struct PrepWork { SelWork s; FeatWork f; size_t o_old, o_seen, o_q, o_mcnt, o_mptr, o_v1, o_v2, o_T12, o_Lam, o_cs, o_tmp; };
+struct PrepWork {
+  SelWork s; FeatWork f;
+  int *old, *seen, *mcnt, *mptr, *v1, *v2, *cs; ReinitNode* q; double *T12, *Lam; char* tmp;
+};
 
 // steps 2, 4 and 5 once the counts have fitted: from here on the map changes
 static int prepare_apply(svs_map* h, const PrepWork& w, int root, int loop, int P, int nM, int nfeat, int max_feat) {
   const int V = h->V, nn = h->nnzN;
-  char* W = h->d_sel;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  auto D = [&](size_t o) { return reinterpret_cast<double*>(W + o); };
-  const int* new_t = I(w.s.o_wtype);
+  const int* new_t = w.s.wtype;
   h->d_win_last = nullptr;   // absorbing the previous window would overwrite the reinitialised poses
-  SVS_CK(h, cudaMemsetAsync(I(w.o_seen), 0, sizeof(int) * V, h->stream));
-  k_reinit<<<1, 32, 0, h->stream>>>(h->g, root, loop, new_t, I(w.o_old), const_cast<double*>(h->m.pose), I(w.o_seen),
-                                    reinterpret_cast<ReinitNode*>(W + w.o_q), nn + 1);
+  SVS_CK(h, cudaMemsetAsync(w.seen, 0, sizeof(int) * V, h->stream));
+  k_reinit<<<1, 32, 0, h->stream>>>(h->g, root, loop, new_t, w.old, h->t.pose, w.seen, w.q, nn + 1);
   SVS_CK(h, cudaGetLastError());
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   SVS_CK(h, svs::grow(sizeof(int) * (size_t)V, &h->wt_cap, &h->d_wt));
   SVS_CK(h, cudaMemcpyAsync(h->d_wt, new_t, sizeof(int) * (size_t)V, cudaMemcpyDeviceToDevice, h->stream));
   h->wtV = V;
   if (P >= 2) {
-    const GraphLayout lo = graph_layout(V, nn);
-    unsigned char* mrg = reinterpret_cast<unsigned char*>(h->d_graph + lo.o_M);
     const int bV = (V + 255) / 256;
-    k_unmarg<<<bV, 256, 0, h->stream>>>(V, h->g, new_t, mrg);
+    k_unmarg<<<bV, 256, 0, h->stream>>>(V, h->g, new_t, h->gt.mrg);
     if (nM) {
-      k_marg_emit<<<bV, 256, 0, h->stream>>>(V, h->g, I(w.o_old), new_t, I(w.o_mptr), I(w.o_v1), I(w.o_v2));
-      SVS_CK(h, feat_build(h, W, w.f, nfeat, W + w.o_tmp, feat_sort_bytes((size_t)std::max(h->nnz, 1))));
+      k_marg_emit<<<bV, 256, 0, h->stream>>>(V, h->g, w.old, new_t, w.mptr, w.v1, w.v2);
+      SVS_CK(h, feat_build(h, w.f, nfeat, w.tmp, feat_sort_bytes((size_t)std::max(h->nnz, 1))));
       const int stride = svs::constraint_scratch_stride(max_feat);
       if (stride) {
         SVS_CK(h, cudaStreamSynchronize(h->stream));
         SVS_CK(h, svs::grow(sizeof(double) * (size_t)stride * nM, &h->cs_cap, &h->d_cs));
       }
       // computeConstraint(v1 = max, v2 = min) at the reinitialised poses
-      svs::launch_compute_constraint(h->m.pose, I(w.f.o_fptr), I(w.f.o_fpt), h->m.anchor, h->m.xyz, nM, I(w.o_v1), I(w.o_v2),
-                                     D(w.o_T12), D(w.o_Lam), I(w.o_cs), reinterpret_cast<double*>(h->d_cs), stride, h->stream);
-      k_marg_store<<<(nM + 255) / 256, 256, 0, h->stream>>>(nM, h->g, I(w.o_v1), I(w.o_v2), D(w.o_T12), D(w.o_Lam),
-                                                            reinterpret_cast<double*>(h->d_graph + lo.o_T),
-                                                            reinterpret_cast<double*>(h->d_graph + lo.o_L), mrg);
+      svs::launch_compute_constraint(h->m.pose, w.f.fptr, w.f.fpt, h->m.anchor, h->m.xyz, nM, w.v1, w.v2, w.T12, w.Lam, w.cs,
+                                     reinterpret_cast<double*>(h->d_cs), stride, h->stream);
+      k_marg_store<<<(nM + 255) / 256, 256, 0, h->stream>>>(nM, h->g, w.v1, w.v2, w.T12, w.Lam, h->gt.T, h->gt.Lam, h->gt.mrg);
     }
   }
   SVS_CK(h, cudaGetLastError());
@@ -1429,33 +1400,32 @@ extern "C" int svs_map_prepare_for_optimization(svs_map* h, int root, int loop, 
     return SVS_ERR_INVALID;
   }
   cudaSetDevice(h->device);
-  const size_t nf = (size_t)std::max(h->nnz, 1), ne = (size_t)std::max(nn, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
+  const size_t nf = (size_t)std::max(h->nnz, 1);
   PrepWork w;
-  w.s = sel_take(take, V, h->Np, nn);
-  w.f = feat_take(take, V, nf);
-  w.o_old = take(sizeof(int) * V); w.o_seen = take(sizeof(int) * V); w.o_q = take(sizeof(ReinitNode) * ((size_t)nn + 1));
-  w.o_mcnt = take(sizeof(int) * V); w.o_mptr = take(sizeof(int) * ((size_t)V + 1));
-  w.o_v1 = take(sizeof(int) * ne); w.o_v2 = take(sizeof(int) * ne);
-  w.o_T12 = take(sizeof(double) * 7 * ne); w.o_Lam = take(sizeof(double) * 36 * ne); w.o_cs = take(sizeof(int) * ne);
-  w.o_tmp = take(feat_sort_bytes(nf));
+  auto carve = [&](svs::Bump m) {
+    w.s = sel_carve(m, V, h->Np, nn);
+    w.f = feat_carve(m, V, nf);
+    w.old = m.take<int>(V); w.seen = m.take<int>(V); w.q = m.take<ReinitNode>((size_t)nn + 1);
+    w.mcnt = m.take<int>(V); w.mptr = m.take<int>((size_t)V + 1); w.v1 = m.take<int>(nn); w.v2 = m.take<int>(nn);
+    w.T12 = m.take<double>(7 * (size_t)nn); w.Lam = m.take<double>(36 * (size_t)nn); w.cs = m.take<int>(nn);
+    w.tmp = m.take<char>(feat_sort_bytes(nf));
+    return m.off;
+  };
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(off, &h->sel_cap, &h->d_sel));
-  char* W = h->d_sel;
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
+  SVS_CK(h, svs::grow(carve(svs::Bump{nullptr}), &h->sel_cap, &h->d_sel));
+  carve(svs::Bump{h->d_sel});
   // every count the call needs, before anything changes: window, active points, pairs, marginalised edges, features
-  SVS_CK(h, cudaMemsetAsync(I(w.o_old), 0, sizeof(int) * V, h->stream));   // vertices from wtV on are outside the old window
-  if (h->wtV) SVS_CK(h, cudaMemcpyAsync(I(w.o_old), h->d_wt, sizeof(int) * (size_t)h->wtV, cudaMemcpyDeviceToDevice, h->stream));
+  SVS_CK(h, cudaMemsetAsync(w.old, 0, sizeof(int) * V, h->stream));   // vertices from wtV on are outside the old window
+  if (h->wtV) SVS_CK(h, cudaMemcpyAsync(w.old, h->d_wt, sizeof(int) * (size_t)h->wtV, cudaMemcpyDeviceToDevice, h->stream));
   int counts[6] = {0, 0, 0, 0, 0, 0};
-  if ((rc = sel_enqueue(h, W, w.s, root, inner_window_size, double_window_size, counts)) != SVS_OK) return rc;
-  SVS_CK(h, feat_clear(h, W, w.f));
-  k_marg_count<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, I(w.o_old), I(w.s.o_wtype), I(w.o_mcnt), I(w.f.o_touch));
-  k_scan<<<1, 1024, 0, h->stream>>>(I(w.o_mcnt), V, I(w.o_mptr));
-  SVS_CK(h, feat_count(h, W, w.f));
+  if ((rc = sel_enqueue(h, w.s, root, inner_window_size, double_window_size, counts)) != SVS_OK) return rc;
+  SVS_CK(h, feat_clear(h, w.f));
+  k_marg_count<<<(V + 255) / 256, 256, 0, h->stream>>>(V, h->g, w.old, w.s.wtype, w.mcnt, w.f.touch);
+  k_scan<<<1, 1024, 0, h->stream>>>(w.mcnt, V, w.mptr);
+  SVS_CK(h, feat_count(h, w.f));
   SVS_CK(h, cudaGetLastError());
-  SVS_CK(h, cudaMemcpyAsync(counts + 3, I(w.o_mptr) + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  SVS_CK(h, cudaMemcpyAsync(counts + 4, I(w.f.o_ctl), sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts + 3, w.mptr + V, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  SVS_CK(h, cudaMemcpyAsync(counts + 4, w.f.ctl, sizeof(int) * 2, cudaMemcpyDeviceToHost, h->stream));
   SVS_CK(h, cudaStreamSynchronize(h->stream));
   const int P = counts[0], L = counts[1], C = counts[2];
   *P_out = P; *L_out = L;
@@ -1466,7 +1436,7 @@ extern "C" int svs_map_prepare_for_optimization(svs_map* h, int root, int loop, 
     h->g = GraphDev{}; h->nnzN = 0; h->wtV = 0;   // a graph half marginalised must not stay behind
     return rc;
   }
-  return sel_emit(h, W, w.s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
+  return sel_emit(h, w.s, P, L, C, window_vertex, inner, active_point, c_i, c_j, c_T, c_Lambda);
 }
 
 extern "C" int svs_map_get_window_state(svs_map* h, int cap, int* nnzN, unsigned char* window_type, unsigned char* marginalized) {
@@ -1522,37 +1492,39 @@ int svs::map_add_observations(svs_map* h, int vertex, int n, const int* d_point,
   const int V = h->V, Np = h->Np, nnz = h->nnz;
   if (n == 0 || Np == 0) return SVS_OK;
   cudaSetDevice(h->device);
-  // the new tables are sized for n more observations; nnz becomes what the scan counted (a point the vertex already
-  // observes gains none)
-  const MapLayout lo = map_layout(V, Np, nnz + n);
-  const size_t s_add = 0, s_cnt = al256(sizeof(int) * (size_t)Np), need = 2 * s_cnt;
+  // the new tables are sized for n more observations (the handle keeps their pointers: nothing lays them out again);
+  // nnz becomes what the scan counted (a point the vertex already observes gains none)
+  int *add = nullptr, *cnt = nullptr;
+  auto carve = [&](svs::Bump m) { add = m.take<int>(Np); cnt = m.take<int>(Np); return m.off; };
   SVS_CK(h, cudaStreamSynchronize(h->stream));
-  SVS_CK(h, svs::grow(need, &h->upd_cap, &h->d_upd));
+  SVS_CK(h, svs::grow(carve(svs::Bump{nullptr}), &h->upd_cap, &h->d_upd));
+  carve(svs::Bump{h->d_upd});
+  svs::Bump mz{nullptr};
+  map_carve(mz, V, Np, nnz + n);
+  const size_t cap = mz.off + mz.off / 4;
   char* B2 = nullptr;
-  SVS_CK(h, cudaMalloc(&B2, lo.total + lo.total / 4));
-  int* add = reinterpret_cast<int*>(h->d_upd + s_add);
-  int* cnt = reinterpret_cast<int*>(h->d_upd + s_cnt);
+  SVS_CK(h, cudaMalloc(&B2, cap));
+  svs::Bump mb{B2};
+  const MapTables t = map_carve(mb, V, Np, nnz + n);
   int nnz2 = 0;
   cudaError_t e = cudaMemsetAsync(add, 0xff, sizeof(int) * (size_t)Np, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_pose, h->m.pose, sizeof(double) * 7 * (size_t)V, cudaMemcpyDeviceToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_anch, h->m.anchor, sizeof(int) * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(B2 + lo.o_xyz, h->m.xyz, sizeof(double) * 3 * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
-  int* vptr2 = reinterpret_cast<int*>(B2 + lo.o_vptr);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t.pose, h->m.pose, sizeof(double) * 7 * (size_t)V, cudaMemcpyDeviceToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t.anchor, h->m.anchor, sizeof(int) * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t.xyz, h->m.xyz, sizeof(double) * 3 * (size_t)Np, cudaMemcpyDeviceToDevice, h->stream);
   if (e == cudaSuccess) {
     k_mark_tracks<<<(n + 255) / 256, 256, 0, h->stream>>>(n, d_point, add);
     k_grow_count<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, Np, vertex, add, cnt);
-    k_scan<<<1, 1024, 0, h->stream>>>(cnt, Np, vptr2);
-    k_grow_move<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, Np, vertex, add, vptr2, d_center, d_level, nullptr, nullptr,
-                                                        nullptr, nullptr, nullptr, reinterpret_cast<int*>(B2 + lo.o_vpose),
-                                                        reinterpret_cast<double*>(B2 + lo.o_cen), reinterpret_cast<int*>(B2 + lo.o_lvl));
+    k_scan<<<1, 1024, 0, h->stream>>>(cnt, Np, t.vis_ptr);
+    k_grow_move<<<(Np + 255) / 256, 256, 0, h->stream>>>(h->m, Np, vertex, add, t.vis_ptr, d_center, d_level, nullptr, nullptr,
+                                                        nullptr, nullptr, nullptr, t.vis_pose, t.center, t.level);
     e = cudaGetLastError();
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&nnz2, vptr2 + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&nnz2, t.vis_ptr + Np, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e != cudaSuccess) { cudaFree(B2); h->err = std::string("map_add_observations: ") + cudaGetErrorString(e); return SVS_ERR_CUDA; }
   cudaFree(h->d_map);
-  h->d_map = B2; h->map_cap = lo.total + lo.total / 4;
-  map_bind(h, B2, lo, V, Np, nnz2);
+  h->d_map = B2; h->map_cap = cap;
+  map_bind(h, t, V, Np, nnz2);
   h->d_win_last = nullptr;   // the window's observations changed; the pose graph (V vertices) stays
   return SVS_OK;
 }

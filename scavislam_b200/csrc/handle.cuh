@@ -1,8 +1,9 @@
 // handle.cuh -- the host plumbing every opaque handle of the C ABI shares: its device, stream and error text, the CUDA
-// check, opening and closing the handle on its device, and the "grow a buffer" helper
+// check, opening and closing the handle on its device, the "grow a buffer" helper and the layout of a buffer
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstddef>
 #include <string>
 
@@ -83,5 +84,17 @@ cudaError_t grow(size_t n, size_t* cap, T** dev, T** pinned = nullptr) {
   if (e == cudaSuccess) *cap = want;
   return e;
 }
+
+// Lays a module's arrays out in one buffer, each 256-byte aligned, in take order; n = 0 still gets a slot.  A pass
+// with base == nullptr only sizes (every take returns nullptr): off is then the bytes the buffer needs.  The idiom is
+// a sizing pass, grow to `off`, then the same takes on the buffer.  `off` is also the mark of where the next take lies.
+struct Bump {
+  char* base; size_t off = 0;
+  template <typename T> T* take(size_t n) {
+    T* p = base ? reinterpret_cast<T*>(base + off) : nullptr;
+    off += ((std::max<size_t>(n, 1) * sizeof(T) + 255) / 256) * 256;
+    return p;
+  }
+};
 
 }  // namespace svs

@@ -337,12 +337,47 @@ __global__ void k_reg_commit_emit(int nt, const int* __restrict__ flag, const in
 
 // ------------------------------------------------------------------ host steps shared by both entry points
 
-size_t al256(size_t x) { return (x + 255) / 256 * 256; }
-
 struct CandBufs {
   int *flag, *qptr, *qpts, *cflag, *cptr, *cpt;   // [Np], [Np+1], [Np], [Np], [Np+1], [Np]
   svs_match_point *rec, *pts;                     // [Np], [Np]
 };
+
+// the per-call buffers of both entry points (Nq = max(Np, 1)): the control block, the window's flags, the vertices'
+// slots, the candidate scan, the matcher's slot poses saved for a refusal, and the gated tracks
+struct LoopBufs {
+  LoopCtl* ctl; int *win, *slot; CandBufs cb; double* save;
+  int* tp; double* tu; int* tl;   // [Nq], [Nq][3], [Nq]
+};
+LoopBufs loop_carve(svs::Bump& m, int V, int Nq, int max_kf) {
+  LoopBufs b;
+  b.ctl = m.take<LoopCtl>(1); b.win = m.take<int>(V); b.slot = m.take<int>(V);
+  b.cb.flag = m.take<int>(Nq); b.cb.qptr = m.take<int>(Nq + 1); b.cb.qpts = m.take<int>(Nq);
+  b.cb.cflag = m.take<int>(Nq); b.cb.cptr = m.take<int>(Nq + 1);
+  b.cb.rec = m.take<svs_match_point>(Nq); b.cb.pts = m.take<svs_match_point>(Nq); b.cb.cpt = m.take<int>(Nq);
+  b.save = m.take<double>(7 * (size_t)max_kf);
+  b.tp = m.take<int>(Nq); b.tu = m.take<double>(3 * (size_t)Nq); b.tl = m.take<int>(Nq);
+  return b;
+}
+
+// what svs_localRegisterFrame takes after loop_carve; dir .. cnt are zeroed together (zero_bytes from dir on)
+struct RegBufs {
+  int *dir, *join, *scan, *anch, *cnt;   // [V] x 4, [5][V]
+  size_t zero_bytes;
+  int *sflag, *sptr, *qual, *queue, *keep, *gptr, *mflag, *mptr, *mp, *ml; double* mu; svs_register_stats* stats;
+};
+RegBufs reg_carve(svs::Bump& m, int V, int Nq, int nnzN) {
+  RegBufs r;
+  const size_t z = m.off;
+  r.dir = m.take<int>(V); r.join = m.take<int>(V); r.scan = m.take<int>(V); r.anch = m.take<int>(V);
+  r.cnt = m.take<int>(5 * (size_t)V);
+  r.zero_bytes = m.off - z;
+  r.sflag = m.take<int>(V); r.sptr = m.take<int>(V + 1); r.qual = m.take<int>(V);
+  r.stats = m.take<svs_register_stats>(V); r.queue = m.take<int>((size_t)nnzN + 1);
+  r.keep = m.take<int>(Nq); r.gptr = m.take<int>(Nq + 1);
+  r.mflag = m.take<int>(Nq); r.mptr = m.take<int>(Nq + 1);
+  r.mp = m.take<int>(Nq); r.mu = m.take<double>(3 * (size_t)Nq); r.ml = m.take<int>(Nq);
+  return r;
+}
 
 // the candidate scan: the points some vertex of vset[V] observes, in ascending index, then those anchored in the window
 // whose (int) projection from T_ref_from_w (device memory) lies in the anchor level's image (k_cand_test).  Waits for
@@ -478,15 +513,9 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
   cudaSetDevice(m.device);
   cudaStream_t st = m.stream;
   const int Nq = std::max(Np, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_ctl = take(sizeof(LoopCtl)), o_win = take(sizeof(int) * V), o_slot = take(sizeof(int) * V);
-  const size_t o_qset = take(sizeof(int) * V);
-  const size_t o_flag = take(sizeof(int) * Nq), o_qptr = take(sizeof(int) * (Nq + 1)), o_qpts = take(sizeof(int) * Nq);
-  const size_t o_cflag = take(sizeof(int) * Nq), o_cptr = take(sizeof(int) * (Nq + 1));
-  const size_t o_rec = take(sizeof(svs_match_point) * Nq), o_pts = take(sizeof(svs_match_point) * Nq);
-  const size_t o_cpt = take(sizeof(int) * Nq), o_save = take(sizeof(double) * 7 * mv.max_kf);
-  const size_t o_tp = take(sizeof(int) * Nq), o_tu = take(sizeof(double) * 3 * Nq), o_tl = take(sizeof(int) * Nq);
+  svs::Bump m0{nullptr};
+  loop_carve(m0, V, Nq, mv.max_kf);
+  m0.take<int>(V);   // qset
   char* W = nullptr;
   std::string cerr;
   int rc = SVS_OK;
@@ -494,31 +523,29 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
   LoopCtl c{};
   Pose7 Tql;
   memcpy(Tql.v, T_query_from_loop, sizeof Tql.v);
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  LoopCtl* d_ctl = reinterpret_cast<LoopCtl*>(W + o_ctl);
-  svs_match_point* d_pts = nullptr;
+  LoopBufs b{};
+  int* d_qset = nullptr;
   {
     LCK(cudaStreamSynchronize(st));
-    LCK(cudaMalloc(&W, off));
-    d_ctl = reinterpret_cast<LoopCtl*>(W + o_ctl);
-    d_pts = reinterpret_cast<svs_match_point*>(W + o_pts);
-    LCK(cudaMemsetAsync(d_ctl, 0, sizeof(LoopCtl), st));
-    LCK(cudaMemcpyAsync(I(o_win), inwin.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
-    LCK(cudaMemcpyAsync(I(o_slot), vertex_slot, sizeof(int) * V, cudaMemcpyHostToDevice, st));
-    LCK(cudaMemcpyAsync(I(o_qset), qset.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
+    LCK(cudaMalloc(&W, m0.off));
+    svs::Bump mw{W};
+    b = loop_carve(mw, V, Nq, mv.max_kf);
+    d_qset = mw.take<int>(V);
+    LCK(cudaMemsetAsync(b.ctl, 0, sizeof(LoopCtl), st));
+    LCK(cudaMemcpyAsync(b.win, inwin.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
+    LCK(cudaMemcpyAsync(b.slot, vertex_slot, sizeof(int) * V, cudaMemcpyHostToDevice, st));
+    LCK(cudaMemcpyAsync(d_qset, qset.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
     // 1 candidates
-    k_loop_setup<<<1, 32, 0, st>>>(m.pose, query, Tql, d_ctl);
-    const CandBufs cb{I(o_flag), I(o_qptr), I(o_qpts), I(o_cflag), I(o_cptr), I(o_cpt),
-                      reinterpret_cast<svs_match_point*>(W + o_rec), d_pts};
+    k_loop_setup<<<1, 32, 0, st>>>(m.pose, query, Tql, b.ctl);
     int nc = 0;
-    LCK(scan_candidates(m, I(o_qset), I(o_win), I(o_slot), matcher_levels(mv), d_ctl->T_loop_from_w, d_ctl, cb, st, &nc));
+    LCK(scan_candidates(m, d_qset, b.win, b.slot, matcher_levels(mv), b.ctl->T_loop_from_w, b.ctl, b.cb, st, &nc));
     LCK(cudaGetLastError());
-    LCK(cudaMemcpyAsync(&c, d_ctl, sizeof c, cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&c, b.ctl, sizeof c, cudaMemcpyDeviceToHost, st));
     LCK(cudaStreamSynchronize(st));
     res->n_candidates = nc;
     if (const char* why = candidate_refusal(c, nc, mv, max_obs)) { cerr = why; rc = SVS_ERR_INVALID; goto done; }
-    launch_slot_copy(mv, reinterpret_cast<double*>(W + o_save), 0, st);
-    k_slot_refresh<<<(7 * V + 255) / 256, 256, 0, st>>>(V, m.pose, I(o_slot), loop, d_ctl->T_loop_from_w, mv.slot_T, mv.slot_stride);
+    launch_slot_copy(mv, b.save, 0, st);
+    k_slot_refresh<<<(7 * V + 255) / 256, 256, 0, st>>>(V, m.pose, b.slot, loop, b.ctl->T_loop_from_w, mv.slot_T, mv.slot_stride);
     LCK(cudaGetLastError());
     LCK(cudaStreamSynchronize(st));   // the matcher's stream reads the slots and the candidates
     refreshed = true;
@@ -526,7 +553,7 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
     const svs_match_result* d_res = nullptr;
     double T[7];
     int nm[2] = {0, 0}, first_short = 0;
-    rc = match_and_align(mt, po, cam, c.T_loop_from_w, d_pts, nc, covis_thr, d_ctl, st, nm, res->T_align1, T, res->lm, &d_res,
+    rc = match_and_align(mt, po, cam, c.T_loop_from_w, b.cb.pts, nc, covis_thr, b.ctl, st, nm, res->T_align1, T, res->lm, &d_res,
                          &first_short, &cerr);
     res->n_matched1 = nm[0];
     if (rc != SVS_OK) goto done;
@@ -538,19 +565,19 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
     Pose7 Tn;
     memcpy(Tn.v, T, sizeof T);
     const Cam4 c4{cam->f, cam->px, cam->py, cam->b};
-    k_gate<<<1, kGate, 0, st>>>(d_res, d_pts, I(o_cpt), nc, Tn, Tql, c4, mv.lv[0].w, mv.lv[0].h, m.pose, query, d_ctl, I(o_tp),
-                                reinterpret_cast<double*>(W + o_tu), I(o_tl));
+    k_gate<<<1, kGate, 0, st>>>(d_res, b.cb.pts, b.cb.cpt, nc, Tn, Tql, c4, mv.lv[0].w, mv.lv[0].h, m.pose, query, b.ctl, b.tp,
+                                b.tu, b.tl);
     LCK(cudaGetLastError());
-    LCK(cudaMemcpyAsync(&c, d_ctl, sizeof c, cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&c, b.ctl, sizeof c, cudaMemcpyDeviceToHost, st));
     LCK(cudaStreamSynchronize(st));
     const int nt = c.n_tracks;
     res->n_tracks = nt;
     res->num_left = c.num_left; res->num_right = c.num_right; res->num_upper = c.num_upper; res->num_lower = c.num_lower;
     if (nt > cap) { cerr = "cap is smaller than the number of tracks"; rc = SVS_ERR_INVALID; goto done; }
     if (nt) {
-      LCK(cudaMemcpyAsync(track_point, I(o_tp), sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_uvu, W + o_tu, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_level, I(o_tl), sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_point, b.tp, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_uvu, b.tu, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_level, b.tl, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
       LCK(cudaStreamSynchronize(st));
     }
     const int half = covis_thr / 2;
@@ -558,14 +585,14 @@ extern "C" int svs_globalLoopClosure(svs_map* map, svs_matcher* mt, svs_pose* po
     if (c.num_lower < half || c.num_upper < half || c.num_left < half || c.num_right < half) { res->stage = 4; goto done; }
     // 4 commit
     memcpy(res->T_newloop_from_w, c.T_newloop_from_w, sizeof c.T_newloop_from_w);
-    rc = svs::map_add_observations(map, loop, nt, I(o_tp), reinterpret_cast<const double*>(W + o_tu), I(o_tl));
+    rc = svs::map_add_observations(map, loop, nt, b.tp, b.tu, b.tl);
     if (rc != SVS_OK) { cerr = svs_map_last_error(map); goto done; }
     res->verified = 1;
     res->stage = 0;
   }
 done:
   if (rc != SVS_OK && refreshed && rc != SVS_ERR_NUMERIC) {   // a refusal leaves the slots as they were
-    launch_slot_copy(mv, reinterpret_cast<double*>(W + o_save), 1, st);
+    launch_slot_copy(mv, b.save, 1, st);
     cudaStreamSynchronize(st);
   }
   if (W) { cudaStreamSynchronize(st); cudaFree(W); }
@@ -605,49 +632,34 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
   cudaSetDevice(m.device);
   cudaStream_t st = m.stream;
   const int Nq = std::max(Np, 1);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += al256(bytes); return o; };
-  const size_t o_ctl = take(sizeof(LoopCtl)), o_win = take(sizeof(int) * V), o_slot = take(sizeof(int) * V);
-  // zeroed together: direct, joined, scan, anch, cnt
-  const size_t o_dir = take(sizeof(int) * V), o_join = take(sizeof(int) * V), o_scan = take(sizeof(int) * V);
-  const size_t o_anch = take(sizeof(int) * V), o_cnt = take(sizeof(int) * 5 * (size_t)V), o_zero_end = off;
-  const size_t o_sflag = take(sizeof(int) * V), o_sptr = take(sizeof(int) * (V + 1)), o_qual = take(sizeof(int) * V);
-  const size_t o_stats = take(sizeof(svs_register_stats) * V), o_queue = take(sizeof(int) * ((size_t)nnzN + 1));
-  const size_t o_flag = take(sizeof(int) * Nq), o_qptr = take(sizeof(int) * (Nq + 1)), o_qpts = take(sizeof(int) * Nq);
-  const size_t o_cflag = take(sizeof(int) * Nq), o_cptr = take(sizeof(int) * (Nq + 1));
-  const size_t o_rec = take(sizeof(svs_match_point) * Nq), o_pts = take(sizeof(svs_match_point) * Nq);
-  const size_t o_cpt = take(sizeof(int) * Nq), o_save = take(sizeof(double) * 7 * mv.max_kf);
-  const size_t o_keep = take(sizeof(int) * Nq), o_gptr = take(sizeof(int) * (Nq + 1));
-  const size_t o_tp = take(sizeof(int) * Nq), o_tu = take(sizeof(double) * 3 * Nq), o_tl = take(sizeof(int) * Nq);
-  const size_t o_mflag = take(sizeof(int) * Nq), o_mptr = take(sizeof(int) * (Nq + 1));
-  const size_t o_mp = take(sizeof(int) * Nq), o_mu = take(sizeof(double) * 3 * Nq), o_ml = take(sizeof(int) * Nq);
+  svs::Bump m0{nullptr};
+  loop_carve(m0, V, Nq, mv.max_kf);
+  reg_carve(m0, V, Nq, nnzN);
   char* W = nullptr;
   std::string cerr;
   int rc = SVS_OK;
   bool refreshed = false;
   LoopCtl c{};
-  auto I = [&](size_t o) { return reinterpret_cast<int*>(W + o); };
-  LoopCtl* d_ctl = nullptr;
-  svs_match_point* d_pts = nullptr;
+  LoopBufs b{};
+  RegBufs r{};
   {
     LCK(cudaStreamSynchronize(st));
-    LCK(cudaMalloc(&W, off));
-    d_ctl = reinterpret_cast<LoopCtl*>(W + o_ctl);
-    d_pts = reinterpret_cast<svs_match_point*>(W + o_pts);
-    LCK(cudaMemsetAsync(d_ctl, 0, sizeof(LoopCtl), st));
-    LCK(cudaMemsetAsync(W + o_dir, 0, o_zero_end - o_dir, st));
-    LCK(cudaMemcpyAsync(I(o_win), inwin.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
-    LCK(cudaMemcpyAsync(I(o_slot), vertex_slot, sizeof(int) * V, cudaMemcpyHostToDevice, st));
+    LCK(cudaMalloc(&W, m0.off));
+    svs::Bump mw{W};
+    b = loop_carve(mw, V, Nq, mv.max_kf);
+    r = reg_carve(mw, V, Nq, nnzN);
+    LCK(cudaMemsetAsync(b.ctl, 0, sizeof(LoopCtl), st));
+    LCK(cudaMemsetAsync(r.dir, 0, r.zero_bytes, st));
+    LCK(cudaMemcpyAsync(b.win, inwin.data(), sizeof(int) * V, cudaMemcpyHostToDevice, st));
+    LCK(cudaMemcpyAsync(b.slot, vertex_slot, sizeof(int) * V, cudaMemcpyHostToDevice, st));
     // 1 neighbourhoods and candidates (pointsVisibleInRoot, backend.cpp:472-546)
-    k_neighborhood<<<1, 32, 0, st>>>(nbr_ptr, nbr_id, root, I(o_win), I(o_dir), I(o_join), I(o_scan), I(o_queue), d_ctl);
+    k_neighborhood<<<1, 32, 0, st>>>(nbr_ptr, nbr_id, root, b.win, r.dir, r.join, r.scan, r.queue, b.ctl);
     const double* d_Troot = m.pose + 7 * (size_t)root;
-    const CandBufs cb{I(o_flag), I(o_qptr), I(o_qpts), I(o_cflag), I(o_cptr), I(o_cpt),
-                      reinterpret_cast<svs_match_point*>(W + o_rec), d_pts};
     int nc = 0;
-    LCK(scan_candidates(m, I(o_scan), I(o_win), I(o_slot), matcher_levels(mv), d_Troot, d_ctl, cb, st, &nc));
-    if (nc) k_anchor_flag<<<(nc + 255) / 256, 256, 0, st>>>(nc, m.anchor, I(o_cpt), I(o_anch));
+    LCK(scan_candidates(m, r.scan, b.win, b.slot, matcher_levels(mv), d_Troot, b.ctl, b.cb, st, &nc));
+    if (nc) k_anchor_flag<<<(nc + 255) / 256, 256, 0, st>>>(nc, m.anchor, b.cb.cpt, r.anch);
     LCK(cudaGetLastError());
-    LCK(cudaMemcpyAsync(&c, d_ctl, sizeof c, cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&c, b.ctl, sizeof c, cudaMemcpyDeviceToHost, st));
     double Troot[7];
     LCK(cudaMemcpyAsync(Troot, d_Troot, sizeof Troot, cudaMemcpyDeviceToHost, st));
     LCK(cudaStreamSynchronize(st));
@@ -656,8 +668,8 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
     res->n_candidates = nc;
     if (const char* why = candidate_refusal(c, nc, mv, max_obs)) { cerr = why; rc = SVS_ERR_INVALID; goto done; }
     if (nc < covis_thr) { res->stage = 1; goto done; }
-    launch_slot_copy(mv, reinterpret_cast<double*>(W + o_save), 0, st);
-    k_slot_refresh<<<(7 * V + 255) / 256, 256, 0, st>>>(V, m.pose, I(o_slot), -1, nullptr, mv.slot_T, mv.slot_stride);
+    launch_slot_copy(mv, b.save, 0, st);
+    k_slot_refresh<<<(7 * V + 255) / 256, 256, 0, st>>>(V, m.pose, b.slot, -1, nullptr, mv.slot_T, mv.slot_stride);
     LCK(cudaGetLastError());
     LCK(cudaStreamSynchronize(st));   // the matcher's stream reads the slots and the candidates
     refreshed = true;
@@ -665,7 +677,7 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
     const svs_match_result* d_res = nullptr;
     double T[7];
     int nm[2] = {0, 0}, first_short = 0;
-    rc = match_and_align(mt, po, cam, Troot, d_pts, nc, covis_thr, d_ctl, st, nm, res->T_align1, T, res->lm, &d_res,
+    rc = match_and_align(mt, po, cam, Troot, b.cb.pts, nc, covis_thr, b.ctl, st, nm, res->T_align1, T, res->lm, &d_res,
                          &first_short, &cerr);
     res->n_matched1 = nm[0];
     if (rc != SVS_OK) goto done;
@@ -678,18 +690,18 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
     memcpy(Tn.v, T, sizeof T);
     const Cam4 c4{cam->f, cam->px, cam->py, cam->b};
     const int bc = (nc + 255) / 256, bV = (V + 255) / 256;
-    k_reg_gate<<<bc, 256, 0, st>>>(d_res, d_pts, nc, Tn, c4, I(o_keep));
-    svs::launch_scan(I(o_keep), nc, I(o_gptr), st);
-    k_reg_count<<<bc, 256, 0, st>>>(m, d_res, d_pts, I(o_cpt), nc, I(o_keep), I(o_gptr), I(o_anch), I(o_dir), mv.lv[0].w,
-                                     mv.lv[0].h, I(o_cnt), I(o_tp), reinterpret_cast<double*>(W + o_tu), I(o_tl));
-    k_reg_qualify<<<bV, 256, 0, st>>>(V, I(o_cnt), covis_thr, Tn, m.pose, root, I(o_sflag), I(o_qual), d_ctl);
-    svs::launch_scan(I(o_sflag), V, I(o_sptr), st);
-    k_reg_stats<<<bV, 256, 0, st>>>(V, I(o_cnt), I(o_sflag), I(o_sptr), I(o_qual), reinterpret_cast<svs_register_stats*>(W + o_stats));
+    k_reg_gate<<<bc, 256, 0, st>>>(d_res, b.cb.pts, nc, Tn, c4, r.keep);
+    svs::launch_scan(r.keep, nc, r.gptr, st);
+    k_reg_count<<<bc, 256, 0, st>>>(m, d_res, b.cb.pts, b.cb.cpt, nc, r.keep, r.gptr, r.anch, r.dir, mv.lv[0].w,
+                                     mv.lv[0].h, r.cnt, b.tp, b.tu, b.tl);
+    k_reg_qualify<<<bV, 256, 0, st>>>(V, r.cnt, covis_thr, Tn, m.pose, root, r.sflag, r.qual, b.ctl);
+    svs::launch_scan(r.sflag, V, r.sptr, st);
+    k_reg_stats<<<bV, 256, 0, st>>>(V, r.cnt, r.sflag, r.sptr, r.qual, r.stats);
     LCK(cudaGetLastError());
     int nt = 0, ns = 0;
-    LCK(cudaMemcpyAsync(&nt, I(o_gptr) + nc, sizeof(int), cudaMemcpyDeviceToHost, st));
-    LCK(cudaMemcpyAsync(&ns, I(o_sptr) + V, sizeof(int), cudaMemcpyDeviceToHost, st));
-    LCK(cudaMemcpyAsync(&c, d_ctl, sizeof c, cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&nt, r.gptr + nc, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&ns, r.sptr + V, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LCK(cudaMemcpyAsync(&c, b.ctl, sizeof c, cudaMemcpyDeviceToHost, st));
     LCK(cudaStreamSynchronize(st));
     res->n_tracks = nt;
     res->n_stats = ns;
@@ -698,31 +710,31 @@ extern "C" int svs_localRegisterFrame(svs_map* map, svs_matcher* mt, svs_pose* p
     int ncommit = 0;
     if (nt) {
       const int bt = (nt + 255) / 256;
-      k_reg_commit_flag<<<bt, 256, 0, st>>>(m, nt, I(o_tp), I(o_qual), I(o_mflag));
-      svs::launch_scan(I(o_mflag), nt, I(o_mptr), st);
-      k_reg_commit_emit<<<bt, 256, 0, st>>>(nt, I(o_mflag), I(o_mptr), I(o_tp), reinterpret_cast<const double*>(W + o_tu), I(o_tl),
-                                            I(o_mp), reinterpret_cast<double*>(W + o_mu), I(o_ml));
+      k_reg_commit_flag<<<bt, 256, 0, st>>>(m, nt, b.tp, r.qual, r.mflag);
+      svs::launch_scan(r.mflag, nt, r.mptr, st);
+      k_reg_commit_emit<<<bt, 256, 0, st>>>(nt, r.mflag, r.mptr, b.tp, b.tu, b.tl,
+                                            r.mp, r.mu, r.ml);
       LCK(cudaGetLastError());
-      LCK(cudaMemcpyAsync(&ncommit, I(o_mptr) + nt, sizeof(int), cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_point, I(o_tp), sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_uvu, W + o_tu, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_level, I(o_tl), sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
-      LCK(cudaMemcpyAsync(track_committed, I(o_mflag), sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(&ncommit, r.mptr + nt, sizeof(int), cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_point, b.tp, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_uvu, b.tu, sizeof(double) * 3 * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_level, b.tl, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
+      LCK(cudaMemcpyAsync(track_committed, r.mflag, sizeof(int) * nt, cudaMemcpyDeviceToHost, st));
     }
-    if (ns) LCK(cudaMemcpyAsync(stats, W + o_stats, sizeof(svs_register_stats) * ns, cudaMemcpyDeviceToHost, st));
+    if (ns) LCK(cudaMemcpyAsync(stats, r.stats, sizeof(svs_register_stats) * ns, cudaMemcpyDeviceToHost, st));
     LCK(cudaStreamSynchronize(st));
     if (c.n_neighbors == 0) { res->stage = 4; goto done; }
     // 4 commit (registerKeyframes' addNewObsToOldPoints, slam_graph.cpp:189-205); root's pose stays
     res->n_committed = ncommit;
     memcpy(res->T_newroot_from_w, c.T_newroot_from_w, sizeof c.T_newroot_from_w);
-    rc = svs::map_add_observations(map, root, ncommit, I(o_mp), reinterpret_cast<const double*>(W + o_mu), I(o_ml));
+    rc = svs::map_add_observations(map, root, ncommit, r.mp, r.mu, r.ml);
     if (rc != SVS_OK) { cerr = svs_map_last_error(map); goto done; }
     res->registered = 1;
     res->stage = 0;
   }
 done:
   if (rc != SVS_OK && refreshed && rc != SVS_ERR_NUMERIC) {   // a refusal leaves the slots as they were
-    launch_slot_copy(mv, reinterpret_cast<double*>(W + o_save), 1, st);
+    launch_slot_copy(mv, b.save, 1, st);
     cudaStreamSynchronize(st);
   }
   if (W) { cudaStreamSynchronize(st); cudaFree(W); }
